@@ -171,7 +171,46 @@ def hbm_peak():
         with open(os.path.join(REPO, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "data sheet (H100 SXM HBM3, not measured)"
+
+
+DUMP_LIMIT = 64 << 20  # bytes of .npy data --dump-outputs writes at most
+
+
+def _hash52(s):
+    """a string column as a float64 that holds it exactly enough to compare (52 bits of its md5; NaN for '*')"""
+    return float("nan") if s in (b"*", b"") else float(int(hashlib.md5(s).hexdigest()[:13], 16))
+
+
+def dump_outputs(out_dir, gaf, names):
+    """The GAF text of the last timed step as one float64 array per column (DIR/<column>.npy): the numeric fields as they are,
+    '*' as NaN, strand as +1/-1, path and CIGAR as 52-bit hashes.  Lines are in read order; a fixed, seeded sample of them is
+    kept when all would exceed DUMP_LIMIT."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    rid = {n: i for i, n in enumerate(names)}
+    cols = ["read", "qlen", "qs", "qe", "strand", "path", "plen", "ps", "pe", "mlen", "blen", "mapq", "tp", "cm", "s1", "s2", "dv", "cg"]
+    tags = {b"tp": 12, b"cm": 13, b"s1": 14, b"s2": 15, b"dv": 16, b"cg": 17}
+    lines = [ln for ln in gaf.split(b"\n") if ln]
+    n_keep = min(len(lines), DUMP_LIMIT // (8 * len(cols)))
+    keep = range(len(lines)) if n_keep == len(lines) else sorted(np.random.default_rng(12345).choice(len(lines), n_keep, replace=False))
+    out = np.full((len(keep), len(cols)), np.nan)
+    for r, i in enumerate(keep):
+        t = lines[i].split(b"\t")
+        row = out[r]
+        row[0] = rid.get(t[0], -1)
+        for c in (1, 2, 3, 6, 7, 8, 9, 10, 11):
+            if t[c] != b"*":
+                row[c] = float(t[c])
+        row[4] = {b"+": 1.0, b"-": -1.0}.get(t[4], float("nan"))
+        row[5] = _hash52(t[5])
+        for tag in t[12:]:
+            k, typ, v = tag[:2], tag[3:4], tag[5:]
+            if k in tags:
+                row[tags[k]] = {b"P": 1.0, b"S": 0.0}.get(v, float("nan")) if k == b"tp" else _hash52(v) if typ == b"Z" else float(v)
+    for j, c in enumerate(cols):
+        np.save(os.path.join(out_dir, c + ".npy"), np.ascontiguousarray(out[:, j]))
+    return len(lines), len(keep)
 
 
 def mini_batches(lens, max_bases):
@@ -201,6 +240,7 @@ def main():
     ap.add_argument("--pipe", type=int, default=3, help="host threads calling mg_map_batch() at once")
     ap.add_argument("--no-cpu", action="store_true", help="skip the reference run on the host cores (no cpu_baseline, no parity check): profiling runs")
     ap.add_argument("--check", default="all", help="'all': after the timed region the GAF text of every read of rank 0 is compared with the reference binary's, byte for byte; N: the first N reads; 0: skip")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what rank 0's last step computed (its GAF records, column by column) as DIR/<column>.npy")
     a = ap.parse_args()
     # stdout carries exactly one JSON line: everything libraries print to fd 1 (NCCL's version banner, ...) goes to stderr instead
     sys.stdout.flush()
@@ -434,6 +474,11 @@ def main():
             dist.destroy_process_group()
         return
 
+    dumped = None
+    if a.dump_outputs:
+        n_lines, n_kept = dump_outputs(a.dump_outputs, b"".join(C.string_at(gaf_buf[k], gaf_len[k].value) for k in range(M)), [cnames[i] for i in range(n)])
+        dumped = {"dir": a.dump_outputs, "gaf_lines": n_lines, "lines_written": n_kept}
+
     # ---- untimed: the reference on the host cores, once: CPU baseline and, from its output, the parity check ----
     check, cpu = None, None
     n_chk = 0 if a.no_cpu or a.check == "0" else (n if a.check == "all" else min(n, int(a.check)))
@@ -499,7 +544,7 @@ def main():
                      "algorithmic_bytes_per_launch": chain_bytes / n_launch_chain, "launch_ms": t_chain / n_launch_chain * 1e3, "launches_timed": n_launch_chain,
                      "peak_source": peak_src,
                      "bytes_model": "16 B x %d seeds in + 16 B x %d anchors out + 8 B x %d chains over %d launches" % (acc["seeds"], acc["anchors"], acc["chains"], n_launch_chain)},
-        "cpu_baseline": cpu, "parity_check": check,
+        "cpu_baseline": cpu, "parity_check": check, "dump_outputs": dumped,
         "clocks": sampler.summary(),
     }
     if dry:

@@ -1,4 +1,4 @@
-/* mgb200.h -- C ABI of libmgb200.so, the B200-native replacement of minigraph's seed-chain-align hot path.
+/* mgb200.h -- C ABI of libmgb200.so, the GPU-native (H100) replacement of minigraph's seed-chain-align hot path.
  *
  * The library is a drop-in for the mapping entry points of the reference: it keeps the symbol names, argument
  * meaning and ownership rules of minigraph.h so that the unmodified C host (main.c, gfa-*.c, bseq.c, format.c,
@@ -6,7 +6,7 @@
  * headers they cite; they are restated here (not included) so that the library builds without the reference tree.
  * If the reference headers are included first (MINIGRAPH_H / __GFA_H__ defined), the restated types are skipped.
  *
- * Every entry point needs a CUDA device (sm_100a); there is no CPU fallback: without a device mg_index() returns
+ * Every entry point needs a CUDA device (an H100, sm_90a); there is no CPU fallback: without a device mg_index() returns
  * NULL after printing an error, and mgb_last_error() tells why.
  */
 #ifndef MGB200_H

@@ -1,4 +1,4 @@
-// mgb_common.cuh -- shared device-side building blocks of the B200 mapping engine.
+// mgb_common.cuh -- shared device-side building blocks of the mapping engine.
 //
 // Everything in csrc/*.cuh is written once as warp-cooperative device code.  The functions are
 // marked MG_HD so that the *same* source can also be compiled by g++ into tests/hostsim (a

@@ -1,6 +1,6 @@
 // mgb_engine.cu -- host side of libmgb200.so: model construction, batch dispatcher and the C ABI (include/mgb200.h).
 //
-// Compiled by nvcc for sm_100a into the product library.  With -DMGB_HOSTSIM the same file is compiled by g++ into
+// Compiled by nvcc for sm_90a (H100) into the product library.  With -DMGB_HOSTSIM the same file is compiled by g++ into
 // tests/hostsim/libmgb_hostsim.so, where "device memory" is host memory and a "launch" is a loop over reads with a
 // single lane: that build exists only so that the CPU-only unit tests can exercise the control flow of the kernels.
 // It is never loaded by the product path; the product library refuses to work without a CUDA device.
@@ -36,7 +36,10 @@ using namespace mgb;
 static std::string g_last_error;
 static void set_error(const std::string &s) { g_last_error = s; fprintf(stderr, "[E::mgb200] %s\n", s.c_str()); }
 
-static int64_t p_arena_mb = 6;        // per worker, first pass
+// Per worker, first pass.  The slots' arenas take slots x SMs x workers_per_sm x arena_mb of HBM (3 x 132 x 32 x 3 MB = 37 GiB on an
+// H100), which leaves the rest of its 80 GB to the output pools and the large-arena retry pass; a read needs far less than 3 MB
+// (1.5 MB at most on the bench workloads), and one that needs more is redone with a large arena.
+static int64_t p_arena_mb = 3;
 static int64_t p_arena_big_mb = 1024; // per worker, retry pass
 static int64_t p_workers_per_sm = 32;
 static int64_t p_device = 0;

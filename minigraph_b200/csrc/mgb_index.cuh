@@ -61,7 +61,10 @@ inline cudaError_t build_index_device(const u128 *d_mz, uint64_t n, int hash_bit
 	const uint64_t n1 = n? n : 1;
 	for (int b = 0; b < 2; ++b) { MGB_CU(cudaMalloc(&key[b], n1 * 8)); MGB_CU(cudaMalloc(&val[b], n1 * 8)); }
 	MGB_CU(cudaMalloc(&flag, n1 * 4)); MGB_CU(cudaMalloc(&rank, n1 * 4));
-	const int grid = 148 * 8, blk = 256;
+	int dev = 0, n_sm = 0;
+	MGB_CU(cudaGetDevice(&dev));
+	MGB_CU(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+	const int grid = n_sm * 8, blk = 256; // grid-stride loops: eight blocks per SM
 	k_idx_split<<<grid, blk, 0, stream>>>(d_mz, n, key[0], val[0]);
 	// order by (minimizer, position): a stable sort by position, then a stable sort by minimizer
 	cub::DoubleBuffer<uint64_t> kb(val[0], val[1]), vb(key[0], key[1]); // first pass: positions are the keys

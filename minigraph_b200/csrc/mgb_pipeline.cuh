@@ -173,7 +173,7 @@ MG_HD inline int stage_seed(const PipeCtx &c, int rid, Arena &A, int lane, int32
 			Arena R;
 			arena_init(R, smem, smem? (uint64_t)SKETCH_SMEM_BYTES : 0);
 			Arena &S = smem && R.cap >= (uint64_t)n_a / 4 + 3400? R : A;
-			MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, &A, true)); // digit walk: k_seed 31.9 -> 24.5 ms per 40 000 reads
+			MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, &A, true)); // digit walk: the seeds are in HBM
 		}
 	}
 	if (lane == 0) prof_add(c, PROF_SEED_SKETCH_CYC, t1 - t0), prof_add(c, PROF_SEED_MATCH_CYC, t2 - t1), prof_add(c, PROF_SEED_SORT_CYC, prof_clock() - t2);
@@ -249,8 +249,8 @@ MG_HD inline int stage_chain_tail2(const PipeCtx &c, ReadMeta &m, const LChain *
 // arrays the chaining loops re-read for every anchor (f/p/v/t, the RMQ priorities and window) are taken from the rest of the slice
 // (MGB_ALLOC_HOT); only the surviving anchors go back to HBM, as one bulk store.  What is touched once (end-point list, sort
 // scratch, chain records) stays in the worker's HBM arena, so that a slice is small and many warps are resident: the loops are
-// bound by the latency of their warp-wide votes, and what hides that is warps (measured on B200: everything in a 36 KB slice,
-// 6 warps per SM, was 2.2 times faster per warp and 2 times slower per kernel than 26 warps per SM working in HBM).
+// bound by the latency of their warp-wide votes, and what hides that is warps (everything in a 36 KB slice, 6 warps per SM, was
+// faster per warp but slower per kernel than many more warps per SM working in HBM).
 // A read whose seeds do not fit the slice works on the HBM copy, with whatever fits of the hot arrays still on chip.
 static const int CHAIN_SMEM_BYTES = 16 * 1024;        // per warp, k_chain: anchors + f/p/v/t of a read of up to ~500 seeds
 static const int CHAIN_RESCUE_SMEM_BYTES = 18 * 1024; // per warp, k_chain_rescue: + window and block summaries of the RMQ pass (the priorities if they fit)
@@ -315,7 +315,7 @@ MG_HD inline int chain_pass(const PipeCtx &c, int rid, Arena &H, Arena &A, u128 
 	} else {
 		{ // back into target order; the sort's range stack and bin tables on chip when the slice has the room (it is empty but for the anchors)
 			Arena &S = H.cap - H.top >= (uint64_t)n_a / 4 + 3400? H : A;
-			MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, 0, false)); // (in place: with the digit walk the chaining kernels measured 2 ms per 40 000 reads slower)
+			MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, 0, false)); // (in place: the list is on chip, where the digit walk was slower)
 		}
 		MGB_TRY(chain_rmq_w(H, A, o.max_gap, o.max_gap_pre, o.bw_long, o.max_lc_skip, o.rmq_size_cap, o.min_lc_cnt, o.min_lc_score,
 							o.chn_pen_gap, o.chn_pen_skip, n_a, a, &n_lc, &u, &n_a_new, lane));

@@ -1,4 +1,4 @@
-// mgb_tma.cuh -- bulk asynchronous copies between HBM and shared memory (sm_90+/sm_100a: cp.async.bulk + mbarrier; SASS UBLKCP /
+// mgb_tma.cuh -- bulk asynchronous copies between HBM and shared memory (sm_90a: cp.async.bulk + mbarrier; SASS UBLKCP /
 // SYNCS).  One lane issues a copy of a whole contiguous record array (a read's seeds, 16 bytes each) and the warp waits on the
 // transaction barrier; the way back is a bulk store of the compacted array.  Addresses and sizes are multiples of 16 bytes.
 // In the CPU simulators of the tests the same calls are plain copies.

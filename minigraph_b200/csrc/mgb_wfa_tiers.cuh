@@ -8,8 +8,7 @@
 //   shared-memory loads at columns (d-1, d, d+1) mod W.  The window may hold W - 2 diagonals (column lo-1 must not alias hi+1);
 // * the four votes of a wavefront are one OR-reduction of four bits; the corner test runs on the one diagonal that can
 //   reach the corner; the "does the window still grow" test runs on the two edge cells only.
-// Measured on B200 (round 2, config 2): 131 instead of 189 SASS instructions per 32 cells against the bounds-checked layout it
-// replaced; k_wfa_small 7.6 -> 5.1 ms, k_wfa_mid 21.8 -> 18.3 ms, k_wfa_big 13.6 -> 12.8 ms.
+// The layout compiles to about two thirds of the SASS instructions per 32 cells of the bounds-checked layout it replaced.
 #pragma once
 #include "mgb_wfa.cuh"
 
@@ -40,12 +39,11 @@ MG_HD inline int32_t wf2_ld(const void *base, int32_t off)
 // votes, extension along exact matches (miniwfa.c:212-226) and the five stores.  The slots of score ns are not read while a
 // wavefront is computed, so the FINISH of one cell may follow the LOAD of the next.  Expected in scope: H E1 F1 E2 F2 (arrays),
 // bHx bHo1 bHo2 bE1 bE2 bnH bn3 bn2 (byte offsets of the slices), colmask2 (2W-1), ax, lo, hi, tl, ql, ts, qs, d_corner, vote.
-// Measured on B200 (round 2, config 3, ms per 40 000 reads): tiers 1/2 (ring in shared memory) walk a wavefront one cell per lane at a
-// time -- two cells in flight were slower (k_wfa_mid 103.9 -> 114.1), and so was a packed walk of two adjacent diagonals per lane
-// (word loads, VIMNMX.S16x2 maxima whose predicates are the traceback bits: 103.2 -> 115.7; per pair it executes as many instructions
-// as two cells, on half the lanes); tier 3 (ring in L2) keeps two cells in flight: eighteen loads before the first use
-// (k_wfa_big 108.5 -> 82.2 at 16 warps per SM; 86.5 at 20 warps / 96 registers, 102.4 at 24 / 80 with spills; three cells in
-// flight 80.4, four 87.6: the kernel is bound by what L2 delivers, not by the latency one warp sees).
+// Tiers 1/2 (ring in shared memory) walk a wavefront one cell per lane at a time -- two cells in flight were slower, and so was a
+// packed walk of two adjacent diagonals per lane (word loads, VIMNMX.S16x2 maxima whose predicates are the traceback bits; per pair
+// it executes as many instructions as two cells, on half the lanes); tier 3 (ring in L2) keeps two cells in flight: eighteen loads
+// before the first use, at 16 warps per SM (more warps cost registers and spills; more cells in flight did not help: the kernel
+// is bound by what L2 delivers, not by the latency one warp sees).
 #define MGB_WF_CELL_LOAD(S, d_) \
 	int32_t h##S, e1##S, e2##S, f1##S, f2##S; \
 	uint8_t xz##S; \
@@ -222,8 +220,8 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 // has a cell inside the matrix in any of its five components -- the one reader of E/F values older than two scores.  Instead of
 // keeping 17 slots of all five arrays for it (85 slices), the 17 wavefronts in front of a shrink note, per diagonal, the last
 // score with such a cell in one extra slice G; the ring is then H x 17, E1/F1 x 3, E2/F2 x 2 as in the on-chip tiers: 28 slices.
-// Measured on B200 (round 2, config 3): the 85-slice ring of the resident warps did not fit L2 -- k_wfa_big moved 67 GB through
-// DRAM per 20 000 reads (11 bytes written per cell, every wavefront evicted before its slot was reused).
+// An 85-slice ring of the resident warps does not fit L2: every wavefront is evicted before its slot is reused, and each cell
+// costs about 11 bytes of DRAM writes.
 static const int WF3_NSL = 17 + 3 + 3 + 2 + 2 + 1;
 #define MGB_WF2_FILL(need_lo_, need_hi_) do { \
 		const int32_t nl_ = (need_lo_), nh_ = (need_hi_); \

@@ -355,13 +355,31 @@ def case_wfa_band_shrinks(lib, n_cases=48, seed=99):
 def case_radix_exact(lib, n_cases=60, seed=17):
     """the warp-wide replay of klib's unstable radix sort (mgb_common.cuh radix_sort_exact_w), in place and as a walk over digits, with
     scratch on "chip" and in the arena: the same order as radix_sort_128x() of the reference, ties included (ksort.h:112-162) --
-    few distinct keys (long runs of ties), keys that differ in one byte only (one level), bins above 64 elements (recursion), skewed bins"""
+    few distinct keys (long runs of ties), keys that differ in one byte only (one level), bins above 64 elements (recursion), skewed bins.
+    Without a build of the reference, its order comes from the plain-C restatement (oracle/mgoracle.c), whose tie order
+    tests/test_oracle.py pins against golden vectors of the reference's sort."""
     import ctypes as C
     import random
     from minigraph_b200 import capi
-    ref = T.load_ref()
-    ref.radix_sort_128x.restype = None
-    ref.radix_sort_128x.argtypes = [C.POINTER(capi.mg128_t), C.POINTER(capi.mg128_t)]
+    if T.have_ref():
+        ref = T.load_ref()
+        ref.radix_sort_128x.restype = None
+        ref.radix_sort_128x.argtypes = [C.POINTER(capi.mg128_t), C.POINTER(capi.mg128_t)]
+
+        def ref_sort(a, n):
+            ref.radix_sort_128x(a, C.cast(C.byref(a, C.sizeof(a)), C.POINTER(capi.mg128_t)))
+    else:
+        import subprocess
+        subprocess.check_call(["make", "-s", "-C", os.path.join(T.REPO, "oracle"), "liboracle.so"])
+        orc = C.CDLL(os.path.join(T.REPO, "oracle", "liboracle.so"))
+        orc.orc_radix_sort_128x.restype = None
+        orc.orc_radix_sort_128x.argtypes = [C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.c_int64]
+
+        def ref_sort(a, n):
+            x, y = (C.c_uint64 * n)(*[a[i].x for i in range(n)]), (C.c_uint64 * n)(*[a[i].y for i in range(n)])
+            orc.orc_radix_sort_128x(x, y, n)
+            for i in range(n):
+                a[i].x, a[i].y = x[i], y[i]
     lib.mgb_test_radix128.restype = C.c_int
     lib.mgb_test_radix128.argtypes = [C.POINTER(capi.mg128_t), C.c_int64, C.c_int, C.c_int]
     rng = random.Random(seed)
@@ -377,7 +395,7 @@ def case_radix_exact(lib, n_cases=60, seed=17):
         want = (capi.mg128_t * n)()
         for i, x in enumerate(keys):
             want[i].x, want[i].y = x, i
-        ref.radix_sort_128x(want, C.cast(C.byref(want, C.sizeof(want)), C.POINTER(capi.mg128_t)))
+        ref_sort(want, n)
         for walk, hot in ((0, 0), (1, 0), (1, 16384), (1, n // 4 + 3400), (0, 16384)):  # (n/4 + 3400: what the callers ask of the on-chip slice; the digits then go to the arena)
             got = (capi.mg128_t * n)()
             for i, x in enumerate(keys):

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(REPO, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `pytest -m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device, an H100 (run with `pytest -m gpu`)")
 
 
 @pytest.fixture(scope="session", autouse=True)

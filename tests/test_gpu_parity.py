@@ -1,4 +1,4 @@
-"""GPU parity tests: libmgb200.so (CUDA, sm_100a) through the C ABI against the golden GAF and oracle/_ref."""
+"""GPU parity tests: libmgb200.so (CUDA, sm_90a) through the C ABI against the golden GAF and oracle/_ref."""
 import os
 
 import pytest

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """SASS of libmgb200.so by kernel: size, instruction mix, and the bulk-copy / barrier sequence of the chaining kernels.
 
-    python tools/sass_counts.py [minigraph_b200/libmgb200.so] > profiles/rNN_sass_counts.txt
+    python tools/sass_counts.py [minigraph_b200/libmgb200.so] > sass_counts.txt
 
 (cuobjdump -sass; no GPU needed.)  UBLKCP = cp.async.bulk, SYNCS = mbarrier, VIMNMX/REDUX = the integer paths of the WFA cell and of the
 warp reductions.  Device functions kept out of line (MG_NOINLINE) are counted with the kernel they belong to."""
@@ -29,7 +29,7 @@ for line in txt.split("\n"):
         if m:
             kern[cur].append((m.group(1), re.sub(r"\s+", " ", m.group(2))))
 COLS = ("LDG", "LDS", "STG", "STS", "LDL", "STL", "SHFL", "VOTE", "REDUX", "VIMNMX", "UBLKCP", "SYNCS")
-print("# SASS of minigraph_b200/libmgb200.so (cuobjdump -sass, sm_100a): size and instruction mix of every kernel of the path (tools/sass_counts.py),")
+print("# SASS of minigraph_b200/libmgb200.so (cuobjdump -sass, sm_90a): size and instruction mix of every kernel of the path (tools/sass_counts.py),")
 print("# then the bulk-copy / barrier sequence of the chaining kernels (UBLKCP = cp.async.bulk, SYNCS = mbarrier).\n")
 print("%-18s %7s " % ("kernel", "instr") + " ".join("%6s" % c for c in COLS))
 for k, ins in kern.items():
