@@ -250,6 +250,24 @@ typedef struct {
  * heuristic, miniwfa.c:824-834, with checkpoints every `step` scores); returns n_cigar (len<<4|op) or a negative code */
 int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int64_t max_iter, int step, uint32_t *cigar, int cap, int *score);
 
+/* test hook: n gaps through one on-chip WFA tier (1: windows of 62 diagonals, sides of 256 bases, 4096 traceback bytes in shared
+ * memory; 2: 254 diagonals, 1024 bases), launched as the tier's kernel is.  Gap i is ts[t_off[i]..+tl[i]) against
+ * qs[q_off[i]..+ql[i]).  out[4i..4i+3] = rc (0: aligned, 1: does not fit the tier, < 0: error), score, n_iter, n_cigar; the CIGAR
+ * (len<<4|op) goes to cigar[i*cap..].  Returns 0, or a negative code (nothing run) when a gap has an empty side. */
+int mgb_test_wfa_tier(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
+					  const int32_t *ql, int64_t *out, uint32_t *cigar, int cap);
+
+/* test hook: n bridging alignments (gchain1.c:349-381 bridge_gwfa) on the graph of gi: query q[q_off[i]..+ql[i]) from
+ * (v0[i], off0[i]) to (v1[i], off1[i]), stopping at score max_ed[i].  mode 0: the warp-wide alignment of the bridging kernel;
+ * mode 1: the sequential one of graph chaining.  out[6i..6i+5] = rc, s (-1: not reached), end_v, end_off, nv, n_iter; the walk
+ * goes to walk[i*walk_cap..].  Returns 0, or a negative code (nothing run) when a query is empty or an end lies outside the graph. */
+int mgb_test_gwfa(const mg_idx_t *gi, int mode, int n, const char *q, const int64_t *q_off, const int32_t *ql, const uint32_t *v0,
+				  const int32_t *off0, const uint32_t *v1, const int32_t *off1, const int32_t *max_ed, int64_t *out, int32_t *walk, int walk_cap);
+
+/* test hook: the exact radix sort of the seeds (klib's radix_sort_128x order, ties included) on one warp, in place (walk 0) or
+ * by digit walk (walk 1), with hot_bytes of shared memory for its scratch (0: all of it in global memory); 0 or a negative code */
+int mgb_test_radix128(mg128_t *a, int64_t n, int walk, int hot_bytes);
+
 const char *mgb_last_error(void);
 void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st);
 /* knobs: "arena_mb" (per worker), "workers_per_sm", "device"; returns 0 if the key is known */

@@ -171,6 +171,13 @@ def bind_engine_api(lib):
                                   C.POINTER(mg_gchains_t), C.c_int32, C.c_char_p, C.c_uint64]
     lib.mgb_test_wfa.restype = C.c_int
     lib.mgb_test_wfa.argtypes = [C.c_char_p, C.c_int, C.c_char_p, C.c_int, C.c_int64, C.c_int, C.POINTER(C.c_uint32), C.c_int, C.POINTER(C.c_int)]
+    i64p, i32p, u32p = C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_uint32)
+    lib.mgb_test_wfa_tier.restype = C.c_int
+    lib.mgb_test_wfa_tier.argtypes = [C.c_int, C.c_int, C.c_char_p, i64p, i32p, C.c_char_p, i64p, i32p, i64p, u32p, C.c_int]
+    lib.mgb_test_gwfa.restype = C.c_int
+    lib.mgb_test_gwfa.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.c_int, C.c_char_p, i64p, i32p, u32p, i32p, u32p, i32p, i32p, i64p, i32p, C.c_int]
+    lib.mgb_test_radix128.restype = C.c_int
+    lib.mgb_test_radix128.argtypes = [C.POINTER(mg128_t), C.c_int64, C.c_int, C.c_int]
     lib.mg_map_batch_frag.restype = C.c_int
     lib.mg_map_batch_frag.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
                                       C.POINTER(C.POINTER(mg_gchains_t)), C.POINTER(mg_mapopt_t)]

@@ -1903,30 +1903,297 @@ extern "C" int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int6
 	try { return test_wfa_impl(ts, tl, qs, ql, max_iter, step, cigar, cap, score); } catch (const MgbError &e) { return e.code; }
 }
 
-#ifdef MGB_HOSTSIM
-// TEST INFRASTRUCTURE (simulator builds only): the warp-wide exact radix sort on an array of 16-byte records, in place or with the digit
-// walk, with `hot_bytes` of "on-chip" scratch (0: everything in the arena).  tests/test_hostsim32_lanes.py holds it against klib's.
-extern "C" int mgb_test_radix128(u128 *a, int64_t n, int walk, int hot_bytes)
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: a batch of gaps through one on-chip WFA tier, wfa_smem() with the template arguments of k_wfa_small (tier 1)
+// or k_wfa_mid (tier 2), launched as those kernels are: STAGE_WARPS[4] / [6] warps per block, WfTier1/2::STRIDE bytes of
+// shared memory per warp, one gap per warp at a time.  The shared memory starts out filled with cells that are not -inf,
+// and a warp aligns several gaps in a row, so the results also show that wfa_smem() clears the slices it reads and that the
+// warps of a block keep to their own slices.
+// ---------------------------------------------------------------------------------------------------------------
+static const uint32_t TEST_SMEM_FILL = 0x00050005u; // two cells holding offset 5, a value a real wavefront holds
+struct TestTierArgs {
+	int tier, n, cap;
+	const char *ts, *qs;
+	const int64_t *t_off, *q_off;
+	const int32_t *tl, *ql;
+	int64_t *out;       // per gap: rc (0: aligned, 1: does not fit the tier), score, n_iter, n_cigar
+	uint32_t *cigar;    // per gap: cap entries
+	char *arena;
+	uint64_t arena_bytes;
+};
+MG_HD inline void test_wfa_tier_body(const TestTierArgs &t, int i, int32_t *smem, Arena &A, int lane)
 {
-	std::vector<char> cold((size_t)n * 64 + (1 << 20)), hot((size_t)(hot_bytes > 0? hot_bytes : 16));
-	int rc_all = 0;
-#if MGB_W > 1
-	int rcs[MGB_W];
-	sim::run_warp(MGB_W, [&](int lane) {
-		Arena A, H;
-		arena_init(A, cold.data(), cold.size());
-		arena_init(H, hot.data(), hot_bytes > 0? (uint64_t)hot_bytes : 0);
-		rcs[lane] = radix_sort_128x_w(hot_bytes > 0? H : A, a, n, lane, &A, walk != 0);
-	});
-	for (int l = 0; l < MGB_W; ++l) if (rcs[l] != rcs[0]) return -99; else rc_all = rcs[0];
-#else
-	Arena A, H;
-	arena_init(A, cold.data(), cold.size());
-	arena_init(H, hot.data(), hot_bytes > 0? (uint64_t)hot_bytes : 0);
-	rc_all = radix_sort_128x_w(hot_bytes > 0? H : A, a, n, 0, &A, walk != 0);
-#endif
-	return rc_all;
+	WfResult r;
+	A.top = 0;
+	const char *ts = t.ts + t.t_off[i], *qs = t.qs + t.q_off[i];
+	int rc = t.tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane)
+						: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane);
+	if (rc == 0 && r.n_cigar > t.cap) rc = MGB_E_INTERNAL;
+	if (rc == 0) for (int32_t j = lane; j < r.n_cigar; j += MGB_W) t.cigar[(int64_t)i * t.cap + j] = r.cigar[j];
+	if (lane == 0) {
+		int64_t *o = t.out + 4 * (int64_t)i;
+		o[0] = rc, o[1] = rc == 0? r.s : -1, o[2] = rc == 0? r.n_iter : 0, o[3] = rc == 0? r.n_cigar : 0;
+	}
+	warp_sync();
+}
+#ifndef MGB_HOSTSIM
+template<int TIER>
+__global__ void k_test_wfa_tier(TestTierArgs t)
+{
+	extern __shared__ int4 dyn_smem[];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+	const int stride = TIER == 1? WfTier1::STRIDE : WfTier2::STRIDE;
+	for (int j = threadIdx.x; j < n_warps * stride / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
+	__syncthreads();
+	int32_t *smem = (int32_t*)((char*)dyn_smem + (size_t)warp * stride);
+	const int worker = blockIdx.x * n_warps + warp;
+	Arena A;
+	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
+	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_wfa_tier_body(t, i, smem, A, lane);
 }
 #endif
+
+// copies a host array to the device (or, in the simulators, to a fresh host block); released by the caller with dfree()
+template<typename T> static T *dcopy(const T *h, int64_t n)
+{
+	T *d = (T*)dmalloc((size_t)n * sizeof(T));
+	h2d(d, h, (size_t)n * sizeof(T));
+	return d;
+}
+static int64_t test_seq_bytes(int n, const int64_t *off, const int32_t *len)
+{
+	int64_t end = 0;
+	for (int i = 0; i < n; ++i) end = std::max(end, off[i] + len[i]);
+	return end;
+}
+
+static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
+							  const int32_t *ql, int64_t *out, uint32_t *cigar, int cap)
+{
+	if ((tier != 1 && tier != 2) || n < 0 || cap < 0) { set_error("mgb_test_wfa_tier: tier must be 1 or 2, n and cap at least 0"); return MGB_E_UNSUPPORTED; }
+	for (int i = 0; i < n; ++i) // the gaps of real jobs are never empty on either side (galign.c:97-99 emits plain I/D for those)
+		if (tl[i] < 1 || ql[i] < 1 || t_off[i] < 0 || q_off[i] < 0) { set_error("mgb_test_wfa_tier: gap " + std::to_string(i) + " has an empty side"); return MGB_E_UNSUPPORTED; }
+	if (n == 0) return 0;
+	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
+	const int stage = tier == 1? 4 : 6, warps = STAGE_WARPS[stage];
+	const int stride = tier == 1? WfTier1::STRIDE : WfTier2::STRIDE;
+	const int n_workers = std::min(n, 64 * warps);
+	TestTierArgs t;
+	t.tier = tier, t.n = n, t.cap = cap;
+	t.ts = dcopy(ts, test_seq_bytes(n, t_off, tl)), t.qs = dcopy(qs, test_seq_bytes(n, q_off, ql));
+	t.t_off = dcopy(t_off, n), t.q_off = dcopy(q_off, n), t.tl = dcopy(tl, n), t.ql = dcopy(ql, n);
+	t.out = (int64_t*)dmalloc(sizeof(int64_t) * 4 * (size_t)n);
+	t.cigar = (uint32_t*)dmalloc(sizeof(uint32_t) * ((size_t)n * cap + 1));
+	t.arena_bytes = (uint64_t)256 << 10; // a tier-2 gap needs at most 8 KB of CIGAR and 70 KB of traceback rows
+	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
+#ifdef MGB_HOSTSIM
+	std::vector<uint32_t> sim_smem((size_t)warps * stride / 4, TEST_SMEM_FILL);
+	for (int i = 0; i < n; ++i) {
+		int32_t *smem = (int32_t*)((char*)sim_smem.data() + (size_t)(i % warps) * stride);
+		char *arena = t.arena + (uint64_t)(i % n_workers) * t.arena_bytes;
+#if MGB_W > 1
+		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, arena, t.arena_bytes); test_wfa_tier_body(t, i, smem, A, lane); });
+#else
+		Arena A;
+		arena_init(A, arena, t.arena_bytes);
+		test_wfa_tier_body(t, i, smem, A, 0);
+#endif
+	}
+#else
+	const size_t smem = (size_t)warps * stride;
+	void (*kern)(TestTierArgs) = tier == 1? k_test_wfa_tier<1> : k_test_wfa_tier<2>;
+	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	kern<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
+	CUDA_OK(cudaGetLastError());
+	dsync();
+#endif
+	d2h(out, t.out, sizeof(int64_t) * 4 * (size_t)n);
+	d2h(cigar, t.cigar, sizeof(uint32_t) * (size_t)n * cap);
+	dfree((void*)t.ts), dfree((void*)t.qs), dfree((void*)t.t_off), dfree((void*)t.q_off), dfree((void*)t.tl), dfree((void*)t.ql);
+	dfree(t.out), dfree(t.cigar), dfree(t.arena);
+	return 0;
+}
+
+extern "C" int mgb_test_wfa_tier(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
+								 const int32_t *ql, int64_t *out, uint32_t *cigar, int cap)
+{
+	try { return test_wfa_tier_impl(tier, n, ts, t_off, tl, qs, q_off, ql, out, cigar, cap); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: bridging alignments (reference: gchain1.c:349-381 bridge_gwfa) on the device graph of an index, with the
+// options bridge_gwfa gives gfa_ed_init/gfa_ed_step.  mode 0: gwf_align_w() on one warp, the alignment state in shared
+// memory and the arena in global memory, as k_gwfa runs it (gwfa_job_run); mode 1: the sequential gwf_align() on lane 0,
+// as graph chaining runs it (gc_bridge_gwfa).
+// ---------------------------------------------------------------------------------------------------------------
+struct TestGwfaArgs {
+	GraphDev g;
+	int mode, n, walk_cap;
+	const char *q;
+	const int64_t *q_off;
+	const int32_t *ql, *off0, *off1, *max_ed;
+	const uint32_t *v0, *v1;
+	int64_t *out;       // per bridge: rc, s, end_v, end_off, nv, n_iter
+	int32_t *walk;      // per bridge: walk_cap vertices
+	char *arena;
+	uint64_t arena_bytes;
+};
+MG_HD inline void test_gwfa_body(const TestGwfaArgs &t, int i, GwfShared *sh, Arena &A, int lane)
+{
+	GwfOpt opt;
+	opt.traceback = 1, opt.max_chk = 1000, opt.bw_dyn = 1000, opt.max_lag = t.max_ed[i] / 2, opt.s_term = -1;
+	opt.i_term = 500000000LL;
+	A.top = 0, A.peak = 0;
+	const char *q = t.q + t.q_off[i];
+	int rc = 0;
+	GwfResult rs;
+	const GwfResult *r = &rs;
+	if (t.mode == 0) {
+		if (lane == 0) sh->A = A;
+		warp_sync();
+		rc = gwf_align_w(sh, t.g, opt, t.ql[i], q, t.v0[i], t.off0[i], t.v1[i], t.off1[i], t.max_ed[i], lane); // s_term: max_ed
+		r = &sh->r;
+	} else {
+		if (lane == 0) rc = gwf_align(A, t.g, opt, t.ql[i], q, t.v0[i], t.off0[i], t.v1[i], t.off1[i], t.max_ed[i], &rs);
+		rc = warp_bcast_i32(rc, 0);
+	}
+	if (lane == 0) {
+		int64_t *o = t.out + 6 * (int64_t)i;
+		const int32_t nv = rc == 0 && r->s >= 0? r->nv : 0;
+		if (nv > t.walk_cap) rc = MGB_E_INTERNAL;
+		o[0] = rc;
+		o[1] = rc == 0? r->s : -1, o[2] = rc == 0? (int64_t)r->end_v : -1, o[3] = rc == 0? r->end_off : -1;
+		o[4] = rc == 0? nv : 0, o[5] = rc == 0? r->n_iter : 0;
+		if (rc == 0) for (int32_t j = 0; j < nv; ++j) t.walk[(int64_t)i * t.walk_cap + j] = r->v[j];
+	}
+	warp_sync();
+}
+#ifndef MGB_HOSTSIM
+__global__ void k_test_gwfa(TestGwfaArgs t)
+{
+	extern __shared__ int4 dyn_smem[];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+	GwfShared *sh = (GwfShared*)((char*)dyn_smem + (size_t)warp * GWFA_SMEM_ARENA);
+	const int worker = blockIdx.x * n_warps + warp;
+	Arena A;
+	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
+	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_gwfa_body(t, i, sh, A, lane);
+}
+#endif
+
+static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, const int64_t *q_off, const int32_t *ql, const uint32_t *v0,
+						  const int32_t *off0, const uint32_t *v1, const int32_t *off1, const int32_t *max_ed, int64_t *out, int32_t *walk, int walk_cap)
+{
+	if (gi == 0 || (mode != 0 && mode != 1) || n < 0 || walk_cap < 0) { set_error("mgb_test_gwfa: an index, mode 0 or 1, n and walk_cap at least 0"); return MGB_E_UNSUPPORTED; }
+	const Model *M = model_of(gi);
+	for (int i = 0; i < n; ++i)
+		if (ql[i] < 1 || q_off[i] < 0 || (v0[i] >> 1) >= (uint32_t)M->g.n_seg || (v1[i] >> 1) >= (uint32_t)M->g.n_seg || off0[i] < 0 || off0[i] >= M->seg_len[v0[i] >> 1]
+			|| off1[i] < 0 || off1[i] >= M->seg_len[v1[i] >> 1]) {
+			set_error("mgb_test_gwfa: bridge " + std::to_string(i) + " has an empty query or an end outside the graph");
+			return MGB_E_UNSUPPORTED;
+		}
+	if (n == 0) return 0;
+	if (!dev_ok(M->device)) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
+	const int warps = STAGE_WARPS[8], n_workers = std::min(n, 8 * warps);
+	TestGwfaArgs t;
+	t.g = M->g, t.mode = mode, t.n = n, t.walk_cap = walk_cap;
+	t.q = dcopy(q, test_seq_bytes(n, q_off, ql));
+	t.q_off = dcopy(q_off, n), t.ql = dcopy(ql, n), t.off0 = dcopy(off0, n), t.off1 = dcopy(off1, n), t.max_ed = dcopy(max_ed, n);
+	t.v0 = dcopy(v0, n), t.v1 = dcopy(v1, n);
+	t.out = (int64_t*)dmalloc(sizeof(int64_t) * 6 * (size_t)n);
+	t.walk = (int32_t*)dmalloc(sizeof(int32_t) * ((size_t)n * walk_cap + 1));
+	t.arena_bytes = (uint64_t)64 << 20;
+	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
+#ifdef MGB_HOSTSIM
+	std::vector<u128> sim_smem(GWFA_SMEM_ARENA / sizeof(u128));
+	GwfShared *sh = (GwfShared*)sim_smem.data();
+	for (int i = 0; i < n; ++i) {
+#if MGB_W > 1
+		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, t.arena, t.arena_bytes); test_gwfa_body(t, i, sh, A, lane); });
+#else
+		Arena A;
+		arena_init(A, t.arena, t.arena_bytes);
+		test_gwfa_body(t, i, sh, A, 0);
+#endif
+	}
+#else
+	const size_t smem = (size_t)warps * GWFA_SMEM_ARENA;
+	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test_gwfa, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	k_test_gwfa<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
+	CUDA_OK(cudaGetLastError());
+	dsync();
+#endif
+	d2h(out, t.out, sizeof(int64_t) * 6 * (size_t)n);
+	d2h(walk, t.walk, sizeof(int32_t) * (size_t)n * walk_cap);
+	dfree((void*)t.q), dfree((void*)t.q_off), dfree((void*)t.ql), dfree((void*)t.off0), dfree((void*)t.off1), dfree((void*)t.max_ed);
+	dfree((void*)t.v0), dfree((void*)t.v1), dfree(t.out), dfree(t.walk), dfree(t.arena);
+	return 0;
+}
+
+extern "C" int mgb_test_gwfa(const mg_idx_t *gi, int mode, int n, const char *q, const int64_t *q_off, const int32_t *ql, const uint32_t *v0,
+							 const int32_t *off0, const uint32_t *v1, const int32_t *off1, const int32_t *max_ed, int64_t *out, int32_t *walk, int walk_cap)
+{
+	try { return test_gwfa_impl(gi, mode, n, q, q_off, ql, v0, off0, v1, off1, max_ed, out, walk, walk_cap); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: the warp-wide exact radix sort on an array of 16-byte records, in place or with the digit walk, on one warp with
+// `hot_bytes` of shared memory for the range stack and bin tables (0: everything in the arena in global memory), as k_seed sorts
+// its seeds; tests/cases.py holds it against klib's.
+// ---------------------------------------------------------------------------------------------------------------
+struct TestRadixArgs { u128 *a; int64_t n; int walk, hot_bytes; char *cold; uint64_t cold_bytes; int32_t *rc; };
+MG_HD inline int test_radix_body(const TestRadixArgs &t, char *hot, int lane)
+{
+	Arena A, H;
+	arena_init(A, t.cold, t.cold_bytes);
+	arena_init(H, hot, t.hot_bytes > 0? (uint64_t)t.hot_bytes : 0);
+	return radix_sort_128x_w(t.hot_bytes > 0? H : A, t.a, t.n, lane, &A, t.walk != 0);
+}
+#ifndef MGB_HOSTSIM
+__global__ void k_test_radix128(TestRadixArgs t)
+{
+	extern __shared__ int4 dyn_smem[];
+	const int rc = test_radix_body(t, (char*)dyn_smem, threadIdx.x & 31);
+	if (threadIdx.x == 0) *t.rc = rc;
+}
+#endif
+
+static int test_radix128_impl(u128 *a, int64_t n, int walk, int hot_bytes)
+{
+	if (n < 0 || hot_bytes < 0 || hot_bytes > 200 * 1024) { set_error("mgb_test_radix128: n >= 0 and 0 <= hot_bytes <= 200 KB"); return MGB_E_UNSUPPORTED; }
+	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
+	TestRadixArgs t;
+	t.a = dcopy(a, n), t.n = n, t.walk = walk, t.hot_bytes = hot_bytes;
+	t.cold_bytes = (uint64_t)n * 64 + (1 << 20);
+	t.cold = (char*)dmalloc(t.cold_bytes);
+	t.rc = (int32_t*)dmalloc(sizeof(int32_t));
+	int32_t rc = 0;
+#ifdef MGB_HOSTSIM
+	std::vector<u128> hot((size_t)hot_bytes / sizeof(u128) + 1);
+#if MGB_W > 1
+	int rcs[MGB_W];
+	sim::run_warp(MGB_W, [&](int lane) { rcs[lane] = test_radix_body(t, (char*)hot.data(), lane); });
+	rc = rcs[0];
+	for (int l = 1; l < MGB_W; ++l) if (rcs[l] != rc) { set_error("simulated warp: lanes returned different codes from the sort"); rc = MGB_E_INTERNAL; }
+#else
+	rc = test_radix_body(t, (char*)hot.data(), 0);
+#endif
+#else
+	if (hot_bytes > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test_radix128, cudaFuncAttributeMaxDynamicSharedMemorySize, hot_bytes));
+	k_test_radix128<<<1, 32, (size_t)hot_bytes, t_stream>>>(t);
+	CUDA_OK(cudaGetLastError());
+	dsync();
+	d2h(&rc, t.rc, sizeof(rc));
+#endif
+	if (rc == 0) d2h(a, t.a, sizeof(u128) * (size_t)n);
+	dfree(t.a), dfree(t.cold), dfree(t.rc);
+	return rc;
+}
+
+extern "C" int mgb_test_radix128(mg128_t *a, int64_t n, int walk, int hot_bytes)
+{
+	static_assert(sizeof(mg128_t) == sizeof(u128), "mg128_t and u128 are the same record");
+	try { return test_radix128_impl((u128*)a, n, walk, hot_bytes); } catch (const MgbError &e) { return e.code; }
+}
 
 extern "C" void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st) { *st = t_has_stats? t_last_stats : model_of(gi)->stats; } // the calling thread's last batch

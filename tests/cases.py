@@ -352,7 +352,7 @@ def case_wfa_band_shrinks(lib, n_cases=48, seed=99):
     assert n_shrunk >= n_cases // 2
 
 
-def case_radix_exact(lib, n_cases=60, seed=17):
+def case_radix_exact(lib, n_cases=60, seed=17, hot_max=16384):
     """the warp-wide replay of klib's unstable radix sort (mgb_common.cuh radix_sort_exact_w), in place and as a walk over digits, with
     scratch on "chip" and in the arena: the same order as radix_sort_128x() of the reference, ties included (ksort.h:112-162) --
     few distinct keys (long runs of ties), keys that differ in one byte only (one level), bins above 64 elements (recursion), skewed bins.
@@ -380,8 +380,6 @@ def case_radix_exact(lib, n_cases=60, seed=17):
             orc.orc_radix_sort_128x(x, y, n)
             for i in range(n):
                 a[i].x, a[i].y = x[i], y[i]
-    lib.mgb_test_radix128.restype = C.c_int
-    lib.mgb_test_radix128.argtypes = [C.POINTER(capi.mg128_t), C.c_int64, C.c_int, C.c_int]
     rng = random.Random(seed)
     for it in range(n_cases):
         n = rng.choice([65, 191, 192, 193, 700, 1100, 3000, 9000])
@@ -396,7 +394,7 @@ def case_radix_exact(lib, n_cases=60, seed=17):
         for i, x in enumerate(keys):
             want[i].x, want[i].y = x, i
         ref_sort(want, n)
-        for walk, hot in ((0, 0), (1, 0), (1, 16384), (1, n // 4 + 3400), (0, 16384)):  # (n/4 + 3400: what the callers ask of the on-chip slice; the digits then go to the arena)
+        for walk, hot in ((0, 0), (1, 0), (1, hot_max), (1, n // 4 + 3400), (0, hot_max)):  # (n/4 + 3400: what the callers ask of the on-chip slice; the digits then go to the arena)
             got = (capi.mg128_t * n)()
             for i, x in enumerate(keys):
                 got[i].x, got[i].y = x, i
@@ -845,3 +843,462 @@ def case_no_diag(lib, workdir):
         assert d is None, (i, d)
     plain, _ = T.map_with_ref(fa, names[:2], seqs[:2], "asm")
     assert T.diff_results(plain[1], want[1]) is not None  # the flag did change something for the self-named prefix
+
+
+def _ref_wfa_exact(ts, qs):
+    """the reference's exact WFA with traceback and no cap (miniwfa.c:380-435 through mwf_wfa_exact): score, CIGAR, n_iter"""
+    import ctypes as C
+    ref = T.load_ref()
+    mwf_opt_t, mwf_rst_t = _mwf_types()
+    opt = mwf_opt_t()
+    ref.mwf_opt_init(C.byref(opt))
+    opt.flag |= 1
+    opt.step, opt.max_iter = 0, 10 ** 8
+    rst = mwf_rst_t()
+    ref.mwf_wfa_exact(None, C.byref(opt), len(ts), ts, len(qs), qs, C.byref(rst))
+    return rst.s, [rst.cigar[i] for i in range(rst.n_cigar)], rst.n_iter
+
+
+# the two on-chip tiers: (W diagonals in the ring, longest side, traceback bytes in shared memory or 0)
+WFA_TIERS = {1: (64, 256, 4096), 2: (256, 1024, 0)}
+
+
+def wfa_tier_gaps(tier, rng, scale=1):
+    """gaps drawn around every limit of an on-chip tier, as (tag, target, query) byte strings"""
+    W, maxlen, tbcap = WFA_TIERS[tier]
+
+    def rnd(n, alpha="ACGT"):
+        return "".join(rng.choices(alpha, k=n))
+
+    def noisy(s, rate):
+        out = []
+        for c in s:
+            u = rng.random()
+            if u < rate * 0.5:
+                out.append(rng.choice("ACGT"))
+            elif u < rate * 0.75:
+                continue
+            elif u < rate:
+                out += [c, rng.choice("ACGT")]
+            else:
+                out.append(c)
+        return "".join(out) or rng.choice("ACGT")
+    gaps = []
+    # lengths at the tier's limit and 1 past it, and single bases (jobs never have an empty side)
+    for L in sorted({1, 255, 256, 257, maxlen - 1, maxlen, maxlen + 1}):
+        t = rnd(L)
+        gaps += [("len", t, t), ("len", t, noisy(t, 0.02)), ("len", noisy(t, 0.03), t), ("len", t[:max(1, L - 3)], t),
+                 ("len", t, t[2:] or t), ("len", t[:1], t[:1]), ("len", t[:1], rnd(1)), ("len", rnd(3), t[:1])]
+    # windows that span the matrix: tl + ql + 1 just below, at and past the W - 2 diagonals the ring can hold
+    for span in range(W - 4, W + 1):
+        for _ in range(6 * scale):
+            tl = rng.randint(max(1, span // 2 - 8), span // 2 + 8)
+            ql = span - 1 - tl
+            t = rnd(tl)
+            gaps.append(("window", t, rnd(ql)))
+            gaps.append(("window", t, (noisy(t, rng.choice([0.1, 0.2, 0.35])) + rnd(ql))[:ql]))
+    # scores just below and at 255, found by asking the reference (tier 2; tier 1 cannot reach them in a window of 62 diagonals)
+    want_s = []
+    for _ in range(3000 * scale if tier == 2 else 0):
+        if len(want_s) >= 24 * scale:
+            break
+        n = rng.randint(90, 126)
+        t = rnd(n)
+        q = rnd(rng.randint(n - 6, min(253 - n, n + 6))) if rng.random() < 0.5 else noisy(t, rng.choice([0.45, 0.6]))[:253 - n]
+        s, _, _ = _ref_wfa_exact(t.encode(), q.encode())
+        if 236 <= s <= 274:
+            want_s.append(("score", t, q))
+    gaps += want_s
+    # the most traceback bytes a window that fits tier 1 can take: pairs without a single match that span the whole window
+    for _ in range(12 * scale if tbcap else 0):
+        n = rng.randint(20, 41)
+        gaps.append(("tbcap", rnd(n, "AC"), rnd(rng.choice([59, 60, 61]) - n, "GT")))
+    # identical pairs (the corner reached at score 0, a hit without extension), prefixes, low-complexity pairs (many ties),
+    # and N and lower-case bytes, which the alignment compares as they are
+    for n in (1, 2, 5, 40, 200):
+        t = rnd(n)
+        gaps += [("ident", t, t), ("prefix", t, t + rnd(3)), ("prefix", t + rnd(5), t)]
+    for _ in range(8 * scale):
+        n = rng.choice([10, 25, 60, 120, 300])
+        t = rnd(n, "AC")
+        gaps += [("ac", t, noisy(t, 0.1).replace("G", "A").replace("T", "C")), ("ac", t, rnd(max(1, n - 5), "AC"))]
+        t = rnd(n)
+        b = list(noisy(t, 0.05))
+        for j in rng.sample(range(len(b)), min(len(b), 3)):
+            b[j] = rng.choice("Nacgtn")
+        gaps += [("nlower", t, "".join(b)), ("nlower", t.lower(), t), ("nlower", "N" * n, "N" * (n + 1))]
+    return [(tag, t.encode(), q.encode()) for tag, t, q in gaps]
+
+
+def run_wfa_tier(lib, tier, gaps):
+    """all gaps in one call of the tier hook: [(rc, score, n_iter, cigar)] in input order"""
+    import ctypes as C
+    n = len(gaps)
+    ts, qs = b"".join(t for _, t, _ in gaps), b"".join(q for _, _, q in gaps)
+    t_off, q_off, tl, ql = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int32 * n)(), (C.c_int32 * n)()
+    a = b = 0
+    for i, (_, t, q) in enumerate(gaps):
+        t_off[i], q_off[i], tl[i], ql[i] = a, b, len(t), len(q)
+        a, b = a + len(t), b + len(q)
+    cap = max(len(t) + len(q) for _, t, q in gaps) + 2
+    out, cig = (C.c_int64 * (4 * n))(), (C.c_uint32 * (n * cap))()
+    assert lib.mgb_test_wfa_tier(tier, n, ts, t_off, tl, qs, q_off, ql, out, cig, cap) == 0, lib.mgb_last_error()
+    return [(out[4 * i], out[4 * i + 1], out[4 * i + 2], list(cig[i * cap:i * cap + out[4 * i + 3]])) for i in range(n)]
+
+
+def case_wfa_tier_edges(lib, tier, scale=1, seed=None):
+    """one on-chip WFA tier (wfa_smem, mgb_wfa_tiers.cuh: no bounds checks, 16-bit cells) on its own, against the reference's
+    mwf_wfa_exact, with gaps drawn around each of its limits.  Exact when accepted: a gap the tier aligns has the reference's
+    score, CIGAR and n_iter.  Must fit when provably in bounds: the window grows by at most one diagonal per side and score, so
+    a gap with both sides within the tier's length, a score below 255, min(2s+1, tl+ql+1) + 2 <= W and (tier 1) no more
+    traceback bytes than fit -- the reference's n_iter counts exactly those bytes -- may not be handed on to the next tier.  Must
+    give up past a limit that cannot be met: longer sides, score 255 or more, too many traceback bytes.  And every limit is met
+    in both directions: some gaps are aligned just inside it and some refused just past it -- except tier 1's traceback bytes,
+    which a window of 62 diagonals cannot fill (the gaps that come closest are aligned)."""
+    import random
+    W, maxlen, tbcap = WFA_TIERS[tier]
+    rng = random.Random(seed if seed is not None else 7 + tier)
+    gaps = wfa_tier_gaps(tier, rng, scale)
+    got = run_wfa_tier(lib, tier, gaps)
+    hits = {}
+    for i, ((tag, t, q), (rc, s, n_iter, cigar)) in enumerate(zip(gaps, got)):
+        tl, ql = len(t), len(q)
+        rs, rcig, rn = _ref_wfa_exact(t, q)
+        what = "tier %d gap %d (%s, tl=%d ql=%d, reference score %d n_iter %d): " % (tier, i, tag, tl, ql, rs, rn)
+        assert rc in (0, 1), what + "rc %d" % rc
+        if rc == 0:
+            assert (s, cigar, n_iter) == (rs, rcig, rn), what + "score %d n_iter %d, CIGAR %s" % (s, n_iter, "same" if cigar == rcig else "differs")
+        len_ok, s_ok = max(tl, ql) <= maxlen, rs <= 254
+        w_need = min(2 * rs + 1, tl + ql + 1) + 2
+        tb_ok = tbcap == 0 or rn <= tbcap
+        if len_ok and s_ok and w_need <= W and tb_ok:
+            assert rc == 0, what + "provably fits the tier (window of at most %d of %d columns) but was refused" % (w_need, W)
+        if not len_ok or not s_ok or not tb_ok:
+            assert rc == 1, what + "cannot fit the tier but was accepted"
+        inside, past = [], []
+        (inside if max(tl, ql) == maxlen else past if max(tl, ql) == maxlen + 1 else []).append("length")
+        if len_ok and s_ok and tb_ok:
+            (inside if W - 1 <= w_need <= W else past if W < w_need <= W + 2 else []).append("window")
+        if tier == 2 and len_ok and w_need <= W:
+            (inside if 240 <= rs <= 254 else past if 255 <= rs <= 270 else []).append("score")
+        if tbcap and w_need <= W:
+            # (tier 1) the window limit comes first: a gap whose window fits takes fewer than 4000 traceback bytes, so the
+            # capacity of 4096 never decides and nothing can be refused just past it; what is checked is that it is enough
+            assert rn <= tbcap, what + "fits the window but not the traceback bytes"
+            if rn >= tbcap - 300:
+                inside.append("traceback bytes")
+        for lim in inside:
+            hits.setdefault(lim, [0, 0])[0] += rc == 0
+        for lim in past:
+            hits.setdefault(lim, [0, 0])[1] += rc == 1
+    for lim in ["length", "window", "score"] if tier == 2 else ["length", "window", "traceback bytes"]:
+        a, r = hits.get(lim, [0, 0])
+        both = lim != "traceback bytes"
+        assert a > 0 and (r > 0 or not both), "tier %d: the %s limit was not met in both directions (%d gaps aligned just inside it, %d refused just past it)" % (tier, lim, a, r)
+    return hits
+
+
+def case_wfa_tier_rejects_empty(lib):
+    """a gap with an empty side is refused before anything runs (real jobs never have one: galign.c:97-99)"""
+    import ctypes as C
+    for tier in (1, 2):
+        for tl, ql in ((0, 5), (5, 0), (0, 0)):
+            one = lambda x: (C.c_int64 * 1)(x)  # noqa: E731
+            out, cig = (C.c_int64 * 4)(-7, -7, -7, -7), (C.c_uint32 * 16)()
+            rc = lib.mgb_test_wfa_tier(tier, 1, b"ACGTA", one(0), (C.c_int32 * 1)(tl), b"ACGTA", one(0), (C.c_int32 * 1)(ql), out, cig, 16)
+            assert rc < 0 and list(out) == [-7] * 4, (tier, tl, ql, rc)
+    out, cig = (C.c_int64 * 4)(), (C.c_uint32 * 16)()
+    assert lib.mgb_test_wfa_tier(3, 1, b"A", (C.c_int64 * 1)(0), (C.c_int32 * 1)(1), b"A", (C.c_int64 * 1)(0), (C.c_int32 * 1)(1), out, cig, 16) < 0
+
+
+_ged = None
+
+
+def _gfa_ed_types():
+    """ctypes view of gfa-priv.h:73-89 (gfa_edopt_t, gfa_edrst_t) and the prototypes of the reference's graph edit distance"""
+    global _ged
+    if _ged is None:
+        import ctypes as C
+        ref = T.load_ref()
+
+        class gfa_edopt_t(C.Structure):
+            _fields_ = [("traceback", C.c_int32), ("bw_dyn", C.c_int32), ("max_lag", C.c_int32), ("max_chk", C.c_int32),
+                        ("s_term", C.c_int32), ("i_term", C.c_int64)]
+
+        class gfa_edrst_t(C.Structure):
+            _fields_ = [("s", C.c_int32), ("end_v", C.c_uint32), ("end_off", C.c_int32), ("wlen", C.c_int32), ("n_end", C.c_int32),
+                        ("nv", C.c_int32), ("n_iter", C.c_int64), ("v", C.POINTER(C.c_int32))]
+        ref.gfa_edopt_init.restype = None
+        ref.gfa_edopt_init.argtypes = [C.POINTER(gfa_edopt_t)]
+        ref.gfa_edseq_init.restype = C.c_void_p
+        ref.gfa_edseq_init.argtypes = [C.POINTER(capi.gfa_t)]
+        ref.gfa_edseq_destroy.restype = None
+        ref.gfa_edseq_destroy.argtypes = [C.c_int32, C.c_void_p]
+        ref.gfa_ed_init.restype = C.c_void_p
+        ref.gfa_ed_init.argtypes = [C.c_void_p, C.POINTER(gfa_edopt_t), C.POINTER(capi.gfa_t), C.c_void_p, C.c_int32, C.c_char_p, C.c_uint32, C.c_int32]
+        ref.gfa_ed_step.restype = None
+        ref.gfa_ed_step.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_int32, C.POINTER(gfa_edrst_t)]
+        ref.gfa_ed_destroy.restype = None
+        ref.gfa_ed_destroy.argtypes = [C.c_void_p]
+        _ged = (gfa_edopt_t, gfa_edrst_t)
+    return _ged
+
+
+def _ref_bridge(g, es, q, v0, off0, v1, off1, max_ed, max_lag=None):
+    """gchain1.c:349-381 bridge_gwfa: gfa_ed_init + gfa_ed_step of the reference; (s, end_v, end_off, nv, walk, n_iter)"""
+    import ctypes as C
+    ref = T.load_ref()
+    gfa_edopt_t, gfa_edrst_t = _gfa_ed_types()
+    opt = gfa_edopt_t()
+    ref.gfa_edopt_init(C.byref(opt))
+    opt.traceback, opt.max_chk, opt.bw_dyn, opt.max_lag = 1, 1000, 1000, max_ed // 2 if max_lag is None else max_lag
+    opt.i_term = 500000000
+    r = gfa_edrst_t()
+    z = ref.gfa_ed_init(None, C.byref(opt), g, es, len(q), q, v0, off0)
+    ref.gfa_ed_step(z, v1, off1, max_ed, C.byref(r))
+    ref.gfa_ed_destroy(z)
+    walk = [r.v[i] for i in range(r.nv)] if r.s >= 0 else []
+    if r.s >= 0:
+        C.CDLL(None).free(r.v)
+    return r.s, r.end_v, r.end_off, len(walk), walk, r.n_iter
+
+
+class _Graph:
+    """segments and arcs of a GFA as the tests draw walks on it (vertex v = segment << 1 | reverse strand)"""
+
+    def __init__(self, fn):
+        self.names, self.seq, self.out = [], [], {}
+        ids = {}
+        for ln in open(fn):
+            t = ln.rstrip("\n").split("\t")
+            if t[0] == "S":
+                ids[t[1]] = len(self.names)
+                self.names.append(t[1])
+                self.seq.append(t[2].upper())
+        for ln in open(fn):
+            t = ln.rstrip("\n").split("\t")
+            if t[0] == "L":
+                v, w = ids[t[1]] << 1 | (t[2] == "-"), ids[t[3]] << 1 | (t[4] == "-")
+                self.out.setdefault(v, []).append(w)
+                self.out.setdefault(w ^ 1, []).append(v ^ 1)
+
+    def vseq(self, v):
+        s = self.seq[v >> 1]
+        return s[::-1].translate(str.maketrans("ACGTN", "TGCAN")) if v & 1 else s
+
+    def walk(self, rng, v, min_len):
+        """a random walk from v until it holds min_len bases (or meets a dead end)"""
+        w, n = [v], len(self.seq[v >> 1])
+        while n < min_len and self.out.get(w[-1]):
+            w.append(rng.choice(self.out[w[-1]]))
+            n += len(self.seq[w[-1] >> 1])
+        return w
+
+
+def _write_gfa(fn, segs, links):
+    with open(fn, "w") as f:
+        for name, s in segs:
+            f.write("S\t%s\t%s\n" % (name, s))
+        for a, sa, b, sb in links:
+            f.write("L\t%s\t%s\t%s\t%s\t0M\n" % (a, sa, b, sb))
+
+
+def _bridge_graphs(workdir, rng):
+    """small GFAs for the situations the bridging alignment has to get right: {tag: path}"""
+    def rnd(n):
+        return "".join(rng.choices("ACGT", k=n))
+    out = {}
+    segs = [("c%d" % i, rnd(1)) for i in range(80)]  # a chain of 1-bp segments between two longer ones
+    segs = [("cL", rnd(30))] + segs + [("cR", rnd(30))]
+    out["chain1bp"] = (segs, [(segs[i][0], "+", segs[i + 1][0], "+") for i in range(len(segs) - 1)])
+    alle = [rnd(rng.randint(4, 9)) for _ in range(30)]
+    alle += [alle[i] for i in range(5)] + [alle[i][:-1] for i in range(5, 10)]  # alleles twice, and alleles one base shorter
+    segs = [("fA", rnd(40))] + [("f%d" % i, a) for i, a in enumerate(alle)] + [("fB", rnd(40))]
+    out["fanout40"] = (segs, [("fA", "+", "f%d" % i, "+") for i in range(40)] + [("f%d" % i, "+", "fB", "+") for i in range(40)])
+    segs, links = [("w0", rnd(20))], []  # eight 40-way bubbles in a row: wavefronts of more than max_chk diagonals (pruning)
+    for b in range(8):
+        for i in range(40):
+            segs.append(("w%d_%d" % (b, i), rnd(rng.randint(3, 12)) if i % 4 else alle[i]))
+            links += [("w%d" % b, "+", "w%d_%d" % (b, i), "+"), ("w%d_%d" % (b, i), "+", "w%d" % (b + 1), "+")]
+        segs.append(("w%d" % (b + 1), rnd(20)))
+    out["wide"] = (segs, links)
+    segs = [(n, rnd(rng.randint(5, 40))) for n in "ABCDEFGHIJ"]  # nested bubbles
+    out["nested"] = (segs, [("A", "+", "B", "+"), ("A", "+", "F", "+"), ("B", "+", "C", "+"), ("B", "+", "D", "+"), ("C", "+", "E", "+"),
+                            ("D", "+", "E", "+"), ("E", "+", "G", "+"), ("F", "+", "G", "+"), ("G", "+", "H", "+"), ("G", "+", "I", "+"),
+                            ("H", "+", "J", "+"), ("I", "+", "J", "+"), ("B", "+", "E", "+")])
+    segs = [("sA", rnd(25)), ("sL", rnd(6)), ("sB", rnd(9)), ("sC", rnd(7)), ("sD", rnd(30)), ("sZ", rnd(50))]  # loops, strand switches
+    out["cycles"] = (segs, [("sA", "+", "sL", "+"), ("sL", "+", "sL", "+"), ("sL", "+", "sB", "+"), ("sB", "+", "sC", "+"), ("sC", "+", "sB", "+"),
+                            ("sC", "+", "sD", "-"), ("sD", "-", "sA", "-"), ("sB", "-", "sD", "+")])  # sZ: not connected
+    paths = {}
+    for tag, (segs, links) in out.items():
+        paths[tag] = os.path.join(workdir, "bridge_%s.gfa" % tag)
+        _write_gfa(paths[tag], segs, links)
+    return paths
+
+
+def _ont_errors(rng, s, rate):
+    out = []
+    for c in s:
+        u = rng.random()
+        if u < rate * 0.4:
+            out.append(rng.choice("ACGT"))
+        elif u < rate * 0.7:
+            continue
+        elif u < rate:
+            out += [c, rng.choice("ACGT")]
+        else:
+            out.append(c)
+    return "".join(out)
+
+
+def _draw_bridges(G, rng, n, lens, rates, max_eds):
+    """n bridges along random walks of G: (query, v0, off0, v1, off1, max_ed, walk)"""
+    out = []
+    n_v = 2 * len(G.seq)
+    while len(out) < n:
+        v = rng.randrange(n_v)
+        L = rng.choice(lens)
+        w = G.walk(rng, v, L)
+        path = "".join(G.vseq(x) for x in w)
+        off0 = rng.randrange(len(G.seq[v >> 1])) if rng.random() < 0.7 else len(G.seq[v >> 1]) - 1
+        last = len(G.seq[w[-1] >> 1])
+        off1 = rng.randrange(last) if len(w) > 1 else rng.randrange(off0, last)
+        q = path[off0:len(path) - last + off1 + 1]
+        q = _ont_errors(rng, q, rng.choice(rates)) or q
+        if q:
+            out.append((q.encode(), v, off0, w[-1], off1, rng.choice(max_eds), w))
+    return out
+
+
+def run_gwfa(lib, gi, mode, bridges, walk_cap=4096):
+    """all bridges in one call of the bridging hook: [(rc, s, end_v, end_off, nv, walk, n_iter)] in input order"""
+    import ctypes as C
+    n = len(bridges)
+    q = b"".join(b[0] for b in bridges)
+    I64, I32, U32 = C.c_int64 * n, C.c_int32 * n, C.c_uint32 * n
+    q_off, ql = I64(), I32(*[len(b[0]) for b in bridges])
+    a = 0
+    for i, b in enumerate(bridges):
+        q_off[i], a = a, a + len(b[0])
+    v0, off0, v1, off1, med = U32(*[b[1] for b in bridges]), I32(*[b[2] for b in bridges]), U32(*[b[3] for b in bridges]), I32(*[b[4] for b in bridges]), I32(*[b[5] for b in bridges])
+    out, walk = (C.c_int64 * (6 * n))(), (C.c_int32 * (n * walk_cap))()
+    assert lib.mgb_test_gwfa(gi, mode, n, q, q_off, ql, v0, off0, v1, off1, med, out, walk, walk_cap) == 0, lib.mgb_last_error()
+    res = []
+    for i in range(n):
+        o = out[6 * i:6 * i + 6]
+        res.append((o[0], o[1], o[2], o[3], o[4], list(walk[i * walk_cap:i * walk_cap + o[4]]), o[5]))
+    return res
+
+
+def case_gwfa_bridges(lib, workdir, scale=1, seed=13, modes=(0, 1)):
+    """the bridging alignment between two linear chains (gchain1.c:349-381: gfa_ed_init + gfa_ed_step with bridge_gwfa's options)
+    on its own: the warp-wide gwf_align_w of k_gwfa (mode 0) and the sequential gwf_align of graph chaining (mode 1) against the
+    reference's gfa_ed on its own gfa_read of the same file -- score, end vertex and offset, walk and n_iter.  Graphs: a chain of
+    1-bp segments, a vertex with 40 out-arcs (more than a warp has lanes) whose alleles repeat (walks of equal cost), eight 40-way
+    bubbles in a row (wavefronts past max_chk: pruning with max_lag), nested bubbles, a self-loop, a 2-cycle and arcs that switch
+    strand, a segment nothing reaches, and an mgsim SV graph with queries from a few bases to 5 kb with ONT-like errors; plus
+    random queries and small max_ed (the s_term stop)."""
+    import ctypes as C
+    import random
+    from minigraph_b200 import options
+    ref = T.load_ref()
+    rng = random.Random(seed)
+    paths = _bridge_graphs(workdir, rng)
+    sv = os.path.join(workdir, "bridge_sv")
+    T.sim_graph(sv, 200000, 3, seed)
+    paths["sv"] = sv + ".gfa"
+    plan = {"chain1bp": (30, [40, 120], [0, 0.05, 0.15], [5, 30, 200]), "fanout40": (40, [60, 90], [0, 0.03, 0.1], [4, 30, 200]),
+            "wide": (12, [150, 250], [0.1, 0.2], [60, 120]), "nested": (30, [30, 100, 200], [0, 0.05, 0.15], [3, 30, 200]),
+            "cycles": (40, [20, 80, 200], [0, 0.05, 0.15], [2, 20, 200]), "sv": (30, [4, 300, 1500, 5000], [0.02, 0.08], [5, 100, 1000, 3000])}
+    seen, n_ok, n_all = {}, 0, 0
+    for tag, fn in paths.items():
+        n, lens, rates, max_eds = plan[tag]
+        G = _Graph(fn)
+        bridges = _draw_bridges(G, rng, max(4, n * scale // 4), lens, rates, max_eds)
+        if tag == "cycles":
+            sA, sZ, sL = G.names.index("sA") << 1, G.names.index("sZ") << 1, G.names.index("sL") << 1
+            bridges += [(G.seq[sZ >> 1][:20].encode(), sA, 3, sZ, 19, 100, None),  # nothing reaches sZ
+                        (G.seq[sA >> 1][5:15].encode(), sA, 5, sA, 14, 50, [sA]),  # the same vertex, off1 after off0
+                        ((G.seq[sA >> 1][20:] + G.vseq(sL) * 3 + G.vseq(sL)[:2]).encode(), sA, 20, sL, 1, 60, None),  # round the self-loop
+                        (G.vseq(sL)[4:].encode() + G.vseq(sL).encode() + G.vseq(sL)[:2].encode(), sL, 4, sL, 1, 40, None),  # off1 before off0 on one vertex
+                        (b"ACGTTGCA" * 3, sA, 24, sA ^ 1, 3, 200, None)]  # from the last base of a segment to its other strand
+        if tag == "fanout40":  # through an allele that occurs twice: two walks of the same cost, the reference keeps the first
+            fA, fB = G.names.index("fA"), G.names.index("fB")
+            for i in range(10):  # the allele as it is, or with its last base changed: one mismatch, or one insertion after the shorter allele
+                a = G.seq[i + 1] if i < 5 else G.seq[i + 1][:-1] + "ACGT"["CGTA".index(G.seq[i + 1][-1])]
+                bridges.append(((G.seq[fA][-10:] + a + G.seq[fB][:10]).encode(), fA << 1, len(G.seq[fA]) - 10, fB << 1, 9, 30, None))
+        bridges += [(bytes(rng.choices(b"ACGT", k=rng.choice([1, 3, 40, 400]))), rng.randrange(2 * len(G.seq)), 0, rng.randrange(2 * len(G.seq)), 0,
+                     rng.choice([3, 50, 500]), None) for _ in range(max(2, 6 * scale // 4))]  # random queries
+        g = ref.gfa_read(fn.encode())
+        es = ref.gfa_edseq_init(g)
+        want = [_ref_bridge(g, es, *b[:6]) for b in bridges]
+        pruned = [b[5] >= 60 and _ref_bridge(g, es, *b[:6], max_lag=-1) != w for b, w in zip(bridges, want)] if tag == "wide" else [False] * len(bridges)
+        ref.gfa_edseq_destroy(g.contents.n_seg, es)
+        ref.gfa_destroy(g)
+        eg = lib.mgb_gfa_read(fn.encode())
+        io, mo = options.opt_set("lr", True)
+        gi = lib.mg_index(eg, C.byref(io), 1, C.byref(mo))
+        assert gi, lib.mgb_last_error()
+        for mode in modes:
+            got = run_gwfa(lib, gi, mode, bridges)
+            for i, (b, w, r) in enumerate(zip(bridges, want, got)):
+                what = "%s bridge %d (mode %d, ql=%d, %d:%d -> %d:%d, max_ed %d)" % (tag, i, mode, len(b[0]), b[1], b[2], b[3], b[4], b[5])
+                assert r[0] == 0, what + ": rc %d" % r[0]
+                rs, rv, ro, rn, rw, ri = w
+                assert (r[1], r[2], r[3], r[6]) == (rs, rv, ro, ri), what + ": s/end_v/end_off/n_iter %r, the reference %r" % ((r[1], r[2], r[3], r[6]), (rs, rv, ro, ri))
+                assert (r[4], r[5]) == (rn, rw), what + ": walk %r, the reference %r" % (r[5][:12], rw[:12])
+        lib.mg_idx_destroy(gi)
+        lib.mgb_gfa_destroy(eg)
+        for b, w, p in zip(bridges, want, pruned):
+            s, walk = w[0], w[4]
+            n_all += 1
+            n_ok += s >= 0
+            marks = {tag + (" aligned" if s >= 0 else " not aligned")}
+            if s >= 0 and len(set(walk)) < len(walk):
+                marks.add("walk through a cycle")
+            if s >= 0 and len({x & 1 for x in walk}) == 2:
+                marks.add("walk switching strand")
+            if s >= 0 and any(x == y for x, y in zip(walk, walk[1:])):
+                marks.add("self-loop")
+            if b[1] == b[3]:
+                marks.add("v0 == v1, off1 %s off0" % ("after" if b[4] > b[2] else "before"))
+            if b[2] == len(G.seq[b[1] >> 1]) - 1:
+                marks.add("off0 on the last base")
+            if s < 0 and b[6] is not None:
+                marks.add("stopped at max_ed (s_term)")
+            if p:
+                marks.add("pruned")
+            if tag == "fanout40" and s >= 0 and any(G.seq[x >> 1] in G.seq[:x >> 1] + G.seq[(x >> 1) + 1:] or G.seq[x >> 1][:-1] in G.seq for x in walk[1:-1]):
+                marks.add("equal-cost walks")
+            if s >= 0 and len(b[0]) >= 4000:
+                marks.add("query of 4 kb or more")
+            if s >= 0 and len(b[0]) <= 5:
+                marks.add("query of 5 bases or fewer")
+            for m in marks:
+                seen[m] = seen.get(m, 0) + 1
+    assert n_ok >= n_all // 2, "only %d of %d bridges aligned" % (n_ok, n_all)
+    need = ["chain1bp aligned", "fanout40 aligned", "wide aligned", "nested aligned", "cycles aligned", "sv aligned", "cycles not aligned",
+            "walk through a cycle", "walk switching strand", "self-loop", "v0 == v1, off1 after off0", "v0 == v1, off1 before off0",
+            "off0 on the last base", "stopped at max_ed (s_term)", "pruned", "equal-cost walks", "query of 4 kb or more", "query of 5 bases or fewer"]
+    missing = [m for m in need if not seen.get(m)]
+    assert not missing, "situations that did not occur: %s (seen: %r)" % (missing, seen)
+    return seen
+
+
+def case_gwfa_rejects_bad_input(lib, workdir):
+    """an empty query or an end outside the graph is refused before anything runs"""
+    import ctypes as C
+    from minigraph_b200 import options
+    fn = os.path.join(workdir, "bridge_tiny.gfa")
+    _write_gfa(fn, [("a", "ACGTACGTAC"), ("b", "TTGCA")], [("a", "+", "b", "+")])
+    g = lib.mgb_gfa_read(fn.encode())
+    io, mo = options.opt_set("lr", True)
+    gi = lib.mg_index(g, C.byref(io), 1, C.byref(mo))
+    assert gi, lib.mgb_last_error()
+    for q, v0, off0, v1, off1 in ((b"", 0, 0, 2, 1), (b"ACG", 0, 10, 2, 1), (b"ACG", 0, 0, 2, 5), (b"ACG", 4, 0, 2, 1), (b"ACG", 0, -1, 2, 1)):
+        out, walk = (C.c_int64 * 6)(*[-7] * 6), (C.c_int32 * 4)()
+        one32, oneu = (lambda x: (C.c_int32 * 1)(x)), (lambda x: (C.c_uint32 * 1)(x))
+        rc = lib.mgb_test_gwfa(gi, 0, 1, q, (C.c_int64 * 1)(0), one32(len(q)), oneu(v0), one32(off0), oneu(v1), one32(off1), one32(10), out, walk, 4)
+        assert rc < 0 and list(out) == [-7] * 6, (q, v0, off0, v1, off1, rc)
+    lib.mg_idx_destroy(gi)
+    lib.mgb_gfa_destroy(g)

@@ -84,5 +84,14 @@ def test_exact_radix_sort_in_place_and_by_digit_walk(lib):
     cases.case_radix_exact(lib)
 
 
+@pytest.mark.parametrize("tier", [1, 2])
+def test_wfa_tier_limits(lib, tier):
+    cases.case_wfa_tier_edges(lib, tier, scale=2)
+
+
+def test_bridging_alignment(lib, workdir):
+    cases.case_gwfa_bridges(lib, workdir, scale=4)
+
+
 def test_rmq_chaining_with_interleaved_diagonals(lib, workdir):
     cases.case_tandem_diagonals(lib, workdir)
