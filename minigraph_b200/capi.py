@@ -128,7 +128,7 @@ _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def env_params():
-    """engine switches from the environment: MGB_PARAMS="wfa_v2=1,cta_len=1500" (pairs for mgb_set_param)"""
+    """engine parameters from the environment: MGB_PARAMS="lab_cache=0,arena_mb=4" (pairs for mgb_set_param)"""
     out = {}
     for kv in os.environ.get("MGB_PARAMS", "").split(","):
         if "=" in kv:

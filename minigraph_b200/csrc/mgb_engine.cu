@@ -43,26 +43,11 @@ static int64_t p_arena_mb = 3;
 static int64_t p_arena_big_mb = 1024; // per worker, retry pass
 static int64_t p_workers_per_sm = 32;
 static int64_t p_device = 0;
-static int64_t p_block_warps = 4;
 static int64_t p_host_threads = 0; // 0: min(16, hardware threads)
-static int64_t p_thread_mask = 0;      // bit s set: stage s runs one item per thread instead of one per warp (experiments)
 static int64_t p_slots = 3;            // mg_map_batch calls that may run at once on one index (each on its own slot: stream, buffers, arenas)
 static int64_t p_slot_workers = 0;
-static int64_t p_tier_learn = 1;       // 0: every gap tries every tier (no routing)
-static int64_t p_index_dev = 1;        // 0: the minimizer table is grouped and laid out on the host (std::sort) instead of on the device
-static int64_t p_gpu_lock = 1;         // 0: the kernels of concurrent calls may interleave on the device
-static int64_t p_pack2 = 1;            // 0: reads are uploaded as ASCII (1 byte per base) instead of 2 bits per base
 static int64_t p_lab_cache = 1;        // 0: graph chaining searches its walks per read instead of keeping per-source labels in HBM (mgb_gclabel.cuh)
 
-// launch shape per stage: warps per block and blocks per SM wanted (tunable for experiments: "sw<stage>", "mb<stage>")
-#ifndef MGB_BIG_MINB
-#define MGB_BIG_MINB 4 // blocks of k_wfa_big per SM (its register budget follows: 80 at 6, 96 at 5, 128 at 4)
-#endif
-#ifndef MGB_GWFA_MINB
-#define MGB_GWFA_MINB 4
-#endif
-static int STAGE_MINB[20] = { 8, 2, 8, 8, 5, 8, 7, MGB_BIG_MINB, MGB_GWFA_MINB, 4, 0, 0, 0, 0, 0, 0, 0, 8, 8, 2 }; // indexed by stage number (10-16 unused)
-static int STAGE_WARPS[20] = { 4, 7, 4, 4, 4, 4, 2, 4, 4, 4, 0, 0, 0, 0, 0, 0, 0, 4, 4, 6 }; // k_chain: 2 x 7 slices of 16 KB per SM, k_chain_rescue: 2 x 6 of 18 KB
 extern "C" const char *mgb_last_error(void) { return g_last_error.c_str(); }
 extern "C" const char *mgb_version(void) { return "mgb200-r1"; }
 extern "C" int mgb_set_param(const char *key, int64_t value)
@@ -71,18 +56,10 @@ extern "C" int mgb_set_param(const char *key, int64_t value)
 	else if (!strcmp(key, "arena_big_mb")) p_arena_big_mb = value;
 	else if (!strcmp(key, "workers_per_sm")) p_workers_per_sm = value;
 	else if (!strcmp(key, "device")) p_device = value;
-	else if (!strcmp(key, "block_warps")) p_block_warps = value;
 	else if (!strcmp(key, "host_threads")) p_host_threads = value;
-	else if (!strcmp(key, "thread_mask")) p_thread_mask = value;
 	else if (!strcmp(key, "slots")) p_slots = value;
 	else if (!strcmp(key, "slot_workers")) p_slot_workers = value;
 	else if (!strcmp(key, "lab_cache")) p_lab_cache = value;
-	else if (!strcmp(key, "pack2")) p_pack2 = value;
-	else if (!strcmp(key, "gpu_lock")) p_gpu_lock = value;
-	else if (!strcmp(key, "index_dev")) p_index_dev = value;
-	else if (!strcmp(key, "tier_learn")) p_tier_learn = value;
-	else if (!strncmp(key, "sw", 2) && key[2] >= '0' && key[2] <= '9' && !key[3] && value >= 1 && value <= 4) STAGE_WARPS[key[2] - '0'] = (int)value;
-	else if (!strncmp(key, "mb", 2) && key[2] >= '0' && key[2] <= '9' && !key[3] && value >= 1 && value <= 32) STAGE_MINB[key[2] - '0'] = (int)value;
 	else return -1;
 	return 0;
 }
@@ -191,33 +168,39 @@ struct LaunchArgs {
 	char *arena_base;
 	uint64_t arena_bytes;
 	uint64_t *arena_peak;    // per worker
-	int64_t job_start;       // first job of this launch (stage 4)
-	int thread_mode;         // 1: one item per thread (stage_loop_thread)
+	int64_t job_start;       // first job of this launch (bridging jobs, tier-1 gap jobs)
 	// segment sketch (index build)
 	Pool *pool_mz; u128 *mz;
 };
 
-// stages: 0 seed (K1-K3), 1 chain (K4/K5), 2 graph chaining DP + bridge plan (K6), 8 bridging jobs (K7a), 9 graph-chain
-//         materialisation + alignment plan (K7b), 4/6/7 WFA jobs tier 1/2/3 (K8a), 5 finish: CIGAR stitching + ds + result
-//         blob (K8b), 3 segment sketch for the index, 17 reachability labels of the sources graph chaining asks for (one per thread)
-#define MGB_IS_WFA(STAGE) ((STAGE) == 4 || (STAGE) == 6 || (STAGE) == 7)
-#define MGB_IS_WARP(STAGE) (MGB_IS_WFA(STAGE) || (STAGE) == 8 || (STAGE) == 1 || (STAGE) == 2 || (STAGE) == 0 || (STAGE) == 5 || (STAGE) == 9 || (STAGE) == 19) // stages entered by all lanes of the warp
-template<int STAGE>
+// The stages of the pipeline, one kernel each (the table behind stage_loop_thread()).  Stages 0-9 index mgb_stats_t.t_kernel_ms
+// and capi.KERNEL_NAMES.
+enum Stage { S_SEED = 0, S_CHAIN = 1, S_GCHAIN = 2, S_INDEX_SKETCH = 3, S_WFA_SMALL = 4, S_FINISH = 5, S_WFA_MID = 6, S_WFA_BIG = 7, S_GWFA = 8,
+             S_GCHAIN_GEN = 9, S_LABELS = 10, S_LABELS_BIG = 11, S_CHAIN_RESCUE = 12 };
+// How one item of a stage runs: entered by all lanes of the warp, by lane 0 alone (with the warp's arena), or one item per
+// thread (with 1/32 of the warp's arena)
+enum class ItemMode { WARP, LANE0, THREAD };
+// Where a failed item is recorded: on its read, found as the item itself, as rescue_list[item], through its bridging job or
+// through its gap job of tier 1/2/3; in the one status word of the index build; or nowhere
+enum class FailTo { READ, RESCUE_LIST, BRIDGE_JOB, GAP_JOB_T1, GAP_JOB_T2, GAP_JOB_T3, INDEX_STATUS, NOWHERE };
+template<int S> struct StageSpec;
+
+template<int S>
 MG_HD inline int run_stage(const LaunchArgs &L, int item, Arena &A, int lane, int32_t *smem)
 {
-	if (STAGE == 0) return stage_seed(L.c, item, A, lane, smem);
-	if (STAGE == 1) return stage_chain<0>(L.c, item, A, lane, smem);
-	if (STAGE == 19) return stage_chain<1>(L.c, L.c.rescue_list[item], A, lane, smem); // the reads k_chain listed
-	if (STAGE == 2) return stage_gchain(L.c, L.routs, item, A, lane);
-	if (STAGE == 17) return label_job(A, L.c.g, L.c.lab, item, 0);
-	if (STAGE == 18) return label_job(A, L.c.g, L.c.lab, item, 1); // lane 0 with the whole arena of its warp
-	if (STAGE == 5) return stage_finish(L.c, L.routs, item, A, lane);
-	if (STAGE == 8) return gwfa_job_run(A, L.c, L.job_start + item, lane, smem);
-	if (STAGE == 9) return stage_gchain_gen(L.c, L.routs, item, A, lane);
-	if (STAGE == 4) return wfa_job_run(A, L.c, L.job_start + item, lane, smem, 1);
-	if (STAGE == 6) return wfa_job_run(A, L.c, L.c.jobq[0][item], lane, smem, 2);
-	if (STAGE == 7) return wfa_job_run(A, L.c, L.c.jobq[1][item], lane, smem, 3);
-	if (STAGE == 3) { // sketch one graph segment for the index (reference: index.c:200-205)
+	if (S == S_SEED) return stage_seed(L.c, item, A, lane, smem);
+	if (S == S_CHAIN) return stage_chain<0>(L.c, item, A, lane, smem);
+	if (S == S_CHAIN_RESCUE) return stage_chain<1>(L.c, L.c.rescue_list[item], A, lane, smem); // the reads k_chain listed
+	if (S == S_GCHAIN) return stage_gchain(L.c, L.routs, item, A, lane);
+	if (S == S_LABELS) return label_job(A, L.c.g, L.c.lab, item, 0);
+	if (S == S_LABELS_BIG) return label_job(A, L.c.g, L.c.lab, item, 1); // lane 0 with the whole arena of its warp
+	if (S == S_FINISH) return stage_finish(L.c, L.routs, item, A, lane);
+	if (S == S_GWFA) return gwfa_job_run(A, L.c, L.job_start + item, lane, smem);
+	if (S == S_GCHAIN_GEN) return stage_gchain_gen(L.c, L.routs, item, A, lane);
+	if (S == S_WFA_SMALL) return wfa_job_run(A, L.c, L.job_start + item, lane, smem, 1);
+	if (S == S_WFA_MID) return wfa_job_run(A, L.c, L.c.jobq[0][item], lane, smem, 2);
+	if (S == S_WFA_BIG) return wfa_job_run(A, L.c, L.c.jobq[1][item], lane, smem, 3);
+	if (S == S_INDEX_SKETCH) { // sketch one graph segment for the index (reference: index.c:200-205)
 		AVec<u128> mv;
 		avec_init(mv);
 		int32_t len = L.c.g.seg_len[item];
@@ -233,11 +216,12 @@ MG_HD inline int run_stage(const LaunchArgs &L, int item, Arena &A, int lane, in
 }
 
 // record a failure: per read for the mapping stages, a single status word for the index build
-template<int STAGE>
+template<int S>
 MG_HD inline void stage_fail(const LaunchArgs &L, int item, int rc)
 {
-	if (STAGE == 17 || STAGE == 18) return; // a source that could not be finished is searched again by the read that needs it
-	if (STAGE == 3) {
+	constexpr FailTo f = StageSpec<S>::fail;
+	if (f == FailTo::NOWHERE) return; // (labels) a source that could not be finished is searched again by the read that needs it
+	if (f == FailTo::INDEX_STATUS) {
 #if MGB_ON_DEVICE
 		atomicMin((int*)L.routs, rc);
 #else
@@ -245,48 +229,48 @@ MG_HD inline void stage_fail(const LaunchArgs &L, int item, int rc)
 #endif
 		return;
 	}
-	int rid = STAGE == 8? L.c.gjobs[L.job_start + item].rid : STAGE == 4? L.c.jobs[L.job_start + item].rid : STAGE == 6? L.c.jobs[L.c.jobq[0][item]].rid : STAGE == 7? L.c.jobs[L.c.jobq[1][item]].rid : STAGE == 19? L.c.rescue_list[item] : item;
+	int rid = f == FailTo::BRIDGE_JOB? L.c.gjobs[L.job_start + item].rid : f == FailTo::GAP_JOB_T1? L.c.jobs[L.job_start + item].rid : f == FailTo::GAP_JOB_T2? L.c.jobs[L.c.jobq[0][item]].rid
+			: f == FailTo::GAP_JOB_T3? L.c.jobs[L.c.jobq[1][item]].rid : f == FailTo::RESCUE_LIST? L.c.rescue_list[item] : item;
 	L.c.meta[rid].status = rc; // benign race between jobs of one read: any negative code triggers the redo
-	if (STAGE == 2 || MGB_IS_WARP(STAGE) || STAGE == 5 || STAGE == 9) L.routs[rid].status = rc;
+	L.routs[rid].status = rc;
 }
 
 #ifndef MGB_HOSTSIM
 // One warp per work item; items are pulled from a global counter so that long items do not stall a wave.
 // Every mapping stage is warp-uniform (all lanes enter the stage function, see mgb_common.cuh).
-template<int STAGE>
+template<int S>
 __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 {
+	typedef StageSpec<S> Spec;
 	const int lane = threadIdx.x & 31;
 	const int worker = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
 	Arena A;
 	arena_init(A, L.arena_base + (uint64_t)worker * L.arena_bytes, L.arena_bytes);
 	extern __shared__ int4 dyn_smem[];
-	const int smem_stride = STAGE == 4? WfTier1::STRIDE : STAGE == 6? WfTier2::STRIDE : STAGE == 0? SKETCH_SMEM_BYTES : STAGE == 8? GWFA_SMEM_ARENA : STAGE == 1? CHAIN_SMEM_BYTES : STAGE == 19? CHAIN_RESCUE_SMEM_BYTES : 0;
-	int32_t *smem = smem_stride? (int32_t*)((char*)dyn_smem + (size_t)(threadIdx.x >> 5) * smem_stride) : 0;
-	if (STAGE == 1 || STAGE == 19) chain_smem_init(smem, lane);
-	if ((STAGE == 4 || STAGE == 6) && lane == 0) { unsigned long long *ck = wfa_cig_chunk(smem, STAGE == 4? 1 : 2); ck[0] = ck[1] = 0; } // no slice of the CIGAR pool yet
+	int32_t *smem = Spec::smem? (int32_t*)((char*)dyn_smem + (size_t)(threadIdx.x >> 5) * Spec::smem) : 0;
+	if (S == S_CHAIN || S == S_CHAIN_RESCUE) chain_smem_init(smem, lane);
+	if ((S == S_WFA_SMALL || S == S_WFA_MID) && lane == 0) { unsigned long long *ck = wfa_cig_chunk(smem, S == S_WFA_SMALL? 1 : 2); ck[0] = ck[1] = 0; } // no slice of the CIGAR pool yet
 	prof_block_begin();
 	const int n_work = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
-	const int grab = STAGE == 4 || STAGE == 6? 4 : 1; // the short jobs of the on-chip WFA tiers are taken four at a time: one contended ticket per four jobs
 	int next_item = 0, have = 0;
 	for (;;) {
 		if (have == 0) {
-			if (lane == 0) next_item = (int)atomicAdd(L.c.next_read, (unsigned int)grab);
+			if (lane == 0) next_item = (int)atomicAdd(L.c.next_read, (unsigned int)Spec::grab);
 			next_item = __shfl_sync(0xffffffffu, next_item, 0);
-			have = grab;
+			have = Spec::grab;
 		}
 		int item = next_item++;
 		--have;
 		if (item >= n_work) break;
 		if (L.rid_list) item = L.rid_list[item];
-		if (MGB_IS_WARP(STAGE)) {
+		if (Spec::mode == ItemMode::WARP) {
 			A.top = 0;
-			int rc = run_stage<STAGE>(L, item, A, lane, smem);
-			if (rc < 0 && lane == 0) stage_fail<STAGE>(L, item, rc);
+			int rc = run_stage<S>(L, item, A, lane, smem);
+			if (rc < 0 && lane == 0) stage_fail<S>(L, item, rc);
 		} else if (lane == 0) {
 			A.top = 0;
-			int rc = run_stage<STAGE>(L, item, A, 0, 0);
-			if (rc < 0) stage_fail<STAGE>(L, item, rc);
+			int rc = run_stage<S>(L, item, A, 0, 0);
+			if (rc < 0) stage_fail<S>(L, item, rc);
 		}
 		__syncwarp();
 	}
@@ -297,7 +281,7 @@ __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 // Thread-per-item variant for the stages whose control flow is sequential: every THREAD pulls its own item and owns
 // 1/32 of the warp's arena.  The 32 lanes of a warp diverge completely, but the hardware interleaves the diverged
 // lanes, so 32x more items are in flight per warp and their memory latencies overlap.
-template<int STAGE>
+template<int S>
 __device__ __forceinline__ void stage_loop_thread(const LaunchArgs &L)
 {
 	const int lane = threadIdx.x & 31;
@@ -312,44 +296,50 @@ __device__ __forceinline__ void stage_loop_thread(const LaunchArgs &L)
 		if (item >= n_work) break;
 		if (L.rid_list) item = L.rid_list[item];
 		A.top = 0;
-		int rc = run_stage<STAGE>(L, item, A, -1, 0);
-		if (rc < 0) stage_fail<STAGE>(L, item, rc);
+		int rc = run_stage<S>(L, item, A, -1, 0);
+		if (rc < 0) stage_fail<S>(L, item, rc);
 	}
 	if (L.arena_peak) atomicMax((unsigned long long*)&L.arena_peak[worker], (unsigned long long)A.peak);
 	prof_block_end(L.c.prof);
 }
-
-// named entry points (one per stage, so that profiles read well); blocks of 4 warps, MINB blocks per SM wanted
-#define MGB_KERNEL_T(name, STAGE, THREADS, MINB) __global__ void __launch_bounds__(THREADS, MINB) name(LaunchArgs L) { if (!MGB_IS_WARP(STAGE) && L.thread_mode) stage_loop_thread<STAGE>(L); else stage_loop<STAGE>(L); } // (no thread-per-item copy of the warp-wide stages in the kernel)
-#define MGB_KERNEL(name, STAGE, MINB) MGB_KERNEL_T(name, STAGE, 128, MINB)
-MGB_KERNEL(k_seed, 0, 8)          // K1-K3: sketch, index lookup, seed sort
-MGB_KERNEL_T(k_chain, 1, 224, 2)         // K4/K5: linear chaining on chip (seeds bulk-loaded into shared memory)
-MGB_KERNEL_T(k_chain_rescue, 19, 192, 2) // K5: long-join rescue (RMQ chaining) of the reads k_chain listed
-MGB_KERNEL(k_gchain, 2, 8)        // K6: graph chaining DP + k-shortest walks, overlap resolution, bridging plan
-MGB_KERNEL(k_gwfa, 8, MGB_GWFA_MINB)          // K7a: bridging alignments (graph wavefront), one warp per bridge
-MGB_KERNEL(k_gchain_gen, 9, 4)    // K7b: graph-chain materialisation, post filters, mapq, alignment plan
-MGB_KERNEL(k_index_sketch, 3, 8)  // index build: sketch of graph segments
-MGB_KERNEL(k_wfa_small, 4, 5)     // K8a tier 1: small gaps, wavefronts + traceback bytes in shared memory
-MGB_KERNEL(k_wfa_mid, 6, 5)       // K8a tier 2: mid-size gaps, wavefronts in shared memory (blocks of 2 warps)
-MGB_KERNEL(k_wfa_big, 7, MGB_BIG_MINB) // K8a tier 3: anything else, wavefronts in the worker arena
-MGB_KERNEL(k_finish, 5, 8)        // K8b: CIGAR stitching, ds strings, result blobs
-MGB_KERNEL(k_gc_labels, 17, 8)    // reachability labels of new source vertices, one search per thread (mgb_gclabel.cuh)
-MGB_KERNEL(k_gc_labels_big, 18, 8) // the few sources whose search outgrew a thread's share of the arena: one per warp
-template<int STAGE> struct StageKernel;
-template<> struct StageKernel<0> { static void (*get())(LaunchArgs) { return k_seed; } };
-template<> struct StageKernel<1> { static void (*get())(LaunchArgs) { return k_chain; } };
-template<> struct StageKernel<2> { static void (*get())(LaunchArgs) { return k_gchain; } };
-template<> struct StageKernel<3> { static void (*get())(LaunchArgs) { return k_index_sketch; } };
-template<> struct StageKernel<4> { static void (*get())(LaunchArgs) { return k_wfa_small; } };
-template<> struct StageKernel<6> { static void (*get())(LaunchArgs) { return k_wfa_mid; } };
-template<> struct StageKernel<7> { static void (*get())(LaunchArgs) { return k_wfa_big; } };
-template<> struct StageKernel<8> { static void (*get())(LaunchArgs) { return k_gwfa; } };
-template<> struct StageKernel<9> { static void (*get())(LaunchArgs) { return k_gchain_gen; } };
-template<> struct StageKernel<5> { static void (*get())(LaunchArgs) { return k_finish; } };
-template<> struct StageKernel<19> { static void (*get())(LaunchArgs) { return k_chain_rescue; } };
-template<> struct StageKernel<17> { static void (*get())(LaunchArgs) { return k_gc_labels; } };
-template<> struct StageKernel<18> { static void (*get())(LaunchArgs) { return k_gc_labels_big; } };
 #endif
+
+// One row per stage: its kernel (named, so that profiles read well), warps per block, blocks per SM wanted, bytes of shared
+// memory per warp, items taken per ticket of the work counter (the short jobs of the on-chip WFA tiers four at a time: one
+// contended ticket per four jobs), how an item runs and where a failure is recorded.  The kernel's __launch_bounds__ are its
+// launch shape; MGB_STAGE_BOUNDS gives a kernel bounds of its own.
+#define MGB_STAGE(KERNEL, S, WARPS, MINB, SMEM, GRAB, MODE, FAIL) MGB_STAGE_BOUNDS(KERNEL, S, WARPS, MINB, SMEM, GRAB, MODE, FAIL, (WARPS) * 32, MINB)
+#ifdef MGB_HOSTSIM
+#define MGB_STAGE_KERNEL(KERNEL, S)
+#else
+#define MGB_STAGE_KERNEL(KERNEL, S) \
+	__global__ void __launch_bounds__(StageSpec<S>::bound_threads, StageSpec<S>::bound_minb) KERNEL(LaunchArgs L) \
+	{ if constexpr (StageSpec<S>::mode == ItemMode::THREAD) stage_loop_thread<S>(L); else stage_loop<S>(L); } \
+	void (*StageSpec<S>::kernel())(LaunchArgs) { return KERNEL; }
+#endif
+#define MGB_STAGE_BOUNDS(KERNEL, S, WARPS, MINB, SMEM, GRAB, MODE, FAIL, BOUND_THREADS, BOUND_MINB) \
+	template<> struct StageSpec<S> { \
+		static constexpr int warps = WARPS, minb = MINB, smem = SMEM, grab = GRAB, bound_threads = BOUND_THREADS, bound_minb = BOUND_MINB; \
+		static constexpr ItemMode mode = ItemMode::MODE; static constexpr FailTo fail = FailTo::FAIL; static void (*kernel())(LaunchArgs); \
+	}; \
+	MGB_STAGE_KERNEL(KERNEL, S)
+
+//        kernel           stage           warps blocks shared memory per warp   grab  item   failure
+MGB_STAGE(k_seed,          S_SEED,         4,    8,     SKETCH_SMEM_BYTES,       1,    WARP,  READ)         // K1-K3: sketch, index lookup, seed sort
+MGB_STAGE(k_chain,         S_CHAIN,        7,    2,     CHAIN_SMEM_BYTES,        1,    WARP,  READ)         // K4/K5: linear chaining on chip (seeds bulk-loaded into shared memory), 2 x 7 slices of 16 KB per SM
+MGB_STAGE(k_chain_rescue,  S_CHAIN_RESCUE, 6,    2,     CHAIN_RESCUE_SMEM_BYTES, 1,    WARP,  RESCUE_LIST)  // K5: long-join rescue (RMQ chaining) of the reads k_chain listed, 2 x 6 slices of 18 KB per SM
+MGB_STAGE(k_gchain,        S_GCHAIN,       4,    8,     0,                       1,    WARP,  READ)         // K6: graph chaining DP + k-shortest walks, overlap resolution, bridging plan
+MGB_STAGE(k_gwfa,          S_GWFA,         4,    4,     GWF_SHARED_BYTES,        1,    WARP,  BRIDGE_JOB)   // K7a: bridging alignments (graph wavefront), one warp per bridge
+MGB_STAGE(k_gchain_gen,    S_GCHAIN_GEN,   4,    4,     0,                       1,    WARP,  READ)         // K7b: graph-chain materialisation, post filters, mapq, alignment plan
+MGB_STAGE(k_index_sketch,  S_INDEX_SKETCH, 4,    8,     0,                       1,    LANE0, INDEX_STATUS) // index build: sketch of graph segments
+MGB_STAGE(k_wfa_small,     S_WFA_SMALL,    4,    5,     WfTier1::STRIDE,         4,    WARP,  GAP_JOB_T1)   // K8a tier 1: small gaps, wavefronts + traceback bytes in shared memory
+// K8a tier 2: mid-size gaps, wavefronts in shared memory.  The one kernel whose bounds (128 threads, 5 blocks per SM) are not its
+// launch shape (2 warps, 7 blocks per SM); it compiles to 79 registers under them.
+MGB_STAGE_BOUNDS(k_wfa_mid, S_WFA_MID,     2,    7,     WfTier2::STRIDE,         4,    WARP,  GAP_JOB_T2, 128, 5)
+MGB_STAGE(k_wfa_big,       S_WFA_BIG,      4,    4,     0,                       1,    WARP,  GAP_JOB_T3)   // K8a tier 3: anything else, wavefronts in the worker arena (128 registers at 4 blocks per SM)
+MGB_STAGE(k_finish,        S_FINISH,       4,    8,     0,                       1,    WARP,  READ)         // K8b: CIGAR stitching, ds strings, result blobs
+MGB_STAGE(k_gc_labels,     S_LABELS,       4,    8,     0,                       1,    THREAD, NOWHERE)     // reachability labels of new source vertices, one search per thread (mgb_gclabel.cuh)
+MGB_STAGE(k_gc_labels_big, S_LABELS_BIG,   4,    8,     0,                       1,    LANE0, NOWHERE)      // the few sources whose search outgrew a thread's share of the arena: one per warp
 
 // Longest-first order of a job list (a tail of a few long jobs otherwise decides the kernel time).  Jobs are binned by
 // size, four bins per octave, largest first; the order inside a bin does not matter (results do not depend on it).
@@ -602,29 +592,31 @@ struct Workers {
 	uint64_t *peak;
 };
 
-template<int STAGE>
-static void launch_stage(LaunchArgs &L, const Workers &W, int warps_override = 0)
+template<int S>
+static void launch_stage(LaunchArgs &L, const Workers &W)
 {
+	typedef StageSpec<S> Spec;
 	L.arena_base = W.arena, L.arena_bytes = W.arena_bytes, L.arena_peak = W.peak;
 	dzero(L.c.next_read, sizeof(unsigned int)); // in stream order: no host round trip per launch
 #ifdef MGB_HOSTSIM
 	Arena A;
-	arena_init(A, W.arena, STAGE == 17? (W.arena_bytes / 32) & ~(uint64_t)15 : W.arena_bytes); // one item per thread: a thread's share, as on the device
-	std::vector<int32_t> sim_smem(std::max<size_t>(std::max<size_t>(WfTier1::STRIDE, WfTier2::STRIDE), std::max<size_t>(std::max<size_t>(GWFA_SMEM_ARENA, CHAIN_RESCUE_SMEM_BYTES), SKETCH_SMEM_BYTES)) / 4);
-	if (STAGE == 1 || STAGE == 19) { mbar_init((uint64_t*)sim_smem.data(), 1); sim_smem[2] = 0; }
+	arena_init(A, W.arena, Spec::mode == ItemMode::THREAD? (W.arena_bytes / 32) & ~(uint64_t)15 : W.arena_bytes); // one item per thread: a thread's share, as on the device
+	std::vector<int32_t> sim_smem(Spec::smem / 4);
+	int32_t *smem = Spec::mode == ItemMode::WARP && Spec::smem? sim_smem.data() : 0; // the slice of one warp, as on the device
+	if (S == S_CHAIN || S == S_CHAIN_RESCUE) { mbar_init((uint64_t*)smem, 1); smem[2] = 0; }
 	const int n_work_sim = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
 	for (int it = 0; it < n_work_sim; ++it) {
 		int item = L.rid_list? L.rid_list[it] : it;
 		A.top = 0;
 		int rc;
 #if MGB_W > 1
-		if (MGB_IS_WARP(STAGE)) { // all lanes of the simulated warp enter, each with its own copy of the arena header (as in registers on the device)
+		if (Spec::mode == ItemMode::WARP) { // all lanes of the simulated warp enter, each with its own copy of the arena header (as in registers on the device)
 			int rcs[MGB_W];
 			uint64_t peaks[MGB_W];
-			sim::tag()[0] = STAGE, sim::tag()[1] = item;
+			sim::tag()[0] = S, sim::tag()[1] = item;
 			sim::run_warp(MGB_W, [&](int lane) {
 				Arena Al = A;
-				rcs[lane] = run_stage<STAGE>(L, item, Al, lane, sim_smem.data());
+				rcs[lane] = run_stage<S>(L, item, Al, lane, smem);
 				peaks[lane] = Al.peak;
 			});
 			rc = rcs[0];
@@ -632,24 +624,17 @@ static void launch_stage(LaunchArgs &L, const Workers &W, int warps_override = 0
 			for (int l = 0; l < MGB_W; ++l) if (peaks[l] > A.peak) A.peak = peaks[l];
 		} else
 #endif
-		rc = run_stage<STAGE>(L, item, A, 0, MGB_IS_WARP(STAGE)? sim_smem.data() : 0);
-		if (rc < 0 && getenv("MGB_HOSTSIM_TRACE")) fprintf(stderr, "[hostsim] stage %d item %d failed with %d\n", STAGE, item, rc);
-		if (rc < 0) stage_fail<STAGE>(L, item, rc);
+		rc = run_stage<S>(L, item, A, 0, smem);
+		if (rc < 0 && getenv("MGB_HOSTSIM_TRACE")) fprintf(stderr, "[hostsim] stage %d item %d failed with %d\n", S, item, rc);
+		if (rc < 0) stage_fail<S>(L, item, rc);
 	}
 	if (W.peak && A.peak > W.peak[0]) W.peak[0] = A.peak;
 #else
-	const int warps = warps_override > 0? warps_override : STAGE_WARPS[STAGE], threads = warps * 32;
-	int want = dev_sm_count() * STAGE_MINB[STAGE] * STAGE_WARPS[STAGE]; // resident warps this stage can keep on the chip
-	int n_w = std::min(W.n_workers, want);
-	int blocks = std::max(1, n_w / warps);
-	size_t smem = STAGE == 4? (size_t)warps * WfTier1::STRIDE : STAGE == 6? (size_t)warps * WfTier2::STRIDE : STAGE == 0? (size_t)warps * SKETCH_SMEM_BYTES : STAGE == 8? (size_t)warps * GWFA_SMEM_ARENA : STAGE == 1? (size_t)warps * CHAIN_SMEM_BYTES : STAGE == 19? (size_t)warps * CHAIN_RESCUE_SMEM_BYTES : 0;
-	void (*kern)(LaunchArgs) = StageKernel<STAGE>::get();
-	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	L.thread_mode = (p_thread_mask >> STAGE) & 1;
-	if (MGB_IS_WARP(STAGE)) L.thread_mode = 0;
-	if (STAGE == 17) L.thread_mode = 1;
-	if (L.thread_mode) smem = 0;
-	kern<<<blocks, threads, smem, t_stream>>>(L);
+	const int n_w = std::min(W.n_workers, dev_sm_count() * Spec::minb * Spec::warps); // resident warps this stage can keep on the chip
+	const int blocks = std::max(1, n_w / Spec::warps);
+	const size_t smem = (size_t)Spec::warps * Spec::smem;
+	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(Spec::kernel(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	Spec::kernel()<<<blocks, Spec::warps * 32, smem, t_stream>>>(L);
 	CUDA_OK(cudaGetLastError());
 #endif
 }
@@ -825,8 +810,10 @@ static Model *model_build(gfa_t *g, int k, int w)
 	M->g.arc = dalloc_copy(M->arc), M->dev_ptrs.push_back((void*)M->g.arc);
 	M->ix.k = k, M->ix.w = w, M->ix.slot = 0, M->ix.pos = 0, M->ix.n_slots_mask = 0;
 
-	// sketch every segment on the device (K1 reused), then build the table on the host
+	// sketch every segment on the device (K1 reused), then build the table: on the device (the simulators: on the host)
+#ifdef MGB_HOSTSIM
 	std::vector<u128> mz;
+#endif
 	{
 		uint64_t tot_len = 0;
 		int32_t max_len = 1;
@@ -851,7 +838,7 @@ static Model *model_build(gfa_t *g, int k, int w)
 			memset(&L, 0, sizeof(L));
 			L.c.g = M->g, L.c.ix = M->ix, L.c.next_read = d_next;
 			L.routs = (ReadOut*)d_status, L.rid_list = 0, L.n_work = (int32_t)n_seg, L.pool_mz = d_pool, L.mz = d_mz;
-			launch_stage<3>(L, M->W);
+			launch_stage<S_INDEX_SKETCH>(L, M->W);
 			dsync();
 			d2h(&st0, d_status, sizeof(int));
 			d2h(&hp, d_pool, sizeof(Pool));
@@ -860,7 +847,7 @@ static Model *model_build(gfa_t *g, int k, int w)
 			else if (st0 == MGB_E_ARENA) arena_b *= 2, nw = std::max(1, nw / 2), retry = true;
 			else if (st0 < 0) { set_error("segment sketch failed with code " + std::to_string(st0)); throw MgbError{st0}; }
 #ifndef MGB_HOSTSIM
-			if (!retry && p_index_dev) { // group, lay out and insert on the device (mgb_index.cuh)
+			if (!retry) { // group, lay out and insert on the device (mgb_index.cuh)
 				DevIndexOut out;
 				dfree(M->W.arena), dfree(M->W.peak); // the sketch arenas are not needed again; the sort wants the memory
 				memset(&M->W, 0, sizeof(Workers));
@@ -872,15 +859,17 @@ static Model *model_build(gfa_t *g, int k, int w)
 				M->dev_ptrs.push_back((void*)out.slot), M->dev_ptrs.push_back((void*)out.pos);
 				return M;
 			}
-#endif
+#else
 			if (!retry) {
 				mz.resize(hp.used / sizeof(u128));
 				d2h(mz.data(), d_mz, hp.used);
 			}
+#endif
 			dfree(d_pool), dfree(d_mz), dfree(d_status), dfree(d_next);
 			if (!retry) break;
 		}
 	}
+#ifdef MGB_HOSTSIM
 	// the sketch arenas are not needed again (every mapping slot owns its arenas)
 	dfree(M->W.arena), dfree(M->W.peak);
 	memset(&M->W, 0, sizeof(Workers));
@@ -912,6 +901,7 @@ static Model *model_build(gfa_t *g, int k, int w)
 	M->ix.n_slots_mask = M->n_slots_mask;
 	M->ix.slot = dalloc_copy(M->slot), M->dev_ptrs.push_back((void*)M->ix.slot);
 	M->ix.pos = dalloc_copy(M->pos), M->dev_ptrs.push_back((void*)M->ix.pos);
+#endif
 	return M;
 }
 
@@ -1007,7 +997,7 @@ extern "C" mg_idx_t *mg_index(gfa_t *g, const mg_idxopt_t *io, int n_threads, mg
 	Model *M = 0;
 	try { M = model_build(g, k, w); } catch (const MgbError &) { return 0; }
 	M->device = devs[0];
-	if (devs.size() > 1) { // every further device builds its own copy (sketch on that device, table on the host), all at once
+	if (devs.size() > 1) { // every further device builds its own copy, all at once
 		M->peers.resize(devs.size() - 1, (Model*)0);
 		std::vector<std::thread> th;
 		for (size_t i = 1; i < devs.size(); ++i)
@@ -1246,7 +1236,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	// The reads go up 2 bits per base (a quarter of the bytes) and k_unpack writes their ASCII copy on the device; a read with any
 	// byte other than A/C/G/T goes up as ASCII, and so does the whole batch when such reads are many or the fragments have segments.
 	uint64_t *pk_off = 0, *d_pk = 0, *d_pk_off = 0;
-	bool packed_mode = p_pack2 && seg_off == 0;
+	bool packed_mode = seg_off == 0;
 	if (packed_mode) {
 		pk_off = (uint64_t*)sl.h_pk.ensure((size_t)n_reads * 8 + 64 + (size_t)(S.n_bases / 4) + (size_t)n_reads * 16);
 		uint64_t wtot = 0;
@@ -1432,38 +1422,38 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 			if (first_kernel) { CUDA_OK(cudaEventRecord(sl.ev_first, t_stream)); first_kernel = false; }
 #endif
 			if (timed) tm_seed.start();
-			{ if (timed) tm_k[0].start(); launch_stage<0>(L, W); if (timed) tm_k[0].stop(); }
+			{ if (timed) tm_k[S_SEED].start(); launch_stage<S_SEED>(L, W); if (timed) tm_k[S_SEED].stop(); }
 			if (timed) tm_seed.stop(), tm_chain.start();
 			{
-				if (timed) tm_k[1].start();
+				if (timed) tm_k[S_CHAIN].start();
 				dzero(d_rescue_n, sizeof(unsigned int));
-				launch_stage<1>(L, W);
+				launch_stage<S_CHAIN>(L, W);
 				L.n_work_dev = d_rescue_n, L.rid_list = 0; // the reads k_chain put on the rescue list (count known on the device only)
-				launch_stage<19>(L, W);
+				launch_stage<S_CHAIN_RESCUE>(L, W);
 				L.n_work_dev = 0, L.rid_list = d_list;
-				if (timed) tm_k[1].stop();
+				if (timed) tm_k[S_CHAIN].stop();
 				S.n_launches += 1;
 			}
 			if (timed) tm_chain.stop(), tm_align.start();
 			if (use_lab) { // labels of the sources k_chain listed (count known on the device only)
 				L.n_work_dev = d_lab_n, L.rid_list = 0;
 				if (timed) tm_lab.start();
-				launch_stage<17>(L, W);
+				launch_stage<S_LABELS>(L, W);
 				L.n_work_dev = d_lab_n + 1;
-				launch_stage<18>(L, W);
+				launch_stage<S_LABELS_BIG>(L, W);
 				if (timed) tm_lab.stop();
 				L.n_work_dev = 0, L.rid_list = d_list;
 				S.n_launches += 2;
 			}
 			if (d_list == 0 && n_list >= 1024) { // whole batch: reads with many linear chains first (a few of them set the time of this kernel)
-				if (timed) tm_k[2].start();
+				if (timed) tm_k[S_GCHAIN].start();
 				make_job_order(L, 2, 0, n_list, order_buf);
 				L.rid_list = order_buf;
-				launch_stage<2>(L, W);
+				launch_stage<S_GCHAIN>(L, W);
 				L.rid_list = d_list;
-				if (timed) tm_k[2].stop();
+				if (timed) tm_k[S_GCHAIN].stop();
 				S.n_launches += 1;
-			} else { if (timed) tm_k[2].start(); launch_stage<2>(L, W); if (timed) tm_k[2].stop(); }
+			} else { if (timed) tm_k[S_GCHAIN].start(); launch_stage<S_GCHAIN>(L, W); if (timed) tm_k[S_GCHAIN].stop(); }
 			auto counts = [&]() {
 #ifndef MGB_HOSTSIM
 				k_job_counts<<<1, 1, 0, t_stream>>>(d_pools, (int)P_GJOBS, (int)P_JOBS, (unsigned int)gjobs_done, (unsigned int)jobs_done, d_cnt);
@@ -1477,13 +1467,13 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 			{ // bridging jobs planned by k_gchain, then materialisation
 				counts();
 				L.rid_list = 0, L.job_start = gjobs_done, L.n_work = 0, L.n_work_dev = d_cnt;
-				if (timed) tm_k[8].start();
+				if (timed) tm_k[S_GWFA].start();
 				make_job_order(L, 0, 0, 0, order_buf, d_cnt);
 				L.rid_list = order_buf;
-				launch_stage<8>(L, W);
-				if (timed) tm_k[8].stop();
+				launch_stage<S_GWFA>(L, W);
+				if (timed) tm_k[S_GWFA].stop();
 				L.rid_list = d_list, L.n_work = n_list, L.n_work_dev = 0;
-				{ if (timed) tm_k[9].start(); launch_stage<9>(L, W); if (timed) tm_k[9].stop(); }
+				{ if (timed) tm_k[S_GCHAIN_GEN].start(); launch_stage<S_GCHAIN_GEN>(L, W); if (timed) tm_k[S_GCHAIN_GEN].stop(); }
 				S.n_launches += 4;
 			}
 			if (timed) tm_align.stop();
@@ -1493,21 +1483,21 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 				L.c.jobq[0] = jobq_buf, L.c.jobq[1] = jobq_buf + max_jobs;
 				dzero(d_jobq_n, 2 * sizeof(unsigned int));
 				L.rid_list = 0, L.job_start = jobs_done, L.n_work = 0, L.n_work_dev = d_cnt + 1;
-				{ if (timed) tm_k[4].start(); launch_stage<4>(L, W); if (timed) tm_k[4].stop(); }
+				{ if (timed) tm_k[S_WFA_SMALL].start(); launch_stage<S_WFA_SMALL>(L, W); if (timed) tm_k[S_WFA_SMALL].stop(); }
 				L.n_work_dev = d_jobq_n;
-				{ if (timed) tm_k[6].start(); launch_stage<6>(L, W); if (timed) tm_k[6].stop(); }
+				{ if (timed) tm_k[S_WFA_MID].start(); launch_stage<S_WFA_MID>(L, W); if (timed) tm_k[S_WFA_MID].stop(); }
 				L.n_work_dev = d_jobq_n + 1;
-				if (timed) tm_k[7].start();
+				if (timed) tm_k[S_WFA_BIG].start();
 				make_job_order(L, 1, L.c.jobq[1], 0, order_buf, d_jobq_n + 1);
 				L.rid_list = order_buf;
-				launch_stage<7>(L, W);
-				if (timed) tm_k[7].stop();
+				launch_stage<S_WFA_BIG>(L, W);
+				if (timed) tm_k[S_WFA_BIG].stop();
 				L.rid_list = 0, L.n_work_dev = 0;
 				S.n_launches += 5;
 			}
 			if (timed) tm_wfa.stop(), tm_fin.start();
 			L.rid_list = d_list, L.n_work = n_list;
-			{ if (timed) tm_k[5].start(); launch_stage<5>(L, W); if (timed) tm_k[5].stop(); }
+			{ if (timed) tm_k[S_FINISH].start(); launch_stage<S_FINISH>(L, W); if (timed) tm_k[S_FINISH].stop(); }
 			if (timed) tm_fin.stop();
 			S.n_launches += 4;
 #ifndef MGB_HOSTSIM
@@ -1521,8 +1511,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		{
 			const double tq = now_ms();
 			if (attempt == 0) S.w_upload_ms = tq - t_host0;
-			std::unique_lock<std::mutex> gpu(M->gpu_mutex, std::defer_lock);
-			if (p_gpu_lock) gpu.lock();
+			std::lock_guard<std::mutex> gpu(M->gpu_mutex);
 			const double tw = now_ms();
 			S.w_gpu_wait_ms += tw - tq;
 			run_pass(0, n_reads, sl.W, true);
@@ -1546,7 +1535,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 			int nw = (int)std::min<uint64_t>(16, std::max<uint64_t>(1, dev_free_mem() / 2 / big)); // a handful of reads per batch at most come here
 			if (M->Wbig.arena == 0 || M->Wbig.arena_bytes != big) ensure_workers(M->Wbig, std::max(1, nw), big);
 			h2d(d_list_buf, redo.data(), redo.size() * sizeof(int32_t));
-			{ std::unique_lock<std::mutex> gpu(M->gpu_mutex, std::defer_lock); if (p_gpu_lock) gpu.lock(); const double tw = now_ms(); run_pass(d_list_buf, (int32_t)redo.size(), M->Wbig, false); S.w_redo_ms += now_ms() - tw; }
+			{ std::lock_guard<std::mutex> gpu(M->gpu_mutex); const double tw = now_ms(); run_pass(d_list_buf, (int32_t)redo.size(), M->Wbig, false); S.w_redo_ms += now_ms() - tw; }
 			S.n_retry += (int64_t)redo.size();
 			d2h(routs, d_routs, sizeof(ReadOut) * (size_t)n_reads);
 			d2h(meta, d_meta, sizeof(ReadMeta) * (size_t)n_reads);
@@ -1604,7 +1593,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		for (int b = 0; b < 32 && t2 == INT32_MAX; ++b) { unsigned int in = h[b * 4 + 1] + h[b * 4 + 2], out = h[b * 4 + 3]; if (in + out >= 8 && in < out) t2 = b * 16; }
 		unsigned int tot = 0;
 		for (int i = 0; i < 128; ++i) tot += h[i];
-		if (tot >= 64 && p_tier_learn) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1, M->skip2_len = t2 < t1? t1 : t2; }
+		if (tot >= 64) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1, M->skip2_len = t2 < t1? t1 : t2; }
 		S.skip1_len = L_skip1, S.skip2_len = L_skip2;
 	}
 	if (rc_final < 0) return rc_final;
@@ -1905,8 +1894,8 @@ extern "C" int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int6
 
 // ---------------------------------------------------------------------------------------------------------------
 // test hook: a batch of gaps through one on-chip WFA tier, wfa_smem() with the template arguments of k_wfa_small (tier 1)
-// or k_wfa_mid (tier 2), launched as those kernels are: STAGE_WARPS[4] / [6] warps per block, WfTier1/2::STRIDE bytes of
-// shared memory per warp, one gap per warp at a time.  The shared memory starts out filled with cells that are not -inf,
+// or k_wfa_mid (tier 2), launched as those kernels are: their stage's warps per block and slice of shared memory per warp, one
+// gap per warp at a time.  The shared memory starts out filled with cells that are not -inf,
 // and a warp aligns several gaps in a row, so the results also show that wfa_smem() clears the slices it reads and that the
 // warps of a block keep to their own slices.
 // ---------------------------------------------------------------------------------------------------------------
@@ -1942,7 +1931,7 @@ __global__ void k_test_wfa_tier(TestTierArgs t)
 {
 	extern __shared__ int4 dyn_smem[];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-	const int stride = TIER == 1? WfTier1::STRIDE : WfTier2::STRIDE;
+	const int stride = StageSpec<TIER == 1? S_WFA_SMALL : S_WFA_MID>::smem;
 	for (int j = threadIdx.x; j < n_warps * stride / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
 	__syncthreads();
 	int32_t *smem = (int32_t*)((char*)dyn_smem + (size_t)warp * stride);
@@ -1975,8 +1964,8 @@ static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_
 		if (tl[i] < 1 || ql[i] < 1 || t_off[i] < 0 || q_off[i] < 0) { set_error("mgb_test_wfa_tier: gap " + std::to_string(i) + " has an empty side"); return MGB_E_UNSUPPORTED; }
 	if (n == 0) return 0;
 	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	const int stage = tier == 1? 4 : 6, warps = STAGE_WARPS[stage];
-	const int stride = tier == 1? WfTier1::STRIDE : WfTier2::STRIDE;
+	const int warps = tier == 1? StageSpec<S_WFA_SMALL>::warps : StageSpec<S_WFA_MID>::warps;
+	const int stride = tier == 1? StageSpec<S_WFA_SMALL>::smem : StageSpec<S_WFA_MID>::smem;
 	const int n_workers = std::min(n, 64 * warps);
 	TestTierArgs t;
 	t.tier = tier, t.n = n, t.cap = cap;
@@ -2073,7 +2062,7 @@ __global__ void k_test_gwfa(TestGwfaArgs t)
 {
 	extern __shared__ int4 dyn_smem[];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-	GwfShared *sh = (GwfShared*)((char*)dyn_smem + (size_t)warp * GWFA_SMEM_ARENA);
+	GwfShared *sh = (GwfShared*)((char*)dyn_smem + (size_t)warp * StageSpec<S_GWFA>::smem);
 	const int worker = blockIdx.x * n_warps + warp;
 	Arena A;
 	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
@@ -2094,7 +2083,7 @@ static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, co
 		}
 	if (n == 0) return 0;
 	if (!dev_ok(M->device)) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	const int warps = STAGE_WARPS[8], n_workers = std::min(n, 8 * warps);
+	const int warps = StageSpec<S_GWFA>::warps, n_workers = std::min(n, 8 * warps);
 	TestGwfaArgs t;
 	t.g = M->g, t.mode = mode, t.n = n, t.walk_cap = walk_cap;
 	t.q = dcopy(q, test_seq_bytes(n, q_off, ql));
@@ -2105,7 +2094,7 @@ static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, co
 	t.arena_bytes = (uint64_t)64 << 20;
 	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
 #ifdef MGB_HOSTSIM
-	std::vector<u128> sim_smem(GWFA_SMEM_ARENA / sizeof(u128));
+	std::vector<u128> sim_smem(StageSpec<S_GWFA>::smem / sizeof(u128));
 	GwfShared *sh = (GwfShared*)sim_smem.data();
 	for (int i = 0; i < n; ++i) {
 #if MGB_W > 1
@@ -2117,7 +2106,7 @@ static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, co
 #endif
 	}
 #else
-	const size_t smem = (size_t)warps * GWFA_SMEM_ARENA;
+	const size_t smem = (size_t)warps * StageSpec<S_GWFA>::smem;
 	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test_gwfa, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 	k_test_gwfa<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
 	CUDA_OK(cudaGetLastError());

@@ -159,9 +159,6 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 		}
 		return 0;
 	}
-#if !MGB_ON_DEVICE && defined(MGB_HOSTSIM)
-	if (getenv("MGB_DUMP_JOBS")) fprintf(stderr, "JOB\t%d\t%d\t%d\t%ld\t%d\t%d\n", tl, ql, rst.s, (long)rst.n_iter, rst.n_cigar, tier);
-#endif
 	if (rst.s < 0) return MGB_E_INTERNAL;
 	int64_t coff = 0;
 	if (lane == 0) {
@@ -548,17 +545,11 @@ MG_HD inline int stage_gchain(const PipeCtx &c, ReadOut *routs, int rid, Arena &
 	return rc;
 }
 
-// K7a: one bridging alignment (reference: gchain1.c:349-381).  The wavefront containers of a typical bridge (tens of
-// diagonals) fit a small per-warp arena in SHARED memory, which removes the global-memory latency from the sequential
-// control flow; a bridge that outgrows it is redone with the worker's arena in HBM.  Lane 0 runs the alignment.
-#ifndef MGB_GWFA_SMEM_KB
-#define MGB_GWFA_SMEM_KB 1
-#endif
-#ifndef MGB_GWFA_SMEM_QL
-#define MGB_GWFA_SMEM_QL 0
-#endif
-static const int GWFA_SMEM_ARENA = MGB_GWFA_SMEM_KB * 1024;
-static const int GWFA_SMEM_MAX_QL = MGB_GWFA_SMEM_QL;
+// K7a: one bridging alignment (reference: gchain1.c:349-381), all lanes of the warp on gwf_align_w().  The alignment state
+// (GwfShared: the arena header, the wavefront state and the result) sits in the warp's slice of shared memory, where every lane
+// sees it; the wavefronts themselves are allocated from the worker's arena in HBM.
+static const int GWF_SHARED_BYTES = 1024; // the slice of shared memory per warp of k_gwfa
+static_assert(sizeof(GwfShared) <= GWF_SHARED_BYTES, "the alignment state has to fit the warp's slice of shared memory");
 
 MG_HD inline int gwfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int lane, int32_t *smem)
 {
@@ -566,44 +557,18 @@ MG_HD inline int gwfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int l
 	if (J->rid < 0) return 0;
 	if (c.meta[J->rid].status < 0) return 0;
 	GwfShared *sh = (GwfShared*)smem; // the one copy of the alignment state, seen by all lanes
-	static_assert(sizeof(GwfShared) + 16 <= GWFA_SMEM_ARENA, "the alignment state has to fit the warp's slice of shared memory");
-	const uint64_t sh_bytes = (sizeof(GwfShared) + 15) & ~(uint64_t)15;
 	GwfOpt opt;
 	opt.traceback = 1, opt.max_chk = 1000, opt.bw_dyn = 1000, opt.max_lag = J->max_ed / 2, opt.s_term = -1;
 	opt.i_term = 500000000LL;
 	const char *qseq = c.b.seq + c.b.seq_off[J->rid];
 	unsigned long long t0 = prof_clock();
-	// one call site for both attempts (the kernel holds one copy of the alignment code): first in the shared-memory arena, then,
-	// if that was outgrown or not worth trying, in the worker's arena in HBM
-	int rc = MGB_E_ARENA, in_smem = 0;
-	uint64_t smem_peak = 0;
-	for (int pass = J->ql < GWFA_SMEM_MAX_QL? 0 : 1; pass < 2; ++pass) { // longer bridges nearly always outgrow the shared-memory arena: do not try
-		uint64_t top0 = 0;
-		if (lane == 0) {
-			if (pass == 0) arena_init(sh->A, (char*)smem + sh_bytes, GWFA_SMEM_ARENA - sh_bytes);
-			else sh->A = A, sh->A.peak = A.top;
-		}
-		warp_sync();
-		if (pass == 1) top0 = sh->A.top;
-		rc = gwf_align_w(sh, c.g, opt, J->ql, qseq + J->qs, J->v0, J->end0, J->v1, J->end1, J->max_ed, lane);
-		if (pass == 0) {
-			if (rc != MGB_E_ARENA) { in_smem = 1, smem_peak = sh->A.peak; break; }
-			warp_sync();
-			continue;
-		}
-#if !MGB_ON_DEVICE && defined(MGB_HOSTSIM)
-		if (getenv("MGB_DUMP_JOBS")) fprintf(stderr, "GWFAG\t%d\t%lu\n", J->ql, (unsigned long)(sh->A.peak - top0));
-#endif
-		(void)top0;
-		if (sh->A.peak > A.peak) A.peak = sh->A.peak;
-	}
-	(void)smem_peak, (void)in_smem;
+	if (lane == 0) sh->A = A, sh->A.peak = A.top;
+	warp_sync();
+	int rc = gwf_align_w(sh, c.g, opt, J->ql, qseq + J->qs, J->v0, J->end0, J->v1, J->end1, J->max_ed, lane);
+	if (sh->A.peak > A.peak) A.peak = sh->A.peak;
 	if (lane == 0) {
 		const GwfResult &r = sh->r;
 		{ unsigned long long dt = prof_clock() - t0; prof_add(c, PROF_GC_GWFA_CYC, dt); prof_max(c, PROF_GWFA_MAX_CYC, dt << 16 | (unsigned long long)(J->ql < 65535? J->ql : 65535)); }
-#if !MGB_ON_DEVICE && defined(MGB_HOSTSIM)
-		if (getenv("MGB_DUMP_JOBS")) fprintf(stderr, "GWFA\t%d\t%d\t%ld\t%d\t%lu\t%d\n", J->ql, r.s, (long)r.n_iter, r.nv, (unsigned long)smem_peak, in_smem);
-#endif
 		if (rc == 0) {
 			J->s = r.s, J->nv = r.s >= 0? r.nv : 0;
 			if (r.s >= 0) {

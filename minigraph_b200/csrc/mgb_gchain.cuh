@@ -225,9 +225,6 @@ MG_HD inline int gchain_dp_w(Arena &A, const GraphDev &g, const LabTab &T, int32
 	}
 	warp_sync();
 	const int32_t n_pairs = roff[n_ext];
-#if !MGB_ON_DEVICE && defined(MGB_HOSTSIM)
-	if (lane == 0 && getenv("MGB_DUMP_GC")) fprintf(stderr, "GC\t%d\t%d\t%d\n", n_lc, n_ext, n_pairs);
-#endif
 	int32_t max_row = 0;
 	for (int32_t i = lane; i < n_ext; i += MGB_W) max_row = x0[i] + 1 > max_row? x0[i] + 1 : max_row;
 	max_row = warp_max_i32(max_row);

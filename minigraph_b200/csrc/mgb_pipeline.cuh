@@ -363,9 +363,6 @@ MG_HD inline int stage_chain(const PipeCtx &c, int rid, Arena &A, int lane, int3
 {
 	ReadMeta &m = c.meta[rid];
 	if (m.status != 0) return 0;
-#if !MGB_ON_DEVICE && defined(MGB_HOSTSIM)
-	if (getenv("MGB_DUMP_CHAIN")) A.peak = A.top;
-#endif
 	u128 *a = c.anchor + m.a_off;
 	const int64_t n_a = m.n_a;
 	ChainRun run;

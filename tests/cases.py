@@ -493,20 +493,16 @@ def case_chain_skip(lib, workdir, n_reads=40):
                 assert d is None, "%s max_lc_skip=%d read %d: %s" % (preset, skip, i, d)
 
 
-def case_switches(lib, workdir, device):
-    """the engine's experiment switches change the schedule, never the result: the same golden GAF with each of them on"""
-    settings = [{b"lab_cache": 0}]  # graph chaining without the label table
-    if device:
-        settings += [{b"sw8": 1, b"mb8": 16, b"sw7": 1, b"mb7": 16}]  # one-warp blocks for the tail-bound job kernels
-    defaults = {b"lab_cache": 1, b"sw8": 4, b"mb8": 4, b"sw7": 4, b"mb7": 4}
-    for st in settings:
-        try:
-            for k, v in st.items():
-                assert lib.mgb_set_param(k, v) == 0
-            case_c3(lib, workdir)
-        finally:
-            for k in st:
-                lib.mgb_set_param(k, defaults[k])
+def case_switches(lib, workdir):
+    """the engine's switch lab_cache=0 (graph chaining without the label table) changes the schedule, never the result: the same
+    golden GAF; keys the engine does not have are refused"""
+    for k in (b"pack2", b"gpu_lock", b"index_dev", b"tier_learn", b"thread_mask", b"block_warps", b"sw8", b"mb8"):
+        assert lib.mgb_set_param(k, 1) == -1, k
+    try:
+        assert lib.mgb_set_param(b"lab_cache", 0) == 0
+        case_c3(lib, workdir)
+    finally:
+        lib.mgb_set_param(b"lab_cache", 1)
 
 
 def case_concurrent_calls(lib, workdir, n_threads=3, n_reads=90):
@@ -555,9 +551,9 @@ def case_concurrent_calls(lib, workdir, n_threads=3, n_reads=90):
 
 
 def case_index_big(lib, workdir, graph_len=50000000, n_probe=40000):
-    """the minimizer table of a graph whose index does not fit L2 (built on the device, mgb_index.cuh) against the reference's
-    (index.c:115-165): the same occurrence list -- content and order -- for tens of thousands of probed minimizers and for keys
-    that are not there, the same quantile-derived mapping options (options.c:120-134), and the switch back to the host build"""
+    """the minimizer table of a graph whose index does not fit L2 (built on the device, mgb_index.cuh; in the simulators on the
+    host) against the reference's (index.c:115-165): the same occurrence list -- content and order -- for tens of thousands of
+    probed minimizers and for keys that are not there, and the same quantile-derived mapping options (options.c:120-134)"""
     import ctypes as C
     import random
     from minigraph_b200 import options
@@ -595,25 +591,20 @@ def case_index_big(lib, workdir, graph_len=50000000, n_probe=40000):
         C.CDLL(None).free(v.a)
     keys = sorted(keys) + [rnd.getrandbits(2 * io.k) for _ in range(2000)]
     n1, n2 = C.c_int(0), C.c_int(0)
-    for index_dev in (1, 0):
-        assert lib.mgb_set_param(b"index_dev", index_dev) == 0
-        try:
-            g = lib.mgb_gfa_read((pre + ".gfa").encode())
-            io2, mo = options.opt_set("lr")
-            gi = lib.mg_index(g, C.byref(io2), 1, C.byref(mo))
-            assert gi, lib.mgb_last_error()
-            assert (mo.occ_max1, mo.lc_max_occ, mo.bw_long) == (rmo.occ_max1, rmo.lc_max_occ, rmo.bw_long)
-            n_multi = 0
-            for k in keys:
-                a, b = ref.mg_idx_get(rgi, k, C.byref(n1)), lib.mg_idx_get(gi, k, C.byref(n2))
-                assert n1.value == n2.value, (hex(k), n1.value, n2.value)
-                assert [a[i] for i in range(n1.value)] == [b[i] for i in range(n2.value)], hex(k)
-                n_multi += n1.value > 1
-            assert n_multi > 100, n_multi
-            lib.mg_idx_destroy(gi)
-            lib.mgb_gfa_destroy(g)
-        finally:
-            lib.mgb_set_param(b"index_dev", 1)
+    g = lib.mgb_gfa_read((pre + ".gfa").encode())
+    io2, mo = options.opt_set("lr")
+    gi = lib.mg_index(g, C.byref(io2), 1, C.byref(mo))
+    assert gi, lib.mgb_last_error()
+    assert (mo.occ_max1, mo.lc_max_occ, mo.bw_long) == (rmo.occ_max1, rmo.lc_max_occ, rmo.bw_long)
+    n_multi = 0
+    for k in keys:
+        a, b = ref.mg_idx_get(rgi, k, C.byref(n1)), lib.mg_idx_get(gi, k, C.byref(n2))
+        assert n1.value == n2.value, (hex(k), n1.value, n2.value)
+        assert [a[i] for i in range(n1.value)] == [b[i] for i in range(n2.value)], hex(k)
+        n_multi += n1.value > 1
+    assert n_multi > 100, n_multi
+    lib.mg_idx_destroy(gi)
+    lib.mgb_gfa_destroy(g)
     ref.mg_idx_destroy(rgi)
     ref.gfa_destroy(rg)
 
@@ -639,8 +630,8 @@ def case_multi_device(lib, workdir, devices="0,0,0", n_reads=100):
 
 def case_upload_modes(lib, workdir, n_reads=80):
     """how the reads reach the device does not change what comes back: 2 bits per base (all A/C/G/T), the same with a few reads that
-    hold N or lower-case letters (those travel as ASCII beside the packed ones), the whole batch as ASCII (many such reads), and the
-    pack2=0 switch; every field against the reference, whose alignment compares raw bytes (N matches N, 'a' does not match 'A')"""
+    hold N or lower-case letters (those travel as ASCII beside the packed ones), and the whole batch as ASCII (many such reads); every
+    field against the reference, whose alignment compares raw bytes (N matches N, 'a' does not match 'A')"""
     pre, reads = os.path.join(workdir, "svu"), os.path.join(workdir, "svu.reads.fa")
     T.sim_graph(pre, 300000, 3, 29)
     T.sim_reads(pre + ".hap.fa", reads, n_reads, 6000, "ont", 67)
@@ -653,18 +644,14 @@ def case_upload_modes(lib, workdir, n_reads=80):
         return bytes(b)
     few = [spoil(s, i) if i % 29 == 0 else s for i, s in enumerate(seqs)]
     many = [spoil(s, i) for i, s in enumerate(seqs)]
-    try:
-        for tag, ss, pack in (("packed", seqs, 1), ("few", few, 1), ("many", many, 1), ("switch", seqs, 0)):
-            assert lib.mgb_set_param(b"pack2", pack) == 0
-            want, _ = T.map_with_ref(pre + ".gfa", names, ss, "lr")
-            got, _, st = T.map_with_engine(lib, pre + ".gfa", names, ss, "lr")
-            bases = sum(len(x) for x in ss)
-            assert (st.h2d_bytes < bases // 2) == (tag in ("packed", "few")), (tag, st.h2d_bytes, bases)
-            for i, (a, b) in enumerate(zip(want, got)):
-                d = T.diff_results(a, b)
-                assert d is None, "%s read %d: %s" % (tag, i, d)
-    finally:
-        lib.mgb_set_param(b"pack2", 1)
+    for tag, ss in (("packed", seqs), ("few", few), ("many", many)):
+        want, _ = T.map_with_ref(pre + ".gfa", names, ss, "lr")
+        got, _, st = T.map_with_engine(lib, pre + ".gfa", names, ss, "lr")
+        bases = sum(len(x) for x in ss)
+        assert (st.h2d_bytes < bases // 2) == (tag in ("packed", "few")), (tag, st.h2d_bytes, bases)
+        for i, (a, b) in enumerate(zip(want, got)):
+            d = T.diff_results(a, b)
+            assert d is None, "%s read %d: %s" % (tag, i, d)
 
 
 def case_tier_routing(lib, workdir, n_reads=120):

@@ -59,17 +59,17 @@ def test_learned_tier_routing_keeps_results(lib, workdir):
     cases.case_tier_routing(lib, workdir)
 
 
-def test_engine_switches_keep_results(lib, workdir):
-    cases.case_switches(lib, workdir, device=True)
+def test_lab_cache_switch_keeps_results(lib, workdir):
+    cases.case_switches(lib, workdir)
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not there")
-def test_upload_modes(lib, workdir):
+def test_upload_modes_chosen_per_batch(lib, workdir):
     cases.case_upload_modes(lib, workdir)
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not shipped")
-def test_index_of_a_50mb_graph(lib, workdir):
+def test_device_index_of_a_50mb_graph(lib, workdir):
     cases.case_index_big(lib, workdir)
 
 

@@ -56,16 +56,16 @@ def test_learned_tier_routing_keeps_results(lib, workdir):
 
 
 def test_engine_switches_keep_results(lib, workdir):
-    cases.case_switches(lib, workdir, device=False)
+    cases.case_switches(lib, workdir)
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not there")
-def test_upload_modes(lib, workdir):
+def test_upload_modes_chosen_per_batch(lib, workdir):
     cases.case_upload_modes(lib, workdir)
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not built")
-def test_index_vs_reference_lists(lib, workdir):
+def test_host_index_vs_reference_lists(lib, workdir):
     cases.case_index_big(lib, workdir, graph_len=2000000, n_probe=5000)
 
 
