@@ -220,7 +220,8 @@ typedef struct {
 	double t_h2d_ms, t_seed_ms, t_chain_ms, t_align_ms, t_d2h_ms, t_host_ms; /* last batch, CUDA events / host clock */
 	double t_wfa_ms, t_finish_ms; /* t_align_ms = graph chaining + alignment plan; t_wfa_ms = gap alignment jobs; t_finish_ms = cigar/ds/blob */
 	double t_dev_span_ms;   /* device time from the first kernel start to the last kernel end over all sub-batches (they overlap) */
-	int64_t skip1_len, skip2_len; /* WFA tier routing this batch ran with: gaps at or above these lengths skipped tier 1 / tier 2 */
+	int64_t skip1_len, skip2_len; /* WFA tier routing this batch ran with: gaps at or above these lengths skipped tier 1 / tier 2
+	                                 (skip2_len is always INT32_MAX: every gap within tier 2's lengths is aligned there) */
 	int64_t n_jobs_side;    /* gaps aligned by the tier-3 launch that runs beside tiers 1/2 */
 	int64_t n_slots;        /* sub-batches the batch was cut into (each on its own stream and host thread) */
 	double t_pack_ms, t_asm_ms; /* host: packing reads into the staging buffer; building mg_gchains_t objects */
@@ -251,9 +252,11 @@ typedef struct {
 int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int64_t max_iter, int step, uint32_t *cigar, int cap, int *score);
 
 /* test hook: n gaps through one on-chip WFA tier (1: windows of 62 diagonals, sides of 256 bases, 4096 traceback bytes in shared
- * memory; 2: 254 diagonals, 1024 bases), launched as the tier's kernel is.  Gap i is ts[t_off[i]..+tl[i]) against
+ * memory; 2: 254 diagonals, 1024 bases; MGB_TEST_TIER2_CONT: tier 2 as k_wfa_mid runs it, where a gap whose window outgrows the
+ * 254 diagonals before score 240 is carried on in the worker arena instead of refused), launched as the tier's kernel is.  Gap i is ts[t_off[i]..+tl[i]) against
  * qs[q_off[i]..+ql[i]).  out[4i..4i+3] = rc (0: aligned, 1: does not fit the tier, < 0: error), score, n_iter, n_cigar; the CIGAR
  * (len<<4|op) goes to cigar[i*cap..].  Returns 0, or a negative code (nothing run) when a gap has an empty side. */
+#define MGB_TEST_TIER2_CONT 4
 int mgb_test_wfa_tier(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
 					  const int32_t *ql, int64_t *out, uint32_t *cigar, int cap);
 

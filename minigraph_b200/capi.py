@@ -103,7 +103,10 @@ class mgb_reads_t(C.Structure):
 KERNEL_NAMES = ["k_seed", "k_chain", "k_gchain", "k_index_sketch", "k_wfa_small", "k_finish", "k_wfa_mid", "k_wfa_big", "k_gwfa", "k_gchain_gen"]
 PROF_NAMES = ["wfa_fast_cyc", "wfa_fast_n", "wfa_slow_cyc", "wfa_slow_n", "wfa_max_cyc", "wfa_cells", "wfa_tb_cyc", "gc_dp_cyc", "gc_gen_cyc",
               "gc_post_cyc", "gc_plan_cyc", "fin_cigar_cyc", "fin_ds_cyc", "seed_sketch_cyc", "seed_match_cyc", "seed_sort_cyc", "chain_dp_cyc",
-              "chain_onchip_n", "chain_rmq_cyc", "chain_post_cyc", "wfa_mid_cyc", "wfa_mid_n", "gc_gwfa_cyc", "gc_bridge_shortk_cyc", "gc_extra_sort_cyc", "gwfa_max_cyc", "gc_dp_max_cyc", "wfa_cta_cyc", "wfa_cta_n", "lab_cyc", "lab_n"]
+              "chain_onchip_n", "chain_rmq_cyc", "chain_post_cyc", "wfa_mid_cyc", "wfa_mid_n", "gc_gwfa_cyc", "gc_bridge_shortk_cyc", "gc_extra_sort_cyc", "gwfa_max_cyc", "gc_dp_max_cyc", "wfa_handoff_cells", "wfa_handoff_n", "lab_cyc", "lab_n"]
+# mgb_test_wfa_tier(): tier 2 as k_wfa_mid runs it, carrying a gap whose window outgrows the shared-memory ring on in the arena
+# (mgb200.h MGB_TEST_TIER2_CONT)
+WFA_TIER2_CONT = 4
 
 
 def bind_mapping_api(lib):

@@ -333,9 +333,7 @@ MGB_STAGE(k_gwfa,          S_GWFA,         4,    4,     GWF_SHARED_BYTES,       
 MGB_STAGE(k_gchain_gen,    S_GCHAIN_GEN,   4,    4,     0,                       1,    WARP,  READ)         // K7b: graph-chain materialisation, post filters, mapq, alignment plan
 MGB_STAGE(k_index_sketch,  S_INDEX_SKETCH, 4,    8,     0,                       1,    LANE0, INDEX_STATUS) // index build: sketch of graph segments
 MGB_STAGE(k_wfa_small,     S_WFA_SMALL,    4,    5,     WfTier1::STRIDE,         4,    WARP,  GAP_JOB_T1)   // K8a tier 1: small gaps, wavefronts + traceback bytes in shared memory
-// K8a tier 2: mid-size gaps, wavefronts in shared memory.  The one kernel whose bounds (128 threads, 5 blocks per SM) are not its
-// launch shape (2 warps, 7 blocks per SM); it compiles to 79 registers under them.
-MGB_STAGE_BOUNDS(k_wfa_mid, S_WFA_MID,     2,    7,     WfTier2::STRIDE,         4,    WARP,  GAP_JOB_T2, 128, 5)
+MGB_STAGE(k_wfa_mid,       S_WFA_MID,      2,    7,     WfTier2::STRIDE,         4,    WARP,  GAP_JOB_T2)   // K8a tier 2: mid-size gaps, wavefronts in shared memory, carried on in the arena ring of tier 3 past 254 diagonals; longer sides in that ring from the start (128 registers at 7 blocks per SM, no spills)
 MGB_STAGE(k_wfa_big,       S_WFA_BIG,      4,    4,     0,                       1,    WARP,  GAP_JOB_T3)   // K8a tier 3: anything else, wavefronts in the worker arena (128 registers at 4 blocks per SM)
 MGB_STAGE(k_finish,        S_FINISH,       4,    8,     0,                       1,    WARP,  READ)         // K8b: CIGAR stitching, ds strings, result blobs
 MGB_STAGE(k_gc_labels,     S_LABELS,       4,    8,     0,                       1,    THREAD, NOWHERE)     // reachability labels of new source vertices, one search per thread (mgb_gclabel.cuh)
@@ -665,7 +663,7 @@ struct Model {
 	std::vector<int32_t> seg_name_id, seg_soff; // MG_M_NO_DIAG: the name a segment goes by (id into name_ids) and its offset there
 	std::unordered_map<std::string, int32_t> name_ids;
 	Workers W, Wbig;
-	int32_t skip1_len = INT32_MAX, skip2_len = INT32_MAX; // WFA tier routing learned from earlier batches (wfa_job_run)
+	int32_t skip1_len = INT32_MAX; // WFA tier routing learned from earlier batches (wfa_job_run)
 	std::vector<float> logf_tab; float *d_logf; int n_logf;
 	mgb_stats_t stats;
 	gfa_edseq_t *es;
@@ -1199,7 +1197,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	memset(&S, 0, sizeof(S));
 	sl.ev_first_ms = sl.ev_last_ms = 0;
 	if (n_reads <= 0) return 0;
-	const int32_t L_skip1 = M->skip1_len, L_skip2 = M->skip2_len; // thresholds this batch runs with
+	const int32_t L_skip1 = M->skip1_len; // threshold this batch runs with
 	double t_host0 = now_ms();
 	// ---- pack the sub-batch into page-locked memory ----
 	uint64_t tot = 0;
@@ -1408,7 +1406,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 			dzero(d_lab_n, 2 * sizeof(unsigned int));
 		}
 		L.c.prof = d_prof;
-		L.c.tier_hist = d_tier_hist, L.c.skip1_len = L_skip1, L.c.skip2_len = L_skip2;
+		L.c.tier_hist = d_tier_hist, L.c.skip1_len = L_skip1;
 		L.c.jobq[0] = 0, L.c.jobq[1] = 0, L.c.jobq_n = d_jobq_n;
 		L.routs = d_routs;
 		int64_t jobs_done = 0, gjobs_done = 0;
@@ -1485,15 +1483,19 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 				L.rid_list = 0, L.job_start = jobs_done, L.n_work = 0, L.n_work_dev = d_cnt + 1;
 				{ if (timed) tm_k[S_WFA_SMALL].start(); launch_stage<S_WFA_SMALL>(L, W); if (timed) tm_k[S_WFA_SMALL].stop(); }
 				L.n_work_dev = d_jobq_n;
-				{ if (timed) tm_k[S_WFA_MID].start(); launch_stage<S_WFA_MID>(L, W); if (timed) tm_k[S_WFA_MID].stop(); }
-				L.n_work_dev = d_jobq_n + 1;
+				if (timed) tm_k[S_WFA_MID].start();
+				make_job_order(L, 1, L.c.jobq[0], 0, order_buf, d_jobq_n); // longest first: the long gaps, which run on one warp each, start early
+				L.rid_list = order_buf;
+				launch_stage<S_WFA_MID>(L, W);
+				if (timed) tm_k[S_WFA_MID].stop();
+				L.rid_list = 0, L.n_work_dev = d_jobq_n + 1;
 				if (timed) tm_k[S_WFA_BIG].start();
 				make_job_order(L, 1, L.c.jobq[1], 0, order_buf, d_jobq_n + 1);
 				L.rid_list = order_buf;
 				launch_stage<S_WFA_BIG>(L, W);
 				if (timed) tm_k[S_WFA_BIG].stop();
 				L.rid_list = 0, L.n_work_dev = 0;
-				S.n_launches += 5;
+				S.n_launches += 6;
 			}
 			if (timed) tm_wfa.stop(), tm_fin.start();
 			L.rid_list = d_list, L.n_work = n_list;
@@ -1586,15 +1588,14 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	S.t_lab_ms = tm_lab.ms();
 	S.arena_peak = mail->arena_peak; // (the mailbox was last filled after the last pass of the batch)
 	for (int i = 0; i < 32; ++i) S.prof[i] = (uint64_t)mail->prof[i];
-	{ // tier routing for the next batch: the first length bucket in which the sampled gaps mostly ended beyond a tier
+	{ // tier-1 routing for the next batch: the first length bucket in which the sampled gaps mostly ended beyond tier 1
 		const unsigned int *h = mail->tier_hist;
-		int32_t t1 = INT32_MAX, t2 = INT32_MAX;
+		int32_t t1 = INT32_MAX;
 		for (int b = 0; b < 32 && t1 == INT32_MAX; ++b) { unsigned int in = h[b * 4 + 1], out = h[b * 4 + 2] + h[b * 4 + 3]; if (in + out >= 8 && in < out) t1 = b * 16; }
-		for (int b = 0; b < 32 && t2 == INT32_MAX; ++b) { unsigned int in = h[b * 4 + 1] + h[b * 4 + 2], out = h[b * 4 + 3]; if (in + out >= 8 && in < out) t2 = b * 16; }
 		unsigned int tot = 0;
 		for (int i = 0; i < 128; ++i) tot += h[i];
-		if (tot >= 64) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1, M->skip2_len = t2 < t1? t1 : t2; }
-		S.skip1_len = L_skip1, S.skip2_len = L_skip2;
+		if (tot >= 64) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1; }
+		S.skip1_len = L_skip1, S.skip2_len = INT32_MAX; // every gap that fits tier 2's lengths is aligned there
 	}
 	if (rc_final < 0) return rc_final;
 
@@ -1915,8 +1916,10 @@ MG_HD inline void test_wfa_tier_body(const TestTierArgs &t, int i, int32_t *smem
 	WfResult r;
 	A.top = 0;
 	const char *ts = t.ts + t.t_off[i], *qs = t.qs + t.q_off[i];
+	int64_t cont_cells = 0;
 	int rc = t.tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane)
-						: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane);
+			: t.tier == 2? wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane)
+						: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane, &cont_cells);
 	if (rc == 0 && r.n_cigar > t.cap) rc = MGB_E_INTERNAL;
 	if (rc == 0) for (int32_t j = lane; j < r.n_cigar; j += MGB_W) t.cigar[(int64_t)i * t.cap + j] = r.cigar[j];
 	if (lane == 0) {
@@ -1959,7 +1962,10 @@ static int64_t test_seq_bytes(int n, const int64_t *off, const int32_t *len)
 static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
 							  const int32_t *ql, int64_t *out, uint32_t *cigar, int cap)
 {
-	if ((tier != 1 && tier != 2) || n < 0 || cap < 0) { set_error("mgb_test_wfa_tier: tier must be 1 or 2, n and cap at least 0"); return MGB_E_UNSUPPORTED; }
+	if ((tier != 1 && tier != 2 && tier != MGB_TEST_TIER2_CONT) || n < 0 || cap < 0) {
+		set_error("mgb_test_wfa_tier: tier must be 1, 2 or MGB_TEST_TIER2_CONT, n and cap at least 0");
+		return MGB_E_UNSUPPORTED;
+	}
 	for (int i = 0; i < n; ++i) // the gaps of real jobs are never empty on either side (galign.c:97-99 emits plain I/D for those)
 		if (tl[i] < 1 || ql[i] < 1 || t_off[i] < 0 || q_off[i] < 0) { set_error("mgb_test_wfa_tier: gap " + std::to_string(i) + " has an empty side"); return MGB_E_UNSUPPORTED; }
 	if (n == 0) return 0;
@@ -1973,7 +1979,9 @@ static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_
 	t.t_off = dcopy(t_off, n), t.q_off = dcopy(q_off, n), t.tl = dcopy(tl, n), t.ql = dcopy(ql, n);
 	t.out = (int64_t*)dmalloc(sizeof(int64_t) * 4 * (size_t)n);
 	t.cigar = (uint32_t*)dmalloc(sizeof(uint32_t) * ((size_t)n * cap + 1));
-	t.arena_bytes = (uint64_t)256 << 10; // a tier-2 gap needs at most 8 KB of CIGAR and 70 KB of traceback rows
+	// a tier-2 gap needs at most 8 KB of CIGAR and 70 KB of traceback rows; one carried on in the arena at most 230 KB of ring and
+	// 4.3 MB of traceback rows (scores below tl + ql + 30, rows of at most tl + ql + 1 bytes)
+	t.arena_bytes = tier == MGB_TEST_TIER2_CONT? (uint64_t)5 << 20 : (uint64_t)256 << 10;
 	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
 #ifdef MGB_HOSTSIM
 	std::vector<uint32_t> sim_smem((size_t)warps * stride / 4, TEST_SMEM_FILL);

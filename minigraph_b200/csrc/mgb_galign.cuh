@@ -63,21 +63,24 @@ static const unsigned long long CIG_CHUNK_BYTES = 2048; // a warp of a WFA kerne
 
 // K8a: align one gap.  Warp-uniform (all lanes enter with identical arguments).
 // tier 1: small gaps, wavefronts + traceback bytes in shared memory; tier 2: mid-size gaps, wavefronts in shared
-// memory; tier 3: anything, wavefronts in the worker arena.  A job that does not fit a tier is appended to the queue
-// of the next one (jobq[tier-1]); the host launches the next tier over that queue.
+// memory, carried on in the worker arena when the window outgrows them (longer sides: in the arena from the start, while
+// wf_ring_always_fits); tier 3: anything, wavefronts in the worker arena.
+// A job that does not fit a tier is appended to the queue of the next one (jobq[tier-1]); the host launches the next tier
+// over that queue.
 MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int lane, int32_t *smem, int tier)
 {
 	WfaJob *J = &c.jobs[job_idx];
 	if (J->rid < 0) return 0; // a slot no read wrote (its allocation ran over the end of the pool; the batch is re-run with a larger one)
 	const int32_t rid = J->rid, l0 = J->l0, l = J->l, tl = J->tl, ql = J->ql;
 	if (c.meta[rid].status < 0) return 0; // the read already failed elsewhere; it will be redone as a whole
-	// Routing: a gap that cannot finish in an on-chip tier costs that tier up to a full window of cells before it gives up.
-	// Which lengths fail depends on the error rate of the reads, so it is learned: one gap in 64 tries every tier and
-	// reports where it finished; the host turns the counts of one batch into the two thresholds of the next.  The
-	// result of a gap does not depend on the tier that computes it.
+	// Routing: a gap that cannot finish in tier 1 costs it up to a full window of cells before it gives up.  Which lengths
+	// fail depends on the error rate of the reads, so it is learned: one gap in 64 tries every tier and reports where it
+	// finished; the host turns the counts of one batch into the threshold of the next.  (Tier 2 loses nothing when its
+	// window overflows, so every gap that fits its lengths stays there.)  The result of a gap does not depend on the tier
+	// that computes it.
 	const int32_t mlen = tl > ql? tl : ql;
 	const int explore = (job_idx & 63) == 0;
-	if (!explore && ((tier == 1 && mlen >= c.skip1_len) || (tier == 2 && mlen >= c.skip2_len))) {
+	if (!explore && tier == 1 && mlen >= c.skip1_len) {
 		if (lane == 0) {
 			unsigned int at;
 #if MGB_ON_DEVICE
@@ -89,7 +92,8 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 		}
 		return 0;
 	}
-	if ((tier == 1 && (tl > WfTier1::MAXLEN_ || ql > WfTier1::MAXLEN_)) || (tier == 2 && (tl > WfTier2::MAXLEN_ || ql > WfTier2::MAXLEN_))) {
+	const bool t2_long = tl > WfTier2::MAXLEN_ || ql > WfTier2::MAXLEN_; // (tier 2) the sequences do not fit shared memory: the arena ring from score 0
+	if ((tier == 1 && (tl > WfTier1::MAXLEN_ || ql > WfTier1::MAXLEN_)) || (tier == 2 && t2_long && !wf_ring_always_fits(tl, ql))) {
 		if (lane == 0) {
 			unsigned int at;
 #if MGB_ON_DEVICE
@@ -128,8 +132,10 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 	WfResult rst;
 	unsigned long long pt0 = prof_clock();
 	int rc;
+	int64_t cont_cells = 0;
 	if (tier == 1) rc = wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, tl, tseq, ql, qs, &rst, lane);
-	else if (tier == 2) rc = wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, tl, tseq, ql, qs, &rst, lane);
+	else if (tier == 2 && !t2_long) rc = wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, tl, tseq, ql, qs, &rst, lane, &cont_cells);
+	else if (tier == 2) rc = wfa_ring_exact(A, tl, tseq, ql, qs, &rst, lane);
 	else rc = wfa_exact(A, tl, tseq, ql, qs, 100000000LL, &rst, lane);
 	if (rc < 0) return rc;
 	if (lane == 0) {
@@ -138,6 +144,7 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 		prof_add(c, slot, dt), prof_add(c, slot + 1, 1);
 		prof_max(c, PROF_WFA_MAX_CYC, dt << 16 | (unsigned long long)(mlen < 65535? mlen : 65535)); // cycles of the slowest gap, its length in the low 16 bits
 		if (rc == 0) prof_add(c, PROF_WFA_CELLS, (unsigned long long)rst.n_iter);
+		if (cont_cells > 0) prof_add(c, PROF_WFA_HANDOFF_N, 1), prof_add(c, PROF_WFA_HANDOFF_CELLS, (unsigned long long)cont_cells);
 		if (rc == 0 && explore && c.tier_hist) {
 			unsigned int *h = &c.tier_hist[(mlen >> 4 < 31? mlen >> 4 : 31) * 4 + tier];
 #if MGB_ON_DEVICE

@@ -36,13 +36,13 @@ struct PipeCtx {
 	// instrumentation: 32 counters, see PROF_* below
 	unsigned long long *prof;
 	// tier routing of the gap alignments, learned from the batches before (see wfa_job_run)
-	int32_t skip1_len, skip2_len; // gaps with max(tl,ql) at or above these go past tier 1 / tier 2 without trying them
+	int32_t skip1_len;            // gaps with max(tl,ql) at or above this go past tier 1 without trying it
 	unsigned int *tier_hist;      // [32 length buckets of 16 bases][4]: final tier of the gaps that tried every tier
 };
 
 enum { PROF_WFA_FAST_CYC = 0, PROF_WFA_FAST_N, PROF_WFA_SLOW_CYC, PROF_WFA_SLOW_N, PROF_WFA_MAX_CYC, PROF_WFA_CELLS, PROF_WFA_TB_CYC,
 	   PROF_GC_DP_CYC, PROF_GC_GEN_CYC, PROF_GC_POST_CYC, PROF_GC_PLAN_CYC, PROF_FIN_CIGAR_CYC, PROF_FIN_DS_CYC, PROF_SEED_SKETCH_CYC,
-	   PROF_SEED_MATCH_CYC, PROF_SEED_SORT_CYC, PROF_CHAIN_DP_CYC, PROF_CHAIN_BT_CYC, PROF_CHAIN_RMQ_CYC, PROF_CHAIN_POST_CYC, PROF_WFA_MID_CYC, PROF_WFA_MID_N, PROF_GC_GWFA_CYC, PROF_GC_SHORTK_CYC, PROF_GC_EXTRA_CYC, PROF_GWFA_MAX_CYC, PROF_GC_DP_MAX_CYC, PROF_WFA_CTA_CYC, PROF_WFA_CTA_N, PROF_LAB_CYC, PROF_LAB_N, PROF_N = 32 };
+	   PROF_SEED_MATCH_CYC, PROF_SEED_SORT_CYC, PROF_CHAIN_DP_CYC, PROF_CHAIN_BT_CYC, PROF_CHAIN_RMQ_CYC, PROF_CHAIN_POST_CYC, PROF_WFA_MID_CYC, PROF_WFA_MID_N, PROF_GC_GWFA_CYC, PROF_GC_SHORTK_CYC, PROF_GC_EXTRA_CYC, PROF_GWFA_MAX_CYC, PROF_GC_DP_MAX_CYC, PROF_WFA_HANDOFF_CELLS, PROF_WFA_HANDOFF_N, PROF_LAB_CYC, PROF_LAB_N, PROF_N = 32 };
 
 MG_HD inline unsigned long long prof_clock()
 {

@@ -88,9 +88,42 @@ MG_HD inline int32_t wf2_ld(const void *base, int32_t off)
 		*(wf_cell_t*)((char*)H + bnH + c##S) = (wf_cell_t)h##S; \
 	}
 
-template<int W, int MAXLEN, int TBCAP>
-MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, WfResult *r, int lane)
+#define MGB_WF_RG(lo_, hi_) ((uint32_t)((hi_) + 0x8000) << 16 | (uint32_t)((lo_) + 0x8000))
+// The state of the tier-3 ring (in the worker arena, see below) between two scores: what wfa_ring_run() starts from.  wfa_ring_g()
+// sets it up at score 0; tier 2 sets it up from its shared-memory ring when the window outgrows that ring (wfa_smem_continue).
+struct WfRing {
+	wf_cell_t *cells;        // WF3_NSL slices of W columns: H x 17, E1/F1 x 3, E2/F2 x 2, G
+	int32_t W, flo, fhi;     // columns (diagonal mod W); [flo,fhi]: the columns on which all slices hold -inf or real cells
+	AVec<WfTbRow> rows;      // traceback rows, row n for score n + 1
+	int32_t n_rows, wlo, whi, s;
+	int hs, m3, m2;          // s % 17, s % 3, s % 2
+	int hit, hit_noext;      // the wavefront of score s reached the corner (... without extension)
+	int64_t n_iter;
+	// [lo,hi] of the last 17 wavefronts, by score modulo 17 (empty ranges before score 0).  On the device lane j keeps entry j in a
+	// register (three shuffles per score instead of a 17-register shift chain); a simulator with fewer lanes keeps the array.
+#if MGB_W >= 32
+	uint32_t g_mine;
+#else
+	uint32_t g_all[17];
+#endif
+};
+// [lo,hi] of the wavefront of score sc, as the history of the last 17 holds it
+MG_HD inline uint32_t wf_ring_range(const WfTbRow *rows, int32_t sc)
 {
+	return sc < 0? MGB_WF_RG(1, 0) : sc == 0? MGB_WF_RG(0, 0) : MGB_WF_RG(rows[sc - 1].lo, rows[sc - 1].hi);
+}
+
+template<int W>
+MG_HD inline int wfa_smem_continue(Arena &A, uint64_t mark, const wf_cell_t *sm, int32_t tl, const char *ts, int32_t ql, const char *qs, WfResult *r,
+								   uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R);
+
+// Returns 0 (aligned) or 1 (does not fit: the caller hands the gap to the next tier).  With CONT (tier 2 in its kernel), a gap whose
+// window outgrows the W columns before score 240 is not given up but carried on in the arena ring of tier 3 by the same warp
+// (wfa_smem_continue); *cont_cells then counts the cells computed there.
+template<int W, int MAXLEN, int TBCAP, bool CONT = false>
+MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, WfResult *r, int lane, int64_t *cont_cells = 0)
+{
+	static_assert(!CONT || TBCAP == 0, "the arena ring continues from traceback rows in the arena");
 	typedef WfSmemLayout<W, MAXLEN, TBCAP, 17> LY;
 	const int HS = 17;
 	if (tl > MAXLEN || ql > MAXLEN) return 1;
@@ -150,7 +183,19 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 		const int32_t lo = wlo > -tl? wlo - 1 : -tl;
 		const int32_t hi = whi < ql? whi + 1 : ql;
 		const int32_t width = hi - lo + 1;
-		if (width + 2 > W || s + 1 >= 255 || (TBCAP > 0 && tb_used + width > TBCAP)) { A.top = mark; return 1; }
+		if (width + 2 > W || s + 1 >= 255 || (TBCAP > 0 && tb_used + width > TBCAP)) {
+			if (CONT && s < 240) { // (then the window is what outgrew the ring)
+				WfRing R;
+				R.rows = rows, R.n_rows = n_rows, R.wlo = wlo, R.whi = whi, R.s = s, R.hs = hs, R.m3 = m3, R.m2 = m2, R.n_iter = n_iter;
+				const int rc = wfa_smem_continue<W>(A, mark_keep, H, tl, ts, ql, qs, r, cig_store, max_cigar, lane, R);
+				if (rc < 0) { A.top = mark; return rc; }
+				if (r->s < 0) { A.top = mark; return MGB_E_INTERNAL; } // (the cell cap cannot be reached, see wfa_smem_continue)
+				*cont_cells = r->n_iter - n_iter;
+				return 0;
+			}
+			A.top = mark;
+			return 1;
+		}
 		const int32_t ns = s + 1;
 		const int nhs = hs + 1 == 17? 0 : hs + 1, n3 = m3 + 1 == 3? 0 : m3 + 1, n2 = m2 ^ 1;
 		uint8_t *ax;
@@ -248,53 +293,30 @@ static const int WF3_NSL = 17 + 3 + 3 + 2 + 2 + 1;
 		} \
 	} while (0)
 
-MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
-							uint32_t *cig_store, int64_t max_cigar, int lane)
+// the score loop of tier 3 from the state R, then the traceback into cig_store; A.top is set back to mark on return
+MG_HD inline int wfa_ring_run(Arena &A, uint64_t mark, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
+							  uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R)
 {
-	if (tl + ql > 16000 || tl <= 0 || ql <= 0) return 1; // (scores stay below 2^15 too: deleting one sequence and inserting the other costs tl + ql + 30)
-	uint64_t mark = A.top;
-	int32_t W = 64;
-	while (W < tl + ql + 2) W <<= 1;
-	const int32_t mask = W - 1;
-	wf_cell_t *cells;
-	MGB_ALLOC(A, cells, wf_cell_t, (int64_t)WF3_NSL * W);
+	const int32_t W = R.W, mask = W - 1;
+	wf_cell_t *cells = R.cells;
 	wf_cell_t *H = cells, *E1 = H + 17 * W, *F1 = E1 + 3 * W, *E2 = F1 + 3 * W, *F2 = E2 + 2 * W, *G = F2 + 2 * W;
-	int32_t flo = 0, fhi = -1; // columns on which all slices have been initialised with -inf (empty so far)
+	int32_t flo = R.flo, fhi = R.fhi;
 	const int32_t d_corner = ql - tl;
-	AVec<WfTbRow> rows;
-	avec_init(rows);
-	MGB_TRY(avec_reserve_w(A, rows, 1024, lane));
-	int32_t n_rows = 0;
-	int32_t wlo = 0, whi = 0, last_state = 0, s = 0, stopped = 0;
-	int64_t n_iter = 0;
-	int hs = 0, m3 = 0, m2 = 0; // s % 17, s % 3, s % 2, kept incrementally
-#define MGB_WF_RG(lo_, hi_) ((uint32_t)((hi_) + 0x8000) << 16 | (uint32_t)((lo_) + 0x8000))
-	// [lo,hi] of the last 17 wavefronts, by score modulo 17 (empty ranges before score 0).  On the device lane j keeps entry j in a
-	// register (three shuffles per score instead of a 17-register shift chain); a simulator with fewer lanes keeps the array.
+	AVec<WfTbRow> rows = R.rows;
+	int32_t n_rows = R.n_rows;
+	int32_t wlo = R.wlo, whi = R.whi, last_state = 0, s = R.s, stopped = 0;
+	int64_t n_iter = R.n_iter;
+	int hs = R.hs, m3 = R.m3, m2 = R.m2;
+	int hit = R.hit, hit_noext = R.hit_noext;
 #if MGB_W >= 32
-	uint32_t g_mine = lane == 0? MGB_WF_RG(0, 0) : MGB_WF_RG(1, 0);
+	uint32_t g_mine = R.g_mine;
 #define MGB_WF_GGET(slot_) ((uint32_t)warp_bcast_i32((int32_t)g_mine, (slot_)))
 #define MGB_WF_GSET(slot_, v_) do { if (lane == (slot_)) g_mine = (v_); } while (0)
 #else
-	uint32_t g_all[17];
-	for (int j = 0; j < 17; ++j) g_all[j] = j == 0? MGB_WF_RG(0, 0) : MGB_WF_RG(1, 0);
+	uint32_t *g_all = R.g_all;
 #define MGB_WF_GGET(slot_) (g_all[(slot_)])
 #define MGB_WF_GSET(slot_, v_) (g_all[(slot_)] = (v_))
 #endif
-	int hit = 0, hit_noext = 0;
-	MGB_WF2_FILL(-1, 1);
-	if (lane == 0) { // score 0: the main diagonal, extended from the corner
-		const int32_t c0 = (1 << 20) & mask;
-		int32_t k0 = -1, k = -1;
-		k = wf_extend(ts, qs, k0, 0);
-		if (k == tl - 1 && k == ql - 1) hit = 1, hit_noext = (k == k0), k = k0;
-		H[c0] = (wf_cell_t)k;
-	}
-	{
-		const uint32_t vb = warp_or_u32((hit? 1u : 0u) | (hit_noext? 2u : 0u));
-		hit = vb & 1, hit_noext = vb >> 1 & 1;
-	}
-	warp_sync();
 	for (;;) {
 		if (hit) {
 			if (hit_noext) { WfTbArena t; t.row = rows.a; last_state = t.get(n_rows - 1, ql - tl) & 7; }
@@ -366,7 +388,6 @@ MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, co
 		n_iter += width;
 		if (max_iter > 0 && n_iter > max_iter) { stopped = 1; break; }
 	}
-#undef MGB_WF_RG
 #undef MGB_WF_GGET
 #undef MGB_WF_GSET
 	r->n_iter = n_iter;
@@ -387,6 +408,102 @@ MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, co
 	A.top = mark;
 	return 0;
 }
+
+MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
+							uint32_t *cig_store, int64_t max_cigar, int lane)
+{
+	if (tl + ql > 16000 || tl <= 0 || ql <= 0) return 1; // (scores stay below 2^15 too: deleting one sequence and inserting the other costs tl + ql + 30)
+	uint64_t mark = A.top;
+	int32_t W = 64;
+	while (W < tl + ql + 2) W <<= 1;
+	const int32_t mask = W - 1;
+	wf_cell_t *cells;
+	MGB_ALLOC(A, cells, wf_cell_t, (int64_t)WF3_NSL * W);
+	int32_t flo = 0, fhi = -1; // columns on which all slices have been initialised with -inf (empty so far)
+	WfRing R;
+	avec_init(R.rows);
+	MGB_TRY(avec_reserve_w(A, R.rows, 1024, lane));
+#if MGB_W >= 32
+	R.g_mine = wf_ring_range(0, lane == 0? 0 : -1);
+#else
+	for (int j = 0; j < 17; ++j) R.g_all[j] = wf_ring_range(0, j == 0? 0 : -1);
+#endif
+	int hit = 0, hit_noext = 0;
+	MGB_WF2_FILL(-1, 1);
+	if (lane == 0) { // score 0: the main diagonal, extended from the corner
+		const int32_t c0 = (1 << 20) & mask;
+		int32_t k0 = -1, k = -1;
+		k = wf_extend(ts, qs, k0, 0);
+		if (k == tl - 1 && k == ql - 1) hit = 1, hit_noext = (k == k0), k = k0;
+		cells[c0] = (wf_cell_t)k;
+	}
+	{
+		const uint32_t vb = warp_or_u32((hit? 1u : 0u) | (hit_noext? 2u : 0u));
+		hit = vb & 1, hit_noext = vb >> 1 & 1;
+	}
+	warp_sync();
+	R.cells = cells, R.W = W, R.flo = flo, R.fhi = fhi;
+	R.n_rows = 0, R.wlo = R.whi = R.s = 0, R.hs = R.m3 = R.m2 = 0, R.hit = hit, R.hit_noext = hit_noext, R.n_iter = 0;
+	return wfa_ring_run(A, mark, tl, ts, ql, qs, max_iter, r, cig_store, max_cigar, lane, R);
+}
+
+// Gaps of tier 2 with a side longer than its shared memory holds: the arena ring from score 0, when the gap is small enough that
+// none of what wfa_exact adds can be reached -- 16-bit cells need tl + ql <= 16000, and with scores below tl + ql + 30 and rows of
+// at most tl + ql + 1 cells the cap of 10^8 cells cannot be hit.  (In tier 3 these gaps were a tail of single-warp runs.)
+MG_HD inline bool wf_ring_always_fits(int32_t tl, int32_t ql) { const int64_t n = (int64_t)tl + ql; return (n + 30) * (n + 1) <= 100000000LL; }
+MG_HD inline int wfa_ring_exact(Arena &A, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, WfResult *r, int lane)
+{
+	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0;
+	uint32_t *cig_store;
+	const int64_t max_cigar = (int64_t)tl + ql + 2;
+	MGB_ALLOC(A, cig_store, uint32_t, max_cigar);
+	const uint64_t mark_keep = A.top;
+	char *ts, *qs;
+	MGB_ALLOC(A, ts, char, tl + WF_SEQ_PAD + 4);
+	MGB_ALLOC(A, qs, char, ql + WF_SEQ_PAD + 4);
+	wf_stage_seq(ts, ts_g, tl, 0xfe, lane);
+	wf_stage_seq(qs, qs_g, ql, 0xff, lane);
+	warp_sync();
+	const int rc = wfa_ring_g(A, tl, ts, ql, qs, 100000000LL, r, cig_store, max_cigar, lane);
+	if (rc < 0) return rc;
+	if (rc != 0 || r->s < 0) return MGB_E_INTERNAL; // (excluded by wf_ring_always_fits)
+	A.top = mark_keep;
+	return 0;
+}
+
+// Tier 2 -> arena ring.  The tier-2 state when its window outgrows the W columns of shared memory is the state wfa_ring_run()
+// needs: the same slots (score mod 17/3/2), the same 16-bit cells, the traceback rows already in the arena.  Only the column
+// of a diagonal changes (mod W on chip, mod a power of two >= tl + ql + 2 in the arena): the 27 slices are copied over the
+// range of the last wavefront, which contains the range of every earlier one (the on-chip window never shrinks), and the
+// slice G starts as -inf -- correct while s < 240, because no wavefront before score 240 is noted in G (see `track`).  Here
+// tl, ql <= 1024, so the score stays below tl + ql + 30 and the cells below 2^15, and a gap takes fewer than 2100 x 2049 cells:
+// far below the cap of 10^8, so neither the 32-bit ring nor the chaining heuristic of tier 3 (wfa_exact) can be reached.
+template<int W>
+MG_HD inline int wfa_smem_continue(Arena &A, uint64_t mark, const wf_cell_t *sm, int32_t tl, const char *ts, int32_t ql, const char *qs, WfResult *r,
+								   uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R)
+{
+	int32_t W2 = 64;
+	while (W2 < tl + ql + 2) W2 <<= 1;
+	const int32_t mask = W2 - 1;
+	MGB_ALLOC(A, R.cells, wf_cell_t, (int64_t)WF3_NSL * W2);
+	R.W = W2;
+	const int32_t clo = R.rows.a[R.n_rows - 1].lo - 1, chi = R.rows.a[R.n_rows - 1].hi + 1; // at most W columns: no two alias on chip
+	for (int sl = 0; sl < WF3_NSL; ++sl) {
+		const wf_cell_t *src = sm + sl * W;
+		wf_cell_t *dst = R.cells + (int64_t)sl * W2;
+		for (int32_t d = clo + lane; d <= chi; d += MGB_W) dst[(d + (1 << 20)) & mask] = sl < WF3_NSL - 1? src[wfs_col<W>(d)] : (wf_cell_t)WF_NEG_INF16;
+	}
+	R.flo = clo, R.fhi = chi;
+#if MGB_W >= 32
+	R.g_mine = lane < 17? wf_ring_range(R.rows.a, R.s - (R.hs - lane + 17) % 17) : wf_ring_range(0, -1);
+#else
+	for (int j = 0; j < 17; ++j) R.g_all[j] = wf_ring_range(R.rows.a, R.s - (R.hs - j + 17) % 17);
+#endif
+	R.hit = R.hit_noext = 0;
+	warp_sync();
+	return wfa_ring_run(A, mark, tl, ts, ql, qs, 100000000LL, r, cig_store, max_cigar, lane, R);
+}
+#undef MGB_WF_RG
 #undef MGB_WF2_CLEAN
 #undef MGB_WF2_FILL
 
