@@ -271,6 +271,21 @@ int mgb_test_gwfa(const mg_idx_t *gi, int mode, int n, const char *q, const int6
  * by digit walk (walk 1), with hot_bytes of shared memory for its scratch (0: all of it in global memory); 0 or a negative code */
 int mgb_test_radix128(mg128_t *a, int64_t n, int walk, int hot_bytes);
 
+/* test hook: linear chaining of n anchor sets as the chaining kernels run it, the anchors staged into a warp's slice of shared
+ * memory when they fit.  mode 0: DP (k_chain, lr); 1: RMQ with opt.bw (k_chain, asm); 2: the anchors sorted back into target
+ * order, then RMQ (k_chain_rescue, which the caller gives bw_long as opt.bw).  Set i is a[off[i]..+cnt[i]) with the options opt[i]
+ * (the RMQ chaining takes max_dist_x as its max_dist).  out[6i..6i+5] = rc, n_u, n_v, staged (0/1), path (0: DP, 1: RMQ, the
+ * warp-wide fill; 2: RMQ, the warp-wide fill gave up on a tie of priorities; 3: RMQ, sequential because cnt[i] > cap_rmq_size;
+ * -1: no anchors), worker; the chains go to u[off[i]..+n_u), the compacted anchors to a_out[off[i]..+n_v).  Returns 0, or a
+ * negative code (nothing run) for a bad mode, offset or count. */
+typedef struct {
+	int32_t max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc;
+	float pen_gap, pen_skip;
+	int32_t is_cdna, n_seg, max_dist_inner, cap_rmq_size;
+} mgb_lchain_opt_t;
+int mgb_test_lchain(int mode, int n, const mg128_t *a, const int64_t *off, const int32_t *cnt, const mgb_lchain_opt_t *opt, int32_t *out,
+					uint64_t *u, mg128_t *a_out);
+
 const char *mgb_last_error(void);
 void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st);
 /* knobs: "arena_mb" (per worker), "workers_per_sm", "device"; returns 0 if the key is known */

@@ -107,6 +107,15 @@ PROF_NAMES = ["wfa_fast_cyc", "wfa_fast_n", "wfa_slow_cyc", "wfa_slow_n", "wfa_m
 # mgb_test_wfa_tier(): tier 2 as k_wfa_mid runs it, carrying a gap whose window outgrows the shared-memory ring on in the arena
 # (mgb200.h MGB_TEST_TIER2_CONT)
 WFA_TIER2_CONT = 4
+# mgb_test_lchain(): modes (k_chain DP, k_chain RMQ, k_chain_rescue) and fill paths (mgb200.h)
+LCHAIN_DP, LCHAIN_RMQ, LCHAIN_RESCUE = 0, 1, 2
+LCHAIN_PATH_DP, LCHAIN_PATH_RMQ_W, LCHAIN_PATH_RMQ_TIE, LCHAIN_PATH_RMQ_CAP = 0, 1, 2, 3
+
+
+class mgb_lchain_opt_t(C.Structure):
+    _fields_ = [(k, C.c_int32) for k in ("max_dist_x", "max_dist_y", "bw", "max_skip", "max_iter", "min_cnt", "min_sc")] + \
+               [("pen_gap", C.c_float), ("pen_skip", C.c_float)] + \
+               [(k, C.c_int32) for k in ("is_cdna", "n_seg", "max_dist_inner", "cap_rmq_size")]
 
 
 def bind_mapping_api(lib):
@@ -181,6 +190,8 @@ def bind_engine_api(lib):
     lib.mgb_test_gwfa.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.c_int, C.c_char_p, i64p, i32p, u32p, i32p, u32p, i32p, i32p, i64p, i32p, C.c_int]
     lib.mgb_test_radix128.restype = C.c_int
     lib.mgb_test_radix128.argtypes = [C.POINTER(mg128_t), C.c_int64, C.c_int, C.c_int]
+    lib.mgb_test_lchain.restype = C.c_int
+    lib.mgb_test_lchain.argtypes = [C.c_int, C.c_int, C.POINTER(mg128_t), i64p, i32p, C.POINTER(mgb_lchain_opt_t), i32p, C.POINTER(C.c_uint64), C.POINTER(mg128_t)]
     lib.mg_map_batch_frag.restype = C.c_int
     lib.mg_map_batch_frag.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
                                       C.POINTER(C.POINTER(mg_gchains_t)), C.POINTER(mg_mapopt_t)]

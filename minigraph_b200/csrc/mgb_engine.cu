@@ -2193,4 +2193,130 @@ extern "C" int mgb_test_radix128(mg128_t *a, int64_t n, int walk, int hot_bytes)
 	try { return test_radix128_impl((u128*)a, n, walk, hot_bytes); } catch (const MgbError &e) { return e.code; }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: the linear chaining of k_chain (mode 0: DP, 1: RMQ) or k_chain_rescue (mode 2: sort into target order, RMQ) on
+// anchor sets with options of their own, launched as those kernels are: their stage's warps per block and slice of shared
+// memory per warp, the anchors staged into the slice when they fit (chain_staged, chain_run: the code of stage_chain).  The
+// slices start out filled with junk and each warp chains several sets in a row, so a warp reuses its slice dirty, flips the
+// parity of its barrier and moves between staged and unstaged sets.  Set i goes to worker i % n_workers.
+// ---------------------------------------------------------------------------------------------------------------
+struct TestLchainArgs {
+	int mode, n;
+	u128 *a;              // every set's anchors, chained in place: the compacted anchors are read back from here
+	const int64_t *off;
+	const int32_t *cnt;
+	const LChainOpt *opt;
+	int32_t *out;         // per set: rc, n_u, n_v, staged, path, worker
+	uint64_t *u;          // per set: the chains at u[off[i]..]
+	char *arena;
+	uint64_t arena_bytes;
+};
+MG_HD inline void test_lchain_body(const TestLchainArgs &t, int i, int32_t *smem, uint64_t slice, Arena &A, int worker, int lane)
+{
+	A.top = 0;
+	u128 *a = t.a + t.off[i];
+	const int64_t n = t.cnt[i];
+	const LChainOpt &co = t.opt[i];
+	int32_t n_u = 0, n_v = 0;
+	uint64_t *u = 0;
+	int path = -1, staged = 0;
+	const int rc = chain_staged(smem, slice, A, a, n, lane, &staged, [&](Arena &H, u128 *aw, int32_t *n_keep) {
+		const int r = t.mode == 2? chain_run<1>(H, A, 1, co, n, aw, &n_u, &u, &n_v, lane, &path) : chain_run<0>(H, A, t.mode == 1, co, n, aw, &n_u, &u, &n_v, lane, &path);
+		*n_keep = n_u > 0? n_v : 0;
+		return r;
+	});
+	if (rc == 0) for (int32_t j = lane; j < n_u; j += MGB_W) t.u[t.off[i] + j] = u[j];
+	if (lane == 0) {
+		int32_t *o = t.out + 6 * (int64_t)i;
+		o[0] = rc, o[1] = n_u, o[2] = n_v, o[3] = staged, o[4] = path, o[5] = worker;
+	}
+	warp_sync();
+}
+#ifndef MGB_HOSTSIM
+template<int S>
+__global__ void k_test_lchain(TestLchainArgs t)
+{
+	extern __shared__ int4 dyn_smem[];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+	const int stride = StageSpec<S>::smem;
+	for (int j = threadIdx.x; j < n_warps * stride / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
+	__syncthreads();
+	int32_t *smem = (int32_t*)((char*)dyn_smem + (size_t)warp * stride);
+	chain_smem_init(smem, lane);
+	const int worker = blockIdx.x * n_warps + warp;
+	Arena A;
+	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
+	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_lchain_body(t, i, smem, (uint64_t)stride, A, worker, lane);
+}
+#endif
+
+static int test_lchain_impl(int mode, int n, const u128 *a, const int64_t *off, const int32_t *cnt, const mgb_lchain_opt_t *opt, int32_t *out, uint64_t *u, u128 *a_out)
+{
+#define MGB_SAME_FIELD(f) static_assert(offsetof(mgb_lchain_opt_t, f) == offsetof(LChainOpt, f) && sizeof(mgb_lchain_opt_t::f) == sizeof(LChainOpt::f), "mgb_lchain_opt_t and LChainOpt differ in " #f)
+	MGB_SAME_FIELD(max_dist_x); MGB_SAME_FIELD(max_dist_y); MGB_SAME_FIELD(bw); MGB_SAME_FIELD(max_skip); MGB_SAME_FIELD(max_iter); MGB_SAME_FIELD(min_cnt);
+	MGB_SAME_FIELD(min_sc); MGB_SAME_FIELD(pen_gap); MGB_SAME_FIELD(pen_skip); MGB_SAME_FIELD(is_cdna); MGB_SAME_FIELD(n_seg); MGB_SAME_FIELD(max_dist_inner);
+	MGB_SAME_FIELD(cap_rmq_size);
+#undef MGB_SAME_FIELD
+	static_assert(sizeof(mgb_lchain_opt_t) == sizeof(LChainOpt), "mgb_lchain_opt_t and LChainOpt are the same record");
+	if (mode < 0 || mode > 2 || n < 0) { set_error("mgb_test_lchain: mode 0, 1 or 2 and n at least 0"); return MGB_E_UNSUPPORTED; }
+	int64_t max_cnt = 0;
+	for (int i = 0; i < n; ++i) {
+		if (cnt[i] < 0 || off[i] < 0) { set_error("mgb_test_lchain: set " + std::to_string(i) + " has a negative offset or count"); return MGB_E_UNSUPPORTED; }
+		max_cnt = std::max(max_cnt, (int64_t)cnt[i]);
+	}
+	if (n == 0) return 0;
+	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
+	const int warps = mode == 2? StageSpec<S_CHAIN_RESCUE>::warps : StageSpec<S_CHAIN>::warps;
+	const int stride = mode == 2? StageSpec<S_CHAIN_RESCUE>::smem : StageSpec<S_CHAIN>::smem;
+	const int n_workers = std::min(n, 2 * warps);
+	const int64_t n_a = test_seq_bytes(n, off, cnt);
+	TestLchainArgs t;
+	t.mode = mode, t.n = n;
+	t.a = (u128*)dmalloc(sizeof(u128) * (size_t)(n_a + 1));
+	if (n_a > 0) h2d(t.a, a, sizeof(u128) * (size_t)n_a);
+	t.off = dcopy(off, n), t.cnt = dcopy(cnt, n), t.opt = dcopy((const LChainOpt*)opt, n);
+	t.out = (int32_t*)dmalloc(sizeof(int32_t) * 6 * (size_t)n);
+	t.u = (uint64_t*)dmalloc(sizeof(uint64_t) * (size_t)(n_a + 1));
+	// per anchor at most ~200 bytes: f/p/v/t, the RMQ window, priorities and block summaries, the end-point list, the compaction's
+	// copy, and the two AVL trees of the sequential fill
+	t.arena_bytes = (uint64_t)max_cnt * 512 + ((uint64_t)1 << 20);
+	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
+#ifdef MGB_HOSTSIM
+	std::vector<uint32_t> sim_smem((size_t)n_workers * stride / 4, TEST_SMEM_FILL);
+	auto slice = [&](int w) { return (int32_t*)((char*)sim_smem.data() + (size_t)w * stride); };
+	auto on_warp = [&](int w, const std::function<void(Arena &, int)> &fn) {
+#if MGB_W > 1
+		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, t.arena + (uint64_t)w * t.arena_bytes, t.arena_bytes); fn(A, lane); });
+#else
+		Arena A;
+		arena_init(A, t.arena + (uint64_t)w * t.arena_bytes, t.arena_bytes);
+		fn(A, 0);
+#endif
+	};
+	for (int w = 0; w < n_workers; ++w) on_warp(w, [&](Arena &, int lane) { chain_smem_init(slice(w), lane); });
+	for (int i = 0; i < n; ++i) {
+		const int w = i % n_workers;
+		on_warp(w, [&](Arena &A, int lane) { test_lchain_body(t, i, slice(w), (uint64_t)stride, A, w, lane); });
+	}
+#else
+	const size_t smem = (size_t)warps * stride;
+	void (*kern)(TestLchainArgs) = mode == 2? k_test_lchain<S_CHAIN_RESCUE> : k_test_lchain<S_CHAIN>;
+	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+	kern<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
+	CUDA_OK(cudaGetLastError());
+	dsync();
+#endif
+	d2h(out, t.out, sizeof(int32_t) * 6 * (size_t)n);
+	d2h(u, t.u, sizeof(uint64_t) * (size_t)n_a);
+	d2h(a_out, t.a, sizeof(u128) * (size_t)n_a);
+	dfree(t.a), dfree((void*)t.off), dfree((void*)t.cnt), dfree((void*)t.opt), dfree(t.out), dfree(t.u), dfree(t.arena);
+	return 0;
+}
+
+extern "C" int mgb_test_lchain(int mode, int n, const mg128_t *a, const int64_t *off, const int32_t *cnt, const mgb_lchain_opt_t *opt, int32_t *out,
+							   uint64_t *u, mg128_t *a_out)
+{
+	try { return test_lchain_impl(mode, n, (const u128*)a, off, cnt, opt, out, u, (u128*)a_out); } catch (const MgbError &e) { return e.code; }
+}
+
 extern "C" void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st) { *st = t_has_stats? t_last_stats : model_of(gi)->stats; } // the calling thread's last batch

@@ -624,10 +624,14 @@ MG_HD inline int chain_rmq_fill_w(Arena &H, Arena &A, int max_dist, int max_dist
 	return 0;
 }
 
+// How chain_rmq_w() filled f/p/v (reported to the tests through its `path` argument)
+enum { CHAIN_PATH_DP = 0, CHAIN_PATH_RMQ_W = 1, CHAIN_PATH_RMQ_TIE = 2, CHAIN_PATH_RMQ_CAP = 3 };
+
 // Warp-uniform RMQ chaining: same contract as chain_rmq(); all lanes enter with identical arguments and leave with
-// identical results (outputs are broadcast from lane 0, which runs the sequential backtrack/compaction).
+// identical results (outputs are broadcast from lane 0, which runs the sequential backtrack/compaction).  path (may be NULL):
+// CHAIN_PATH_RMQ_W when the cooperative fill ran, _TIE when it gave up on a priority tie, _CAP when n > cap_rmq_size.
 MG_HD inline int chain_rmq_w(Arena &H, Arena &A, int max_dist, int max_dist_inner, int bw, int max_chn_skip, int cap_rmq_size, int min_cnt, int min_sc,
-							 float pen_gap, float pen_skip, int64_t n, u128 *a, int32_t *n_u_, uint64_t **u_, int32_t *n_a_, int lane)
+							 float pen_gap, float pen_skip, int64_t n, u128 *a, int32_t *n_u_, uint64_t **u_, int32_t *n_a_, int lane, int *path = 0)
 {
 	int32_t *f, *t, *v, *p;
 	*u_ = 0, *n_u_ = 0, *n_a_ = 0;
@@ -644,6 +648,7 @@ MG_HD inline int chain_rmq_w(Arena &H, Arena &A, int max_dist, int max_dist_inne
 	MGB_ALLOC_HOT(H, A, v, int32_t, n);
 	int rc = n <= cap_rmq_size? chain_rmq_fill_w(H, A, max_dist, max_dist_inner, bw, max_chn_skip, pen_gap, pen_skip, n, a, f, p, t, v, lane) : 1;
 	if (rc < 0) return rc;
+	if (path) *path = n > cap_rmq_size? CHAIN_PATH_RMQ_CAP : rc == 1? CHAIN_PATH_RMQ_TIE : CHAIN_PATH_RMQ_W;
 	int32_t n_u = 0, n_v = 0;
 	if (rc == 1) { // too many anchors for the cooperative fill: sequential replay on one lane
 		int rc2 = 0;

@@ -260,6 +260,33 @@ struct ChainRun { // what one pass leaves behind
 	int32_t rescue;   // pass 0: the read goes on the rescue list
 };
 
+// The arguments of one chaining call (reference: mg_lchain_dp / mg_lchain_rmq); the RMQ chaining takes max_dist_x as its max_dist
+// and ignores max_dist_y, max_iter, is_cdna and n_seg, the DP ignores max_dist_inner and cap_rmq_size.
+struct LChainOpt {
+	int32_t max_dist_x, max_dist_y, bw, max_skip, max_iter, min_cnt, min_sc;
+	float pen_gap, pen_skip;
+	int32_t is_cdna, n_seg, max_dist_inner, cap_rmq_size;
+};
+
+// The chaining of one pass on a read's anchors a[0..n_a) (reference: map-algo.c:386-392, 413-415): pass 0 chains them in target
+// order by DP (lr) or by RMQ (asm, rmq != 0); pass 1 sorts the anchors it was handed back into target order and chains them by RMQ.
+// The n_u chains go to u (score<<32 | anchors), their anchors to a[0..n_v).  path (may be NULL): which fill ran, CHAIN_PATH_*.
+template<int PASS>
+MG_HD inline int chain_run(Arena &H, Arena &A, int rmq, const LChainOpt &co, int64_t n_a, u128 *a, int32_t *n_u, uint64_t **u, int32_t *n_v, int lane,
+						   int *path = 0)
+{
+	if (PASS == 1) { // back into target order; the sort's range stack and bin tables on chip when the slice has the room (it is empty but for the anchors)
+		Arena &S = H.cap - H.top >= (uint64_t)n_a / 4 + 3400? H : A;
+		MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, 0, false)); // (in place: the list is on chip, where the digit walk was slower)
+	}
+	if (PASS == 1 || rmq)
+		return chain_rmq_w(H, A, co.max_dist_x, co.max_dist_inner, co.bw, co.max_skip, co.cap_rmq_size, co.min_cnt, co.min_sc, co.pen_gap, co.pen_skip,
+						   n_a, a, n_u, u, n_v, lane, path);
+	if (path && n_a > 0) *path = CHAIN_PATH_DP;
+	return chain_dp_w(H, A, co.max_dist_x, co.max_dist_y, co.bw, co.max_skip, co.max_iter, co.min_cnt, co.min_sc, co.pen_gap, co.pen_skip, co.is_cdna,
+					  co.n_seg, n_a, a, n_u, u, n_v, lane);
+}
+
 template<int PASS>
 MG_HD inline int chain_pass(const PipeCtx &c, int rid, Arena &H, Arena &A, u128 *a, int64_t n_a, int lane, ChainRun *run)
 {
@@ -283,13 +310,12 @@ MG_HD inline int chain_pass(const PipeCtx &c, int rid, Arena &H, Arena &A, u128 
 			if (max_gap_ref < o.max_gap) max_gap_ref = o.max_gap;
 		} else max_gap_ref = o.max_gap;
 		if (n_a > 0) {
-			if (o.flag & F_RMQ) {
-				MGB_TRY(chain_rmq_w(H, A, o.max_gap, o.max_gap_pre, o.bw, o.max_lc_skip, o.rmq_size_cap, o.min_lc_cnt, o.min_lc_score,
-									o.chn_pen_gap, o.chn_pen_skip, n_a, a, &n_lc, &u, &n_a_new, lane));
-			} else {
-				MGB_TRY(chain_dp_w(H, A, max_gap_ref, max_gap_qry, o.bw, o.max_lc_skip, o.max_lc_iter, o.min_lc_cnt, o.min_lc_score,
-								   o.chn_pen_gap, o.chn_pen_skip, is_splice, batch_n_seg(c.b, rid), n_a, a, &n_lc, &u, &n_a_new, lane));
-			}
+			const int rmq = !!(o.flag & F_RMQ);
+			LChainOpt co;
+			co.max_dist_x = rmq? o.max_gap : max_gap_ref, co.max_dist_y = max_gap_qry, co.bw = o.bw, co.max_skip = o.max_lc_skip, co.max_iter = o.max_lc_iter;
+			co.min_cnt = o.min_lc_cnt, co.min_sc = o.min_lc_score, co.pen_gap = o.chn_pen_gap, co.pen_skip = o.chn_pen_skip;
+			co.is_cdna = is_splice, co.n_seg = batch_n_seg(c.b, rid), co.max_dist_inner = o.max_gap_pre, co.cap_rmq_size = o.rmq_size_cap;
+			MGB_TRY(chain_run<0>(H, A, rmq, co, n_a, a, &n_lc, &u, &n_a_new, lane));
 		}
 		if (lane == 0) m.n_u0 = n_lc, prof_add(c, PROF_CHAIN_DP_CYC, prof_clock() - t0);
 		// long-join rescue (reference: map-algo.c:407-417)
@@ -313,12 +339,11 @@ MG_HD inline int chain_pass(const PipeCtx &c, int rid, Arena &H, Arena &A, u128 
 			}
 		}
 	} else {
-		{ // back into target order; the sort's range stack and bin tables on chip when the slice has the room (it is empty but for the anchors)
-			Arena &S = H.cap - H.top >= (uint64_t)n_a / 4 + 3400? H : A;
-			MGB_TRY(radix_sort_128x_w(S, a, n_a, lane, 0, false)); // (in place: the list is on chip, where the digit walk was slower)
-		}
-		MGB_TRY(chain_rmq_w(H, A, o.max_gap, o.max_gap_pre, o.bw_long, o.max_lc_skip, o.rmq_size_cap, o.min_lc_cnt, o.min_lc_score,
-							o.chn_pen_gap, o.chn_pen_skip, n_a, a, &n_lc, &u, &n_a_new, lane));
+		LChainOpt co;
+		co.max_dist_x = o.max_gap, co.max_dist_y = 0, co.bw = o.bw_long, co.max_skip = o.max_lc_skip, co.max_iter = 0;
+		co.min_cnt = o.min_lc_cnt, co.min_sc = o.min_lc_score, co.pen_gap = o.chn_pen_gap, co.pen_skip = o.chn_pen_skip;
+		co.is_cdna = 0, co.n_seg = 1, co.max_dist_inner = o.max_gap_pre, co.cap_rmq_size = o.rmq_size_cap;
+		MGB_TRY(chain_run<1>(H, A, 1, co, n_a, a, &n_lc, &u, &n_a_new, lane));
 		if (lane == 0) prof_add(c, PROF_CHAIN_RMQ_CYC, prof_clock() - t0);
 	}
 	unsigned long long t2 = prof_clock();
@@ -358,16 +383,16 @@ MG_HD inline void chain_smem_init(int32_t *smem, int lane)
 	warp_sync();
 }
 
-template<int PASS>
-MG_HD inline int stage_chain(const PipeCtx &c, int rid, Arena &A, int lane, int32_t *smem)
+// A read's anchors a[0..n_a) in HBM, worked on in the warp's slice of `slice` bytes (NULL: no slice): staged there by one bulk copy
+// when they fit, the rest of the slice as the hot arena.  run(H, aw, &n_keep) chains the anchors aw[] (the staged copy or a[] itself)
+// and returns its code; the first n_keep of them are stored back to a[] by one bulk copy.  *staged: whether the anchors went on chip.
+template<typename Run>
+MG_HD inline int chain_staged(int32_t *smem, uint64_t slice, Arena &A, u128 *a, int64_t n_a, int lane, int *staged_, Run &&run)
 {
-	ReadMeta &m = c.meta[rid];
-	if (m.status != 0) return 0;
-	u128 *a = c.anchor + m.a_off;
-	const int64_t n_a = m.n_a;
-	ChainRun run;
-	if (smem == 0 || n_a == 0) return chain_pass<PASS>(c, rid, A, A, a, n_a, lane, &run);
-	const uint64_t slice = PASS == 0? CHAIN_SMEM_BYTES : CHAIN_RESCUE_SMEM_BYTES, a_bytes = (uint64_t)n_a * sizeof(u128);
+	int32_t n_keep = 0;
+	*staged_ = 0;
+	if (smem == 0 || n_a == 0) return run(A, a, &n_keep);
+	const uint64_t a_bytes = (uint64_t)n_a * sizeof(u128);
 	const int staged = a_bytes + 16 <= slice;
 	uint64_t *bar = (uint64_t*)smem;
 	u128 *as = (u128*)((char*)smem + 16);
@@ -380,12 +405,31 @@ MG_HD inline int stage_chain(const PipeCtx &c, int rid, Arena &A, int lane, int3
 	}
 	Arena S; // what is left of the slice
 	arena_init(S, (char*)as + (staged? a_bytes : 0), slice - 16 - (staged? a_bytes : 0));
-	const int rc = chain_pass<PASS>(c, rid, S, A, staged? as : a, n_a, lane, &run);
-	if (staged && rc == 0 && run.n_keep > 0) {
+	const int rc = run(S, staged? as : a, &n_keep);
+	if (staged && rc == 0 && n_keep > 0) {
 		warp_sync();
-		if (lane == 0) { bulk_store(a, as, (uint32_t)run.n_keep * (uint32_t)sizeof(u128)); bulk_store_wait(); }
+		if (lane == 0) { bulk_store(a, as, (uint32_t)n_keep * (uint32_t)sizeof(u128)); bulk_store_wait(); }
 		warp_sync();
 	}
+	*staged_ = staged;
+	return rc;
+}
+
+template<int PASS>
+MG_HD inline int stage_chain(const PipeCtx &c, int rid, Arena &A, int lane, int32_t *smem)
+{
+	ReadMeta &m = c.meta[rid];
+	if (m.status != 0) return 0;
+	u128 *a = c.anchor + m.a_off;
+	const int64_t n_a = m.n_a;
+	int staged;
+	const int rc = chain_staged(smem, PASS == 0? CHAIN_SMEM_BYTES : CHAIN_RESCUE_SMEM_BYTES, A, a, n_a, lane, &staged,
+								[&](Arena &H, u128 *aw, int32_t *n_keep) {
+									ChainRun run;
+									const int r = chain_pass<PASS>(c, rid, H, A, aw, n_a, lane, &run);
+									*n_keep = run.n_keep;
+									return r;
+								});
 	if (staged && lane == 0 && c.prof) prof_add(c, PROF_CHAIN_BT_CYC, 1); // reads whose anchors were chained on chip
 	return rc;
 }
