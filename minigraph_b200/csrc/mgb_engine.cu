@@ -1,9 +1,10 @@
 // mgb_engine.cu -- host side of libmgb200.so: model construction, batch dispatcher and the C ABI (include/mgb200.h).
 //
 // Compiled by nvcc for sm_90a (H100) into the product library.  With -DMGB_HOSTSIM the same file is compiled by g++ into
-// tests/hostsim/libmgb_hostsim.so, where "device memory" is host memory and a "launch" is a loop over reads with a
-// single lane: that build exists only so that the CPU-only unit tests can exercise the control flow of the kernels.
-// It is never loaded by the product path; the product library refuses to work without a CUDA device.
+// the simulators of tests/hostsim, where "device memory" is host memory and a "launch" is a loop over the items, each run by
+// one simulated warp: a single lane in libmgb_hostsim.so, 32 lanes as fibres in libmgb_hostsim32.so (-DMGB_SIM_LANES=32,
+// mgb_simlanes.h).  Those builds exist only so that the CPU-only unit tests can exercise the control flow of the kernels.
+// They are never loaded by the product path; the product library refuses to work without a CUDA device.
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -107,10 +108,22 @@ static int dev_sm_count() { static int v = 0; if (v == 0) { int d = 0; CUDA_OK(c
 static size_t dev_free_mem() { size_t f = 0, t = 0; CUDA_OK(cudaMemGetInfo(&f, &t)); return f; }
 #endif
 
-template<typename T> static T *dalloc_copy(const std::vector<T> &v)
+// n elements of device memory, freed when the holder goes out of scope (also when a CUDA call throws) unless release()d
+template<typename T> struct DevBuf {
+	T *p;
+	explicit DevBuf(size_t n) : p((T*)dmalloc(n * sizeof(T))) {}
+	DevBuf(DevBuf &&o) : p(o.p) { o.p = 0; }
+	DevBuf(const DevBuf &) = delete;
+	DevBuf &operator=(const DevBuf &) = delete;
+	~DevBuf() { dfree((void*)p); }
+	operator T*() const { return p; }
+	T *release() { T *r = p; p = 0; return r; }
+};
+// a device copy of the host array h[0..n)
+template<typename T> static DevBuf<T> upload(const T *h, size_t n)
 {
-	T *d = (T*)dmalloc(v.size() * sizeof(T));
-	h2d(d, v.data(), v.size() * sizeof(T));
+	DevBuf<T> d(n);
+	h2d(d, h, n * sizeof(T));
 	return d;
 }
 
@@ -235,6 +248,14 @@ MG_HD inline void stage_fail(const LaunchArgs &L, int item, int rc)
 	L.routs[rid].status = rc;
 }
 
+// What a warp of stage S does to its slice of shared memory before its first item (S < 0: nothing).  Warp-uniform.
+template<int S>
+MG_HD inline void stage_warp_init(int32_t *smem, int lane)
+{
+	if (S == S_CHAIN || S == S_CHAIN_RESCUE) chain_smem_init(smem, lane);
+	if ((S == S_WFA_SMALL || S == S_WFA_MID) && lane == 0) { unsigned long long *ck = wfa_cig_chunk(smem, S == S_WFA_SMALL? 1 : 2); ck[0] = ck[1] = 0; } // no slice of the CIGAR pool yet
+}
+
 #ifndef MGB_HOSTSIM
 // One warp per work item; items are pulled from a global counter so that long items do not stall a wave.
 // Every mapping stage is warp-uniform (all lanes enter the stage function, see mgb_common.cuh).
@@ -248,8 +269,7 @@ __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 	arena_init(A, L.arena_base + (uint64_t)worker * L.arena_bytes, L.arena_bytes);
 	extern __shared__ int4 dyn_smem[];
 	int32_t *smem = Spec::smem? (int32_t*)((char*)dyn_smem + (size_t)(threadIdx.x >> 5) * Spec::smem) : 0;
-	if (S == S_CHAIN || S == S_CHAIN_RESCUE) chain_smem_init(smem, lane);
-	if ((S == S_WFA_SMALL || S == S_WFA_MID) && lane == 0) { unsigned long long *ck = wfa_cig_chunk(smem, S == S_WFA_SMALL? 1 : 2); ck[0] = ck[1] = 0; } // no slice of the CIGAR pool yet
+	stage_warp_init<S>(smem, lane);
 	prof_block_begin();
 	const int n_work = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
 	int next_item = 0, have = 0;
@@ -590,6 +610,25 @@ struct Workers {
 	uint64_t *peak;
 };
 
+#ifdef MGB_HOSTSIM
+// Runs fn(lane) on the MGB_W lanes of one simulated warp, which works on `item` of `stage` (for the simulator's messages), and
+// returns lane 0's code; sets *differ when another lane returned a different one.
+template<typename F>
+static int sim_warp(int stage, int item, const F &fn, bool *differ)
+{
+#if MGB_W > 1
+	int rcs[MGB_W];
+	sim::tag()[0] = stage, sim::tag()[1] = item;
+	sim::run_warp(MGB_W, [&](int lane) { rcs[lane] = fn(lane); });
+	for (int l = 1; l < MGB_W; ++l) if (rcs[l] != rcs[0]) *differ = true;
+	return rcs[0];
+#else
+	(void)stage, (void)item, (void)differ;
+	return fn(0);
+#endif
+}
+#endif
+
 template<int S>
 static void launch_stage(LaunchArgs &L, const Workers &W)
 {
@@ -601,28 +640,20 @@ static void launch_stage(LaunchArgs &L, const Workers &W)
 	arena_init(A, W.arena, Spec::mode == ItemMode::THREAD? (W.arena_bytes / 32) & ~(uint64_t)15 : W.arena_bytes); // one item per thread: a thread's share, as on the device
 	std::vector<int32_t> sim_smem(Spec::smem / 4);
 	int32_t *smem = Spec::mode == ItemMode::WARP && Spec::smem? sim_smem.data() : 0; // the slice of one warp, as on the device
-	if (S == S_CHAIN || S == S_CHAIN_RESCUE) { mbar_init((uint64_t*)smem, 1); smem[2] = 0; }
+	bool differ = false;
+	sim_warp(S, -1, [&](int lane) { stage_warp_init<S>(smem, lane); return 0; }, &differ);
 	const int n_work_sim = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
 	for (int it = 0; it < n_work_sim; ++it) {
 		int item = L.rid_list? L.rid_list[it] : it;
 		A.top = 0;
-		int rc;
-#if MGB_W > 1
-		if (Spec::mode == ItemMode::WARP) { // all lanes of the simulated warp enter, each with its own copy of the arena header (as in registers on the device)
-			int rcs[MGB_W];
-			uint64_t peaks[MGB_W];
-			sim::tag()[0] = S, sim::tag()[1] = item;
-			sim::run_warp(MGB_W, [&](int lane) {
-				Arena Al = A;
-				rcs[lane] = run_stage<S>(L, item, Al, lane, smem);
-				peaks[lane] = Al.peak;
-			});
-			rc = rcs[0];
-			for (int l = 1; l < MGB_W; ++l) if (rcs[l] != rc) { set_error("simulated warp: lanes returned different codes from one stage"); abort(); }
-			for (int l = 0; l < MGB_W; ++l) if (peaks[l] > A.peak) A.peak = peaks[l];
-		} else
-#endif
-		rc = run_stage<S>(L, item, A, 0, smem);
+		// a WARP item: all lanes of the simulated warp enter, each with its own copy of the arena header (as in registers on the device)
+		const int rc = Spec::mode != ItemMode::WARP? run_stage<S>(L, item, A, 0, smem) : sim_warp(S, item, [&](int lane) {
+			Arena Al = A;
+			const int r = run_stage<S>(L, item, Al, lane, smem);
+			A.peak = std::max(A.peak, Al.peak);
+			return r;
+		}, &differ);
+		if (differ) { set_error("simulated warp: lanes returned different codes from one stage"); abort(); }
 		if (rc < 0 && getenv("MGB_HOSTSIM_TRACE")) fprintf(stderr, "[hostsim] stage %d item %d failed with %d\n", S, item, rc);
 		if (rc < 0) stage_fail<S>(L, item, rc);
 	}
@@ -799,13 +830,13 @@ static Model *model_build(gfa_t *g, int k, int w)
 	}
 	// upload the graph
 	M->g.n_seg = (int32_t)n_seg;
-	M->g.seg_name_id = dalloc_copy(M->seg_name_id), M->dev_ptrs.push_back((void*)M->g.seg_name_id);
-	M->g.seg_soff = dalloc_copy(M->seg_soff), M->dev_ptrs.push_back((void*)M->g.seg_soff);
-	M->g.seg_len = dalloc_copy(M->seg_len), M->dev_ptrs.push_back((void*)M->g.seg_len);
-	M->g.vseq_off = dalloc_copy(M->vseq_off), M->dev_ptrs.push_back((void*)M->g.vseq_off);
-	M->g.seq = dalloc_copy(M->seq), M->dev_ptrs.push_back((void*)M->g.seq);
-	M->g.arc_idx = dalloc_copy(M->arc_idx), M->dev_ptrs.push_back((void*)M->g.arc_idx);
-	M->g.arc = dalloc_copy(M->arc), M->dev_ptrs.push_back((void*)M->g.arc);
+	M->g.seg_name_id = upload(M->seg_name_id.data(), M->seg_name_id.size()).release(), M->dev_ptrs.push_back((void*)M->g.seg_name_id);
+	M->g.seg_soff = upload(M->seg_soff.data(), M->seg_soff.size()).release(), M->dev_ptrs.push_back((void*)M->g.seg_soff);
+	M->g.seg_len = upload(M->seg_len.data(), M->seg_len.size()).release(), M->dev_ptrs.push_back((void*)M->g.seg_len);
+	M->g.vseq_off = upload(M->vseq_off.data(), M->vseq_off.size()).release(), M->dev_ptrs.push_back((void*)M->g.vseq_off);
+	M->g.seq = upload(M->seq.data(), M->seq.size()).release(), M->dev_ptrs.push_back((void*)M->g.seq);
+	M->g.arc_idx = upload(M->arc_idx.data(), M->arc_idx.size()).release(), M->dev_ptrs.push_back((void*)M->g.arc_idx);
+	M->g.arc = upload(M->arc.data(), M->arc.size()).release(), M->dev_ptrs.push_back((void*)M->g.arc);
 	M->ix.k = k, M->ix.w = w, M->ix.slot = 0, M->ix.pos = 0, M->ix.n_slots_mask = 0;
 
 	// sketch every segment on the device (K1 reused), then build the table: on the device (the simulators: on the host)
@@ -897,8 +928,8 @@ static Model *model_build(gfa_t *g, int k, int w)
 		i = j;
 	}
 	M->ix.n_slots_mask = M->n_slots_mask;
-	M->ix.slot = dalloc_copy(M->slot), M->dev_ptrs.push_back((void*)M->ix.slot);
-	M->ix.pos = dalloc_copy(M->pos), M->dev_ptrs.push_back((void*)M->ix.pos);
+	M->ix.slot = upload(M->slot.data(), M->slot.size()).release(), M->dev_ptrs.push_back((void*)M->ix.slot);
+	M->ix.pos = upload(M->pos.data(), M->pos.size()).release(), M->dev_ptrs.push_back((void*)M->ix.pos);
 #endif
 	return M;
 }
@@ -1691,7 +1722,7 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 				M->logf_tab.resize(need);
 				for (int i = 0; i < need; ++i) M->logf_tab[i] = logf((float)i);
 				if (M->d_logf) M->dev_ptrs.push_back(M->d_logf); // a call in flight may still read it
-				M->d_logf = dalloc_copy(M->logf_tab);
+				M->d_logf = upload(M->logf_tab.data(), M->logf_tab.size()).release();
 				M->n_logf = need;
 			}
 			o.logf_tab = M->d_logf, o.n_logf_tab = M->n_logf;
@@ -1840,51 +1871,104 @@ extern "C" mg_gchains_t *mg_map(const mg_idx_t *gi, int qlen, const char *seq, m
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// test hook: one gap alignment through the tier-3 path (exact WFA capped at max_iter cells, then the chaining
-// heuristic with low-memory checkpoints every `step` scores), reference: miniwfa.c:824-834 mwf_wfa_auto
+// test hooks: one piece of device code run on inputs from the tests, launched as its pipeline kernel launches it
 // ---------------------------------------------------------------------------------------------------------------
-struct TestWfaArgs { const char *ts, *qs; int32_t tl, ql, step, cap; int64_t max_iter; uint32_t *cigar; int32_t *out; char *arena; uint64_t arena_bytes; };
-MG_HD inline void test_wfa_body(const TestWfaArgs &t, int lane)
-{
-	Arena A;
-	arena_init(A, t.arena, t.arena_bytes);
-	WfResult r;
-	int rc = wfa_exact(A, t.tl, t.ts, t.ql, t.qs, t.max_iter, &r, lane, t.step);
-	if (rc == 0 && r.n_cigar <= t.cap) for (int32_t i = lane; i < r.n_cigar; i += MGB_W) t.cigar[i] = r.cigar[i];
-	if (lane == 0) t.out[0] = rc, t.out[1] = rc == 0? r.n_cigar : 0, t.out[2] = rc == 0? r.s : 0;
-}
+static const int NO_STAGE = -1;                              // a hook that mirrors no stage: its slice is not set up
+static const uint32_t TEST_SMEM_FILL = 0x00050005u;          // two cells holding offset 5, a value a real wavefront holds
+
+// A hook's body(i, slice, A, worker, lane) runs item i on all lanes of a warp, with the warp's slice of shared memory (NULL: none),
+// its arena and its number, and returns a code on which the lanes agree.
 #ifndef MGB_HOSTSIM
-__global__ void k_test_wfa(TestWfaArgs t) { test_wfa_body(t, threadIdx.x & 31); }
-#endif
-static int test_wfa_impl(const char *ts, int tl, const char *qs, int ql, int64_t max_iter, int step, uint32_t *cigar, int cap, int *score)
+template<int S, typename Body>
+__global__ void k_test(Body body, int n, int smem, char *arena, uint64_t arena_bytes)
 {
-	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	TestWfaArgs t;
-	t.tl = tl, t.ql = ql, t.step = step, t.cap = cap, t.max_iter = max_iter, t.arena_bytes = (uint64_t)1 << 30;
-	char *d_ts = (char*)dmalloc((size_t)tl + 64), *d_qs = (char*)dmalloc((size_t)ql + 64);
-	h2d(d_ts, ts, (size_t)tl), h2d(d_qs, qs, (size_t)ql);
-	t.ts = d_ts, t.qs = d_qs;
-	t.cigar = (uint32_t*)dmalloc(sizeof(uint32_t) * (size_t)cap);
-	t.out = (int32_t*)dmalloc(sizeof(int32_t) * 4);
-	t.arena = (char*)dmalloc(t.arena_bytes);
-	int32_t out[4] = {0, 0, 0, 0};
-	{
-#ifdef MGB_HOSTSIM
-#if MGB_W > 1
-	sim::run_warp(MGB_W, [&](int lane) { test_wfa_body(t, lane); });
-#else
-	test_wfa_body(t, 0);
+	extern __shared__ int4 dyn_smem[];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
+	for (int j = threadIdx.x; j < n_warps * smem / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
+	__syncthreads();
+	int32_t *slice = smem? (int32_t*)((char*)dyn_smem + (size_t)warp * smem) : 0;
+	stage_warp_init<S>(slice, lane);
+	const int worker = blockIdx.x * n_warps + warp;
+	Arena A;
+	arena_init(A, arena + (uint64_t)worker * arena_bytes, arena_bytes);
+	for (int i = worker; i < n; i += gridDim.x * n_warps) body(i, slice, A, worker, lane);
+}
 #endif
+
+// Runs body on items 0..n-1 in blocks of `warps` warps (by default stage S's) with `smem` bytes of shared memory per warp (by default
+// stage S's slice), n_workers warps rounded up to whole blocks.  Each warp's slice starts out filled with junk and is then set up as
+// stage S sets it up; each warp has an arena of arena_bytes.  Warp w runs items w, w + (warps launched), ... in this order, so that
+// the results also show that a warp reuses its slice dirty and keeps to its own.  The simulators run the warps one after the
+// other, each on its own slice and arena.  Returns 0, or MGB_E_INTERNAL when the lanes of a simulated warp returned different codes.
+template<int S, typename Body>
+static int test_launch(int n, int n_workers, uint64_t arena_bytes, const Body &body, int warps = StageSpec<S>::warps, int smem = StageSpec<S>::smem)
+{
+	const int blocks = (n_workers + warps - 1) / warps, n_warps = blocks * warps;
+	DevBuf<char> arena((size_t)arena_bytes * n_warps);
+#ifdef MGB_HOSTSIM
+	std::vector<uint32_t> sim_smem((size_t)n_warps * smem / 4 + 1, TEST_SMEM_FILL);
+	bool differ = false;
+	for (int w = 0; w < n_warps; ++w) {
+		int32_t *slice = smem? (int32_t*)((char*)sim_smem.data() + (size_t)w * smem) : 0;
+		sim_warp(S, -1, [&](int lane) { stage_warp_init<S>(slice, lane); return 0; }, &differ);
+		for (int i = w; i < n; i += n_warps)
+			sim_warp(S, i, [&](int lane) { Arena A; arena_init(A, arena + (uint64_t)w * arena_bytes, arena_bytes); return body(i, slice, A, w, lane); }, &differ);
+	}
+	if (differ) { set_error("simulated warp: lanes returned different codes from a test hook"); return MGB_E_INTERNAL; }
 #else
-	k_test_wfa<<<1, 32>>>(t);
+	const size_t smem_b = (size_t)warps * smem;
+	if (smem_b > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test<S, Body>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
+	k_test<S, Body><<<blocks, warps * 32, smem_b, t_stream>>>(body, n, smem, arena, arena_bytes);
 	CUDA_OK(cudaGetLastError());
 	dsync();
 #endif
-	d2h(out, t.out, sizeof(out));
+	return 0;
+}
+
+// the hooks run only where their kernels run
+static int test_no_device(int dev = -1)
+{
+	if (dev_ok(dev)) return 0;
+	set_error("no CUDA device available: libmgb200 has no CPU path");
+	return -100;
+}
+
+static int64_t test_seq_bytes(int n, const int64_t *off, const int32_t *len)
+{
+	int64_t end = 0;
+	for (int i = 0; i < n; ++i) end = std::max(end, off[i] + len[i]);
+	return end;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: one gap alignment through the tier-3 path (exact WFA capped at max_iter cells, then the chaining
+// heuristic with low-memory checkpoints every `step` scores), reference: miniwfa.c:824-834 mwf_wfa_auto
+// ---------------------------------------------------------------------------------------------------------------
+struct TestWfa {
+	const char *ts, *qs; int32_t tl, ql, step, cap; int64_t max_iter; uint32_t *cigar; int32_t *out;
+	MG_HD int operator()(int, int32_t *, Arena &A, int, int lane) const
+	{
+		WfResult r;
+		int rc = wfa_exact(A, tl, ts, ql, qs, max_iter, &r, lane, step);
+		if (rc == 0 && r.n_cigar <= cap) for (int32_t i = lane; i < r.n_cigar; i += MGB_W) cigar[i] = r.cigar[i];
+		if (lane == 0) out[0] = rc, out[1] = rc == 0? r.n_cigar : 0, out[2] = rc == 0? r.s : 0;
+		return 0;
 	}
-	if (out[0] == 0 && out[1] <= cap) d2h(cigar, t.cigar, sizeof(uint32_t) * (size_t)out[1]);
+};
+static int test_wfa_impl(const char *ts, int tl, const char *qs, int ql, int64_t max_iter, int step, uint32_t *cigar, int cap, int *score)
+{
+	if (int e = test_no_device()) return e;
+	DevBuf<char> ts_d((size_t)tl + 64), qs_d((size_t)ql + 64);
+	h2d(ts_d, ts, (size_t)tl), h2d(qs_d, qs, (size_t)ql);
+	DevBuf<uint32_t> cigar_d(cap);
+	DevBuf<int32_t> out_d(4);
+	TestWfa t;
+	t.ts = ts_d, t.qs = qs_d, t.tl = tl, t.ql = ql, t.step = step, t.cap = cap, t.max_iter = max_iter, t.cigar = cigar_d, t.out = out_d;
+	if (int e = test_launch<NO_STAGE>(1, 1, (uint64_t)1 << 30, t, 1, 0)) return e;
+	int32_t out[4] = {0, 0, 0, 0};
+	d2h(out, out_d, sizeof(out));
+	if (out[0] == 0 && out[1] <= cap) d2h(cigar, cigar_d, sizeof(uint32_t) * (size_t)out[1]);
 	*score = out[2];
-	dfree(d_ts), dfree(d_qs), dfree(t.cigar), dfree(t.out), dfree(t.arena);
 	return out[0] < 0? out[0] : out[1];
 }
 
@@ -1895,69 +1979,35 @@ extern "C" int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int6
 
 // ---------------------------------------------------------------------------------------------------------------
 // test hook: a batch of gaps through one on-chip WFA tier, wfa_smem() with the template arguments of k_wfa_small (tier 1)
-// or k_wfa_mid (tier 2), launched as those kernels are: their stage's warps per block and slice of shared memory per warp, one
-// gap per warp at a time.  The shared memory starts out filled with cells that are not -inf,
-// and a warp aligns several gaps in a row, so the results also show that wfa_smem() clears the slices it reads and that the
-// warps of a block keep to their own slices.
+// or k_wfa_mid (tier 2), launched as those kernels are (test_launch).  The junk in the slices is cells that are not -inf, so the
+// results also show that wfa_smem() clears the slices it reads.
 // ---------------------------------------------------------------------------------------------------------------
-static const uint32_t TEST_SMEM_FILL = 0x00050005u; // two cells holding offset 5, a value a real wavefront holds
-struct TestTierArgs {
-	int tier, n, cap;
+struct TestTier {
+	int tier, cap;
 	const char *ts, *qs;
 	const int64_t *t_off, *q_off;
 	const int32_t *tl, *ql;
 	int64_t *out;       // per gap: rc (0: aligned, 1: does not fit the tier), score, n_iter, n_cigar
 	uint32_t *cigar;    // per gap: cap entries
-	char *arena;
-	uint64_t arena_bytes;
-};
-MG_HD inline void test_wfa_tier_body(const TestTierArgs &t, int i, int32_t *smem, Arena &A, int lane)
-{
-	WfResult r;
-	A.top = 0;
-	const char *ts = t.ts + t.t_off[i], *qs = t.qs + t.q_off[i];
-	int64_t cont_cells = 0;
-	int rc = t.tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane)
-			: t.tier == 2? wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane)
-						: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, t.tl[i], ts, t.ql[i], qs, &r, lane, &cont_cells);
-	if (rc == 0 && r.n_cigar > t.cap) rc = MGB_E_INTERNAL;
-	if (rc == 0) for (int32_t j = lane; j < r.n_cigar; j += MGB_W) t.cigar[(int64_t)i * t.cap + j] = r.cigar[j];
-	if (lane == 0) {
-		int64_t *o = t.out + 4 * (int64_t)i;
-		o[0] = rc, o[1] = rc == 0? r.s : -1, o[2] = rc == 0? r.n_iter : 0, o[3] = rc == 0? r.n_cigar : 0;
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
+	{
+		WfResult r;
+		A.top = 0;
+		const char *ts_i = ts + t_off[i], *qs_i = qs + q_off[i];
+		int64_t cont_cells = 0;
+		int rc = tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane)
+				: tier == 2? wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane)
+							: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane, &cont_cells);
+		if (rc == 0 && r.n_cigar > cap) rc = MGB_E_INTERNAL;
+		if (rc == 0) for (int32_t j = lane; j < r.n_cigar; j += MGB_W) cigar[(int64_t)i * cap + j] = r.cigar[j];
+		if (lane == 0) {
+			int64_t *o = out + 4 * (int64_t)i;
+			o[0] = rc, o[1] = rc == 0? r.s : -1, o[2] = rc == 0? r.n_iter : 0, o[3] = rc == 0? r.n_cigar : 0;
+		}
+		warp_sync();
+		return 0;
 	}
-	warp_sync();
-}
-#ifndef MGB_HOSTSIM
-template<int TIER>
-__global__ void k_test_wfa_tier(TestTierArgs t)
-{
-	extern __shared__ int4 dyn_smem[];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-	const int stride = StageSpec<TIER == 1? S_WFA_SMALL : S_WFA_MID>::smem;
-	for (int j = threadIdx.x; j < n_warps * stride / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
-	__syncthreads();
-	int32_t *smem = (int32_t*)((char*)dyn_smem + (size_t)warp * stride);
-	const int worker = blockIdx.x * n_warps + warp;
-	Arena A;
-	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
-	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_wfa_tier_body(t, i, smem, A, lane);
-}
-#endif
-
-// copies a host array to the device (or, in the simulators, to a fresh host block); released by the caller with dfree()
-template<typename T> static T *dcopy(const T *h, int64_t n)
-{
-	T *d = (T*)dmalloc((size_t)n * sizeof(T));
-	h2d(d, h, (size_t)n * sizeof(T));
-	return d;
-}
-static int64_t test_seq_bytes(int n, const int64_t *off, const int32_t *len)
-{
-	int64_t end = 0;
-	for (int i = 0; i < n; ++i) end = std::max(end, off[i] + len[i]);
-	return end;
-}
+};
 
 static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_off, const int32_t *tl, const char *qs, const int64_t *q_off,
 							  const int32_t *ql, int64_t *out, uint32_t *cigar, int cap)
@@ -1969,45 +2019,23 @@ static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_
 	for (int i = 0; i < n; ++i) // the gaps of real jobs are never empty on either side (galign.c:97-99 emits plain I/D for those)
 		if (tl[i] < 1 || ql[i] < 1 || t_off[i] < 0 || q_off[i] < 0) { set_error("mgb_test_wfa_tier: gap " + std::to_string(i) + " has an empty side"); return MGB_E_UNSUPPORTED; }
 	if (n == 0) return 0;
-	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	const int warps = tier == 1? StageSpec<S_WFA_SMALL>::warps : StageSpec<S_WFA_MID>::warps;
-	const int stride = tier == 1? StageSpec<S_WFA_SMALL>::smem : StageSpec<S_WFA_MID>::smem;
-	const int n_workers = std::min(n, 64 * warps);
-	TestTierArgs t;
-	t.tier = tier, t.n = n, t.cap = cap;
-	t.ts = dcopy(ts, test_seq_bytes(n, t_off, tl)), t.qs = dcopy(qs, test_seq_bytes(n, q_off, ql));
-	t.t_off = dcopy(t_off, n), t.q_off = dcopy(q_off, n), t.tl = dcopy(tl, n), t.ql = dcopy(ql, n);
-	t.out = (int64_t*)dmalloc(sizeof(int64_t) * 4 * (size_t)n);
-	t.cigar = (uint32_t*)dmalloc(sizeof(uint32_t) * ((size_t)n * cap + 1));
+	if (int e = test_no_device()) return e;
+	auto ts_d = upload(ts, test_seq_bytes(n, t_off, tl)), qs_d = upload(qs, test_seq_bytes(n, q_off, ql));
+	auto t_off_d = upload(t_off, n), q_off_d = upload(q_off, n);
+	auto tl_d = upload(tl, n), ql_d = upload(ql, n);
+	DevBuf<int64_t> out_d(4 * (size_t)n);
+	DevBuf<uint32_t> cigar_d((size_t)n * cap + 1);
+	TestTier t;
+	t.tier = tier, t.cap = cap;
+	t.ts = ts_d, t.qs = qs_d, t.t_off = t_off_d, t.q_off = q_off_d, t.tl = tl_d, t.ql = ql_d, t.out = out_d, t.cigar = cigar_d;
 	// a tier-2 gap needs at most 8 KB of CIGAR and 70 KB of traceback rows; one carried on in the arena at most 230 KB of ring and
 	// 4.3 MB of traceback rows (scores below tl + ql + 30, rows of at most tl + ql + 1 bytes)
-	t.arena_bytes = tier == MGB_TEST_TIER2_CONT? (uint64_t)5 << 20 : (uint64_t)256 << 10;
-	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
-#ifdef MGB_HOSTSIM
-	std::vector<uint32_t> sim_smem((size_t)warps * stride / 4, TEST_SMEM_FILL);
-	for (int i = 0; i < n; ++i) {
-		int32_t *smem = (int32_t*)((char*)sim_smem.data() + (size_t)(i % warps) * stride);
-		char *arena = t.arena + (uint64_t)(i % n_workers) * t.arena_bytes;
-#if MGB_W > 1
-		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, arena, t.arena_bytes); test_wfa_tier_body(t, i, smem, A, lane); });
-#else
-		Arena A;
-		arena_init(A, arena, t.arena_bytes);
-		test_wfa_tier_body(t, i, smem, A, 0);
-#endif
-	}
-#else
-	const size_t smem = (size_t)warps * stride;
-	void (*kern)(TestTierArgs) = tier == 1? k_test_wfa_tier<1> : k_test_wfa_tier<2>;
-	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	kern<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
-	CUDA_OK(cudaGetLastError());
-	dsync();
-#endif
-	d2h(out, t.out, sizeof(int64_t) * 4 * (size_t)n);
-	d2h(cigar, t.cigar, sizeof(uint32_t) * (size_t)n * cap);
-	dfree((void*)t.ts), dfree((void*)t.qs), dfree((void*)t.t_off), dfree((void*)t.q_off), dfree((void*)t.tl), dfree((void*)t.ql);
-	dfree(t.out), dfree(t.cigar), dfree(t.arena);
+	const uint64_t arena_bytes = tier == MGB_TEST_TIER2_CONT? (uint64_t)5 << 20 : (uint64_t)256 << 10;
+	const int rc = tier == 1? test_launch<S_WFA_SMALL>(n, std::min(n, 64 * StageSpec<S_WFA_SMALL>::warps), arena_bytes, t)
+							: test_launch<S_WFA_MID>(n, std::min(n, 64 * StageSpec<S_WFA_MID>::warps), arena_bytes, t);
+	if (rc) return rc;
+	d2h(out, out_d, sizeof(int64_t) * 4 * (size_t)n);
+	d2h(cigar, cigar_d, sizeof(uint32_t) * (size_t)n * cap);
 	return 0;
 }
 
@@ -2023,60 +2051,48 @@ extern "C" int mgb_test_wfa_tier(int tier, int n, const char *ts, const int64_t 
 // memory and the arena in global memory, as k_gwfa runs it (gwfa_job_run); mode 1: the sequential gwf_align() on lane 0,
 // as graph chaining runs it (gc_bridge_gwfa).
 // ---------------------------------------------------------------------------------------------------------------
-struct TestGwfaArgs {
+struct TestGwfa {
 	GraphDev g;
-	int mode, n, walk_cap;
+	int mode, walk_cap;
 	const char *q;
 	const int64_t *q_off;
 	const int32_t *ql, *off0, *off1, *max_ed;
 	const uint32_t *v0, *v1;
 	int64_t *out;       // per bridge: rc, s, end_v, end_off, nv, n_iter
 	int32_t *walk;      // per bridge: walk_cap vertices
-	char *arena;
-	uint64_t arena_bytes;
-};
-MG_HD inline void test_gwfa_body(const TestGwfaArgs &t, int i, GwfShared *sh, Arena &A, int lane)
-{
-	GwfOpt opt;
-	opt.traceback = 1, opt.max_chk = 1000, opt.bw_dyn = 1000, opt.max_lag = t.max_ed[i] / 2, opt.s_term = -1;
-	opt.i_term = 500000000LL;
-	A.top = 0, A.peak = 0;
-	const char *q = t.q + t.q_off[i];
-	int rc = 0;
-	GwfResult rs;
-	const GwfResult *r = &rs;
-	if (t.mode == 0) {
-		if (lane == 0) sh->A = A;
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
+	{
+		GwfShared *sh = (GwfShared*)smem;
+		GwfOpt opt;
+		opt.traceback = 1, opt.max_chk = 1000, opt.bw_dyn = 1000, opt.max_lag = max_ed[i] / 2, opt.s_term = -1;
+		opt.i_term = 500000000LL;
+		A.top = 0, A.peak = 0;
+		const char *q_i = q + q_off[i];
+		int rc = 0;
+		GwfResult rs;
+		const GwfResult *r = &rs;
+		if (mode == 0) {
+			if (lane == 0) sh->A = A;
+			warp_sync();
+			rc = gwf_align_w(sh, g, opt, ql[i], q_i, v0[i], off0[i], v1[i], off1[i], max_ed[i], lane); // s_term: max_ed
+			r = &sh->r;
+		} else {
+			if (lane == 0) rc = gwf_align(A, g, opt, ql[i], q_i, v0[i], off0[i], v1[i], off1[i], max_ed[i], &rs);
+			rc = warp_bcast_i32(rc, 0);
+		}
+		if (lane == 0) {
+			int64_t *o = out + 6 * (int64_t)i;
+			const int32_t nv = rc == 0 && r->s >= 0? r->nv : 0;
+			if (nv > walk_cap) rc = MGB_E_INTERNAL;
+			o[0] = rc;
+			o[1] = rc == 0? r->s : -1, o[2] = rc == 0? (int64_t)r->end_v : -1, o[3] = rc == 0? r->end_off : -1;
+			o[4] = rc == 0? nv : 0, o[5] = rc == 0? r->n_iter : 0;
+			if (rc == 0) for (int32_t j = 0; j < nv; ++j) walk[(int64_t)i * walk_cap + j] = r->v[j];
+		}
 		warp_sync();
-		rc = gwf_align_w(sh, t.g, opt, t.ql[i], q, t.v0[i], t.off0[i], t.v1[i], t.off1[i], t.max_ed[i], lane); // s_term: max_ed
-		r = &sh->r;
-	} else {
-		if (lane == 0) rc = gwf_align(A, t.g, opt, t.ql[i], q, t.v0[i], t.off0[i], t.v1[i], t.off1[i], t.max_ed[i], &rs);
-		rc = warp_bcast_i32(rc, 0);
+		return 0;
 	}
-	if (lane == 0) {
-		int64_t *o = t.out + 6 * (int64_t)i;
-		const int32_t nv = rc == 0 && r->s >= 0? r->nv : 0;
-		if (nv > t.walk_cap) rc = MGB_E_INTERNAL;
-		o[0] = rc;
-		o[1] = rc == 0? r->s : -1, o[2] = rc == 0? (int64_t)r->end_v : -1, o[3] = rc == 0? r->end_off : -1;
-		o[4] = rc == 0? nv : 0, o[5] = rc == 0? r->n_iter : 0;
-		if (rc == 0) for (int32_t j = 0; j < nv; ++j) t.walk[(int64_t)i * t.walk_cap + j] = r->v[j];
-	}
-	warp_sync();
-}
-#ifndef MGB_HOSTSIM
-__global__ void k_test_gwfa(TestGwfaArgs t)
-{
-	extern __shared__ int4 dyn_smem[];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-	GwfShared *sh = (GwfShared*)((char*)dyn_smem + (size_t)warp * StageSpec<S_GWFA>::smem);
-	const int worker = blockIdx.x * n_warps + warp;
-	Arena A;
-	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
-	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_gwfa_body(t, i, sh, A, lane);
-}
-#endif
+};
 
 static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, const int64_t *q_off, const int32_t *ql, const uint32_t *v0,
 						  const int32_t *off0, const uint32_t *v1, const int32_t *off1, const int32_t *max_ed, int64_t *out, int32_t *walk, int walk_cap)
@@ -2090,40 +2106,19 @@ static int test_gwfa_impl(const mg_idx_t *gi, int mode, int n, const char *q, co
 			return MGB_E_UNSUPPORTED;
 		}
 	if (n == 0) return 0;
-	if (!dev_ok(M->device)) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	const int warps = StageSpec<S_GWFA>::warps, n_workers = std::min(n, 8 * warps);
-	TestGwfaArgs t;
-	t.g = M->g, t.mode = mode, t.n = n, t.walk_cap = walk_cap;
-	t.q = dcopy(q, test_seq_bytes(n, q_off, ql));
-	t.q_off = dcopy(q_off, n), t.ql = dcopy(ql, n), t.off0 = dcopy(off0, n), t.off1 = dcopy(off1, n), t.max_ed = dcopy(max_ed, n);
-	t.v0 = dcopy(v0, n), t.v1 = dcopy(v1, n);
-	t.out = (int64_t*)dmalloc(sizeof(int64_t) * 6 * (size_t)n);
-	t.walk = (int32_t*)dmalloc(sizeof(int32_t) * ((size_t)n * walk_cap + 1));
-	t.arena_bytes = (uint64_t)64 << 20;
-	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
-#ifdef MGB_HOSTSIM
-	std::vector<u128> sim_smem(StageSpec<S_GWFA>::smem / sizeof(u128));
-	GwfShared *sh = (GwfShared*)sim_smem.data();
-	for (int i = 0; i < n; ++i) {
-#if MGB_W > 1
-		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, t.arena, t.arena_bytes); test_gwfa_body(t, i, sh, A, lane); });
-#else
-		Arena A;
-		arena_init(A, t.arena, t.arena_bytes);
-		test_gwfa_body(t, i, sh, A, 0);
-#endif
-	}
-#else
-	const size_t smem = (size_t)warps * StageSpec<S_GWFA>::smem;
-	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test_gwfa, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	k_test_gwfa<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
-	CUDA_OK(cudaGetLastError());
-	dsync();
-#endif
-	d2h(out, t.out, sizeof(int64_t) * 6 * (size_t)n);
-	d2h(walk, t.walk, sizeof(int32_t) * (size_t)n * walk_cap);
-	dfree((void*)t.q), dfree((void*)t.q_off), dfree((void*)t.ql), dfree((void*)t.off0), dfree((void*)t.off1), dfree((void*)t.max_ed);
-	dfree((void*)t.v0), dfree((void*)t.v1), dfree(t.out), dfree(t.walk), dfree(t.arena);
+	if (int e = test_no_device(M->device)) return e;
+	auto q_d = upload(q, test_seq_bytes(n, q_off, ql));
+	auto q_off_d = upload(q_off, n);
+	auto ql_d = upload(ql, n), off0_d = upload(off0, n), off1_d = upload(off1, n), max_ed_d = upload(max_ed, n);
+	auto v0_d = upload(v0, n), v1_d = upload(v1, n);
+	DevBuf<int64_t> out_d(6 * (size_t)n);
+	DevBuf<int32_t> walk_d((size_t)n * walk_cap + 1);
+	TestGwfa t;
+	t.g = M->g, t.mode = mode, t.walk_cap = walk_cap;
+	t.q = q_d, t.q_off = q_off_d, t.ql = ql_d, t.off0 = off0_d, t.off1 = off1_d, t.max_ed = max_ed_d, t.v0 = v0_d, t.v1 = v1_d, t.out = out_d, t.walk = walk_d;
+	if (int e = test_launch<S_GWFA>(n, std::min(n, 8 * StageSpec<S_GWFA>::warps), (uint64_t)64 << 20, t)) return e;
+	d2h(out, out_d, sizeof(int64_t) * 6 * (size_t)n);
+	d2h(walk, walk_d, sizeof(int32_t) * (size_t)n * walk_cap);
 	return 0;
 }
 
@@ -2138,52 +2133,30 @@ extern "C" int mgb_test_gwfa(const mg_idx_t *gi, int mode, int n, const char *q,
 // `hot_bytes` of shared memory for the range stack and bin tables (0: everything in the arena in global memory), as k_seed sorts
 // its seeds; tests/cases.py holds it against klib's.
 // ---------------------------------------------------------------------------------------------------------------
-struct TestRadixArgs { u128 *a; int64_t n; int walk, hot_bytes; char *cold; uint64_t cold_bytes; int32_t *rc; };
-MG_HD inline int test_radix_body(const TestRadixArgs &t, char *hot, int lane)
-{
-	Arena A, H;
-	arena_init(A, t.cold, t.cold_bytes);
-	arena_init(H, hot, t.hot_bytes > 0? (uint64_t)t.hot_bytes : 0);
-	return radix_sort_128x_w(t.hot_bytes > 0? H : A, t.a, t.n, lane, &A, t.walk != 0);
-}
-#ifndef MGB_HOSTSIM
-__global__ void k_test_radix128(TestRadixArgs t)
-{
-	extern __shared__ int4 dyn_smem[];
-	const int rc = test_radix_body(t, (char*)dyn_smem, threadIdx.x & 31);
-	if (threadIdx.x == 0) *t.rc = rc;
-}
-#endif
+struct TestRadix {
+	u128 *a; int64_t n; int walk, hot_bytes; int32_t *rc;
+	MG_HD int operator()(int, int32_t *hot, Arena &A, int, int lane) const
+	{
+		Arena H;
+		arena_init(H, hot, hot_bytes > 0? (uint64_t)hot_bytes : 0);
+		const int r = radix_sort_128x_w(hot_bytes > 0? H : A, a, n, lane, &A, walk != 0);
+		if (lane == 0) *rc = r;
+		return r;
+	}
+};
 
 static int test_radix128_impl(u128 *a, int64_t n, int walk, int hot_bytes)
 {
 	if (n < 0 || hot_bytes < 0 || hot_bytes > 200 * 1024) { set_error("mgb_test_radix128: n >= 0 and 0 <= hot_bytes <= 200 KB"); return MGB_E_UNSUPPORTED; }
-	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	TestRadixArgs t;
-	t.a = dcopy(a, n), t.n = n, t.walk = walk, t.hot_bytes = hot_bytes;
-	t.cold_bytes = (uint64_t)n * 64 + (1 << 20);
-	t.cold = (char*)dmalloc(t.cold_bytes);
-	t.rc = (int32_t*)dmalloc(sizeof(int32_t));
+	if (int e = test_no_device()) return e;
+	auto a_d = upload(a, n);
+	DevBuf<int32_t> rc_d(1);
+	TestRadix t;
+	t.a = a_d, t.n = n, t.walk = walk, t.hot_bytes = hot_bytes, t.rc = rc_d;
+	if (int e = test_launch<NO_STAGE>(1, 1, (uint64_t)n * 64 + (1 << 20), t, 1, hot_bytes)) return e;
 	int32_t rc = 0;
-#ifdef MGB_HOSTSIM
-	std::vector<u128> hot((size_t)hot_bytes / sizeof(u128) + 1);
-#if MGB_W > 1
-	int rcs[MGB_W];
-	sim::run_warp(MGB_W, [&](int lane) { rcs[lane] = test_radix_body(t, (char*)hot.data(), lane); });
-	rc = rcs[0];
-	for (int l = 1; l < MGB_W; ++l) if (rcs[l] != rc) { set_error("simulated warp: lanes returned different codes from the sort"); rc = MGB_E_INTERNAL; }
-#else
-	rc = test_radix_body(t, (char*)hot.data(), 0);
-#endif
-#else
-	if (hot_bytes > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(k_test_radix128, cudaFuncAttributeMaxDynamicSharedMemorySize, hot_bytes));
-	k_test_radix128<<<1, 32, (size_t)hot_bytes, t_stream>>>(t);
-	CUDA_OK(cudaGetLastError());
-	dsync();
-	d2h(&rc, t.rc, sizeof(rc));
-#endif
-	if (rc == 0) d2h(a, t.a, sizeof(u128) * (size_t)n);
-	dfree(t.a), dfree(t.cold), dfree(t.rc);
+	d2h(&rc, rc_d, sizeof(rc));
+	if (rc == 0) d2h(a, a_d, sizeof(u128) * (size_t)n);
 	return rc;
 }
 
@@ -2195,60 +2168,42 @@ extern "C" int mgb_test_radix128(mg128_t *a, int64_t n, int walk, int hot_bytes)
 
 // ---------------------------------------------------------------------------------------------------------------
 // test hook: the linear chaining of k_chain (mode 0: DP, 1: RMQ) or k_chain_rescue (mode 2: sort into target order, RMQ) on
-// anchor sets with options of their own, launched as those kernels are: their stage's warps per block and slice of shared
-// memory per warp, the anchors staged into the slice when they fit (chain_staged, chain_run: the code of stage_chain).  The
-// slices start out filled with junk and each warp chains several sets in a row, so a warp reuses its slice dirty, flips the
-// parity of its barrier and moves between staged and unstaged sets.  Set i goes to worker i % n_workers.
+// anchor sets with options of their own, launched as those kernels are (test_launch), the anchors staged into the slice when
+// they fit (chain_staged, chain_run: the code of stage_chain).  Each warp chains several sets in a row, so it reuses its slice
+// dirty, flips the parity of its barrier and moves between staged and unstaged sets.  Set i goes to worker i % n_workers.
 // ---------------------------------------------------------------------------------------------------------------
-struct TestLchainArgs {
-	int mode, n;
+struct TestLchain {
+	int mode;
+	uint64_t slice;       // bytes of shared memory per warp
 	u128 *a;              // every set's anchors, chained in place: the compacted anchors are read back from here
 	const int64_t *off;
 	const int32_t *cnt;
 	const LChainOpt *opt;
 	int32_t *out;         // per set: rc, n_u, n_v, staged, path, worker
 	uint64_t *u;          // per set: the chains at u[off[i]..]
-	char *arena;
-	uint64_t arena_bytes;
-};
-MG_HD inline void test_lchain_body(const TestLchainArgs &t, int i, int32_t *smem, uint64_t slice, Arena &A, int worker, int lane)
-{
-	A.top = 0;
-	u128 *a = t.a + t.off[i];
-	const int64_t n = t.cnt[i];
-	const LChainOpt &co = t.opt[i];
-	int32_t n_u = 0, n_v = 0;
-	uint64_t *u = 0;
-	int path = -1, staged = 0;
-	const int rc = chain_staged(smem, slice, A, a, n, lane, &staged, [&](Arena &H, u128 *aw, int32_t *n_keep) {
-		const int r = t.mode == 2? chain_run<1>(H, A, 1, co, n, aw, &n_u, &u, &n_v, lane, &path) : chain_run<0>(H, A, t.mode == 1, co, n, aw, &n_u, &u, &n_v, lane, &path);
-		*n_keep = n_u > 0? n_v : 0;
-		return r;
-	});
-	if (rc == 0) for (int32_t j = lane; j < n_u; j += MGB_W) t.u[t.off[i] + j] = u[j];
-	if (lane == 0) {
-		int32_t *o = t.out + 6 * (int64_t)i;
-		o[0] = rc, o[1] = n_u, o[2] = n_v, o[3] = staged, o[4] = path, o[5] = worker;
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int worker, int lane) const
+	{
+		A.top = 0;
+		u128 *a_i = a + off[i];
+		const int64_t n = cnt[i];
+		const LChainOpt &co = opt[i];
+		int32_t n_u = 0, n_v = 0;
+		uint64_t *u_i = 0;
+		int path = -1, staged = 0;
+		const int rc = chain_staged(smem, slice, A, a_i, n, lane, &staged, [&](Arena &H, u128 *aw, int32_t *n_keep) {
+			const int r = mode == 2? chain_run<1>(H, A, 1, co, n, aw, &n_u, &u_i, &n_v, lane, &path) : chain_run<0>(H, A, mode == 1, co, n, aw, &n_u, &u_i, &n_v, lane, &path);
+			*n_keep = n_u > 0? n_v : 0;
+			return r;
+		});
+		if (rc == 0) for (int32_t j = lane; j < n_u; j += MGB_W) u[off[i] + j] = u_i[j];
+		if (lane == 0) {
+			int32_t *o = out + 6 * (int64_t)i;
+			o[0] = rc, o[1] = n_u, o[2] = n_v, o[3] = staged, o[4] = path, o[5] = worker;
+		}
+		warp_sync();
+		return 0;
 	}
-	warp_sync();
-}
-#ifndef MGB_HOSTSIM
-template<int S>
-__global__ void k_test_lchain(TestLchainArgs t)
-{
-	extern __shared__ int4 dyn_smem[];
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5;
-	const int stride = StageSpec<S>::smem;
-	for (int j = threadIdx.x; j < n_warps * stride / 4; j += blockDim.x) ((uint32_t*)dyn_smem)[j] = TEST_SMEM_FILL;
-	__syncthreads();
-	int32_t *smem = (int32_t*)((char*)dyn_smem + (size_t)warp * stride);
-	chain_smem_init(smem, lane);
-	const int worker = blockIdx.x * n_warps + warp;
-	Arena A;
-	arena_init(A, t.arena + (uint64_t)worker * t.arena_bytes, t.arena_bytes);
-	for (int i = worker; i < t.n; i += gridDim.x * n_warps) test_lchain_body(t, i, smem, (uint64_t)stride, A, worker, lane);
-}
-#endif
+};
 
 static int test_lchain_impl(int mode, int n, const u128 *a, const int64_t *off, const int32_t *cnt, const mgb_lchain_opt_t *opt, int32_t *out, uint64_t *u, u128 *a_out)
 {
@@ -2265,51 +2220,26 @@ static int test_lchain_impl(int mode, int n, const u128 *a, const int64_t *off, 
 		max_cnt = std::max(max_cnt, (int64_t)cnt[i]);
 	}
 	if (n == 0) return 0;
-	if (!dev_ok()) { set_error("no CUDA device available: libmgb200 has no CPU path"); return -100; }
-	const int warps = mode == 2? StageSpec<S_CHAIN_RESCUE>::warps : StageSpec<S_CHAIN>::warps;
-	const int stride = mode == 2? StageSpec<S_CHAIN_RESCUE>::smem : StageSpec<S_CHAIN>::smem;
-	const int n_workers = std::min(n, 2 * warps);
+	if (int e = test_no_device()) return e;
 	const int64_t n_a = test_seq_bytes(n, off, cnt);
-	TestLchainArgs t;
-	t.mode = mode, t.n = n;
-	t.a = (u128*)dmalloc(sizeof(u128) * (size_t)(n_a + 1));
-	if (n_a > 0) h2d(t.a, a, sizeof(u128) * (size_t)n_a);
-	t.off = dcopy(off, n), t.cnt = dcopy(cnt, n), t.opt = dcopy((const LChainOpt*)opt, n);
-	t.out = (int32_t*)dmalloc(sizeof(int32_t) * 6 * (size_t)n);
-	t.u = (uint64_t*)dmalloc(sizeof(uint64_t) * (size_t)(n_a + 1));
+	auto a_d = upload(a, n_a);
+	auto off_d = upload(off, n);
+	auto cnt_d = upload(cnt, n);
+	auto opt_d = upload((const LChainOpt*)opt, n);
+	DevBuf<int32_t> out_d(6 * (size_t)n);
+	DevBuf<uint64_t> u_d((size_t)n_a + 1);
+	TestLchain t;
+	t.mode = mode, t.slice = mode == 2? StageSpec<S_CHAIN_RESCUE>::smem : StageSpec<S_CHAIN>::smem;
+	t.a = a_d, t.off = off_d, t.cnt = cnt_d, t.opt = opt_d, t.out = out_d, t.u = u_d;
 	// per anchor at most ~200 bytes: f/p/v/t, the RMQ window, priorities and block summaries, the end-point list, the compaction's
 	// copy, and the two AVL trees of the sequential fill
-	t.arena_bytes = (uint64_t)max_cnt * 512 + ((uint64_t)1 << 20);
-	t.arena = (char*)dmalloc(t.arena_bytes * (size_t)n_workers);
-#ifdef MGB_HOSTSIM
-	std::vector<uint32_t> sim_smem((size_t)n_workers * stride / 4, TEST_SMEM_FILL);
-	auto slice = [&](int w) { return (int32_t*)((char*)sim_smem.data() + (size_t)w * stride); };
-	auto on_warp = [&](int w, const std::function<void(Arena &, int)> &fn) {
-#if MGB_W > 1
-		sim::run_warp(MGB_W, [&](int lane) { Arena A; arena_init(A, t.arena + (uint64_t)w * t.arena_bytes, t.arena_bytes); fn(A, lane); });
-#else
-		Arena A;
-		arena_init(A, t.arena + (uint64_t)w * t.arena_bytes, t.arena_bytes);
-		fn(A, 0);
-#endif
-	};
-	for (int w = 0; w < n_workers; ++w) on_warp(w, [&](Arena &, int lane) { chain_smem_init(slice(w), lane); });
-	for (int i = 0; i < n; ++i) {
-		const int w = i % n_workers;
-		on_warp(w, [&](Arena &A, int lane) { test_lchain_body(t, i, slice(w), (uint64_t)stride, A, w, lane); });
-	}
-#else
-	const size_t smem = (size_t)warps * stride;
-	void (*kern)(TestLchainArgs) = mode == 2? k_test_lchain<S_CHAIN_RESCUE> : k_test_lchain<S_CHAIN>;
-	if (smem > 48 * 1024) CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	kern<<<(n_workers + warps - 1) / warps, warps * 32, smem, t_stream>>>(t);
-	CUDA_OK(cudaGetLastError());
-	dsync();
-#endif
-	d2h(out, t.out, sizeof(int32_t) * 6 * (size_t)n);
-	d2h(u, t.u, sizeof(uint64_t) * (size_t)n_a);
-	d2h(a_out, t.a, sizeof(u128) * (size_t)n_a);
-	dfree(t.a), dfree((void*)t.off), dfree((void*)t.cnt), dfree((void*)t.opt), dfree(t.out), dfree(t.u), dfree(t.arena);
+	const uint64_t arena_bytes = (uint64_t)max_cnt * 512 + ((uint64_t)1 << 20);
+	const int rc = mode == 2? test_launch<S_CHAIN_RESCUE>(n, std::min(n, 2 * StageSpec<S_CHAIN_RESCUE>::warps), arena_bytes, t)
+							: test_launch<S_CHAIN>(n, std::min(n, 2 * StageSpec<S_CHAIN>::warps), arena_bytes, t);
+	if (rc) return rc;
+	d2h(out, out_d, sizeof(int32_t) * 6 * (size_t)n);
+	d2h(u, u_d, sizeof(uint64_t) * (size_t)n_a);
+	d2h(a_out, a_d, sizeof(u128) * (size_t)n_a);
 	return 0;
 }
 
