@@ -212,6 +212,18 @@ int mg_map_batch_frag(const mg_idx_t *gi, int n_frag, const int *n_seg, const in
 /* mg_gchain_free() over a whole batch (what step 2 of the reference pipeline does read by read, gmap.c:130); entries are set to NULL */
 void mgb_free_batch(int n_reads, mg_gchains_t **gcs);
 
+/* Map a batch and return its GAF text, formatted on the device: byte for byte what mg_map_batch_frag() followed by the
+ * reference's mg_write_gaf() (format.c:121-291) on every fragment in input order gives, with opt->flag as the writer's flag.
+ * n_seg == NULL: one segment per read (n_frag reads).  names[f] may be NULL ("*", as mgb_write_gaf_batch).  The text is
+ * 0-terminated; (out, out_len, out_cap) follow mgb_write_gaf_batch(): out_cap == NULL gives a fresh malloc() block, otherwise a
+ * caller-owned buffer that is reused and grown.  Returns 0, or a negative code with the reason in mgb_last_error() and
+ * *out_len = 0 (no partial text).  MG_M_CAL_COV and MG_M_INDEPEND_SEG are refused: the reference prints no per-fragment GAF
+ * record under them.  Slots, host threads and MGB_DEVICES work as for mg_map_batch(); no mg_gchains_t is built.  In the
+ * stats of such a call, out_bytes is the number of text bytes copied back, t_d2h_ms covers the GAF kernels plus that copy,
+ * and t_asm_ms is the host time after the copy (the text copied on into the caller's buffer). */
+int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, const int *qlens, const char *const *seqs,
+					  const char *const *names, const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Engine controls and instrumentation (not part of the reference API)
  * ---------------------------------------------------------------------------------------------------------- */

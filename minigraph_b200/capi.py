@@ -133,6 +133,11 @@ def bind_mapping_api(lib):
     lib.mg_gchain_free.argtypes = [C.POINTER(mg_gchains_t)]
     lib.mg_idx_get.restype = C.POINTER(C.c_uint64)
     lib.mg_idx_get.argtypes = [C.POINTER(mg_idx_t), C.c_uint64, C.POINTER(C.c_int)]
+    if hasattr(lib, "mgb_map_batch_gaf"):  # the engine's; the reference has no such symbol
+        lib.mgb_map_batch_gaf.restype = C.c_int
+        lib.mgb_map_batch_gaf.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_char_p),
+                                          C.POINTER(C.c_char_p), C.POINTER(mg_mapopt_t), C.POINTER(C.c_void_p), C.POINTER(C.c_size_t),
+                                          C.POINTER(C.c_size_t)]
     return lib
 
 

@@ -22,6 +22,7 @@
 
 #include "../../include/mgb200.h"
 #include "mgb_galign.cuh"
+#include "mgb_gaf.cuh"
 
 #ifndef MGB_HOSTSIM
 #include <cuda_runtime.h>
@@ -476,9 +477,8 @@ static void pack_results(const PackArgs &P)
 // when the read holds any other byte (N, lower case, IUPAC): such a read travels as ASCII, because the alignment compares raw bytes.
 static bool pack_read_scalar(const char *s, int len, uint64_t *out)
 {
-	static uint8_t tab[256];
-	static bool init = false;
-	if (!init) { for (int i = 0; i < 256; ++i) tab[i] = 4; tab['A'] = 0, tab['C'] = 1, tab['G'] = 2, tab['T'] = 3; init = true; }
+	static const struct Tab { uint8_t c[256]; Tab() { for (int i = 0; i < 256; ++i) c[i] = 4; c['A'] = 0, c['C'] = 1, c['G'] = 2, c['T'] = 3; } } T; // filled once: several host threads pack at once
+	const uint8_t *tab = T.c;
 	unsigned bad = 0;
 	for (int w = 0; w * 32 < len; ++w) {
 		uint64_t x = 0;
@@ -668,6 +668,50 @@ static void launch_stage(LaunchArgs &L, const Workers &W)
 #endif
 }
 
+// ---- GAF text on the device (mgb_gaf.cuh) ----
+// One warp per read in every pass; the count and the write pass pull reads from a counter, the scan between them puts the reads'
+// texts in read order (as k_out_scan does for the blobs).
+#ifndef MGB_HOSTSIM
+__global__ void __launch_bounds__(256) k_gaf_req(GafArgs G)
+{
+	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
+	for (int r = warp; r < G.n; r += n_warp) gaf_requests(G, r, lane);
+}
+__device__ inline int gaf_next_read(unsigned int *next, int lane)
+{
+	unsigned int r = 0;
+	if (lane == 0) r = atomicAdd(next, 1u);
+	return (int)__shfl_sync(0xffffffffu, r, 0);
+}
+__global__ void __launch_bounds__(256) k_gaf_count(GafArgs G)
+{
+	const int lane = threadIdx.x & 31;
+	for (int r = gaf_next_read(G.next, lane); r < G.n; r = gaf_next_read(G.next, lane)) {
+		const uint64_t n = gaf_read(G, r, 0, lane);
+		if (lane == 0) G.off[r] = n;
+	}
+}
+__global__ void __launch_bounds__(1024) k_gaf_scan(GafArgs G)
+{
+	__shared__ uint64_t part[1024];
+	const int tid = threadIdx.x, per = (G.n + 1023) / 1024;
+	const int r0 = tid * per < G.n? tid * per : G.n, r1 = r0 + per < G.n? r0 + per : G.n;
+	uint64_t sum = 0;
+	for (int r = r0; r < r1; ++r) sum += G.off[r];
+	part[tid] = sum;
+	__syncthreads();
+	if (tid == 0) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[i]; part[i] = acc; acc += c; } G.off[G.n] = acc; }
+	__syncthreads();
+	uint64_t acc = part[tid];
+	for (int r = r0; r < r1; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
+}
+__global__ void __launch_bounds__(256) k_gaf_write(GafArgs G)
+{
+	const int lane = threadIdx.x & 31;
+	for (int r = gaf_next_read(G.next + 1, lane); r < G.n; r = gaf_next_read(G.next + 1, lane)) gaf_read(G, r, G.text + G.off[r], lane);
+}
+#endif
+
 // ---------------------------------------------------------------------------------------------------------------
 // model: flattened graph + minimizer index, host copy and device image
 // ---------------------------------------------------------------------------------------------------------------
@@ -689,6 +733,7 @@ struct Model {
 	// device image
 	GraphDev g;
 	IndexDev ix;
+	GafGraph gafg; // names of the graph for the GAF kernels
 	std::vector<void*> dev_ptrs;
 	// per-model scratch reused across batches
 	std::vector<int32_t> seg_name_id, seg_soff; // MG_M_NO_DIAG: the name a segment goes by (id into name_ids) and its offset there
@@ -702,6 +747,7 @@ struct Model {
 	// so that kernels, copies and host-side result assembly of different sub-batches overlap
 	struct Slot {
 		GrowBuf h_seq{true}, h_out{true}, h_small{true}, h_pk{true}, h_mail{true}, h_routs{true}, d_pk, d_seq, d_meta, d_routs, d_small, d_jobq, d_order, d_packed, d_packoff, d_segs, d_lab_new, d_pool[10];
+		GrowBuf h_gaf{true}, d_gaf, d_gaf_text; // mgb_map_batch_gaf(): the reads' names and segments, requests and cells; the text
 		mgb::HostPool host_pool; // packing and result assembly of the batch on this slot
 		Workers W;
 		mgb_stats_t st;
@@ -748,6 +794,7 @@ static void model_free(Model *M)
 	for (int k = 0; k < Model::MAX_SLOTS; ++k) {
 		Model::Slot &sl = M->slots[k];
 		sl.h_seq.release(), sl.h_out.release(), sl.h_small.release(), sl.h_pk.release(), sl.h_mail.release(), sl.h_routs.release(), sl.d_pk.release(), sl.d_seq.release(), sl.d_meta.release(), sl.d_routs.release(), sl.d_small.release(), sl.d_jobq.release(), sl.d_order.release(), sl.d_packed.release(), sl.d_packoff.release(), sl.d_segs.release(), sl.d_lab_new.release();
+		sl.h_gaf.release(), sl.d_gaf.release(), sl.d_gaf_text.release();
 		for (int i = 0; i < 10; ++i) sl.d_pool[i].release();
 		if (sl.timers) timers_free(sl.timers);
 		if (sl.W.arena) dfree(sl.W.arena);
@@ -759,15 +806,24 @@ static void model_free(Model *M)
 	delete M;
 }
 
-static unsigned char comp_tab[256];
-static void init_comp_tab() // reference: gfa-base.c:509-526 gfa_comp_table
+// reference: gfa-base.c:509-526 gfa_comp_table.  Filled once: with MGB_DEVICES, mg_index() builds the models of the further devices
+// on several threads at once, and a table filled anew by each of them was read half-filled by another (reverse strands of segments
+// left uncomplemented on one device).
+static const unsigned char *comp_tab()
 {
-	static const char *from = "ABCDEFGHIJKLMNOPQRSTUVWXYZ", *to = "TVGHEFCDIJMLKNOPQYSAABWXRZ";
-	for (int i = 0; i < 256; ++i) comp_tab[i] = (unsigned char)i;
-	for (int i = 0; i < 26; ++i) {
-		comp_tab[(unsigned char)from[i]] = (unsigned char)to[i];
-		comp_tab[(unsigned char)(from[i] + 32)] = (unsigned char)(to[i] + 32);
-	}
+	static const struct Tab {
+		unsigned char c[256];
+		Tab()
+		{
+			const char *from = "ABCDEFGHIJKLMNOPQRSTUVWXYZ", *to = "TVGHEFCDIJMLKNOPQYSAABWXRZ";
+			for (int i = 0; i < 256; ++i) c[i] = (unsigned char)i;
+			for (int i = 0; i < 26; ++i) {
+				c[(unsigned char)from[i]] = (unsigned char)to[i];
+				c[(unsigned char)(from[i] + 32)] = (unsigned char)(to[i] + 32);
+			}
+		}
+	} tab;
+	return tab.c;
 }
 
 static void ensure_workers(Workers &W, int n_workers, uint64_t arena_bytes)
@@ -796,7 +852,7 @@ static Model *model_build(gfa_t *g, int k, int w)
 	M->k = k, M->w = w, M->d_logf = 0, M->n_logf = 0, M->es = 0;
 	memset(&M->W, 0, sizeof(Workers)), memset(&M->Wbig, 0, sizeof(Workers));
 	memset(&M->stats, 0, sizeof(M->stats));
-	init_comp_tab();
+	const unsigned char *comp = comp_tab();
 	const uint32_t n_seg = g->n_seg, n_vtx = n_seg * 2;
 	M->seg_len.resize(n_seg);
 	M->vseq_off.resize(n_vtx);
@@ -811,7 +867,7 @@ static Model *model_build(gfa_t *g, int k, int w)
 		const gfa_seg_t *s = &g->seg[i];
 		char *f = &M->seq[M->vseq_off[i << 1]], *r = &M->seq[M->vseq_off[i << 1 | 1]];
 		for (int32_t j = 0; j < s->len; ++j) f[j] = s->seq[j];
-		for (int32_t j = 0; j < s->len; ++j) r[s->len - j - 1] = (char)comp_tab[(uint8_t)s->seq[j]]; // reference: gfa-ed.c:33-36
+		for (int32_t j = 0; j < s->len; ++j) r[s->len - j - 1] = (char)comp[(uint8_t)s->seq[j]]; // reference: gfa-ed.c:33-36
 	}
 	M->arc_idx.assign(g->idx, g->idx + n_vtx);
 	M->arc.resize(g->n_arc);
@@ -838,6 +894,24 @@ static Model *model_build(gfa_t *g, int k, int w)
 	M->g.arc_idx = upload(M->arc_idx.data(), M->arc_idx.size()).release(), M->dev_ptrs.push_back((void*)M->g.arc_idx);
 	M->g.arc = upload(M->arc.data(), M->arc.size()).release(), M->dev_ptrs.push_back((void*)M->g.arc);
 	M->ix.k = k, M->ix.w = w, M->ix.slot = 0, M->ix.pos = 0, M->ix.n_slots_mask = 0;
+	{ // names of segments and stable sequences for the GAF kernels: concatenated bytes + offsets
+		auto names = [&](uint32_t n, const std::function<const char*(uint32_t)> &nm, const char **d_name, const int64_t **d_off) {
+			std::vector<int64_t> off((size_t)n + 1, 0);
+			std::string b;
+			for (uint32_t i = 0; i < n; ++i) { const char *s = nm(i); if (s) b += s; off[(size_t)i + 1] = (int64_t)b.size(); }
+			*d_name = upload(b.data(), b.size()).release(), M->dev_ptrs.push_back((void*)*d_name);
+			*d_off = upload(off.data(), off.size()).release(), M->dev_ptrs.push_back((void*)*d_off);
+		};
+		const uint32_t n_sseq = g->sseq? g->n_sseq : 0;
+		names(n_seg, [&](uint32_t i) { return (const char*)g->seg[i].name; }, &M->gafg.seg_name, &M->gafg.seg_name_off);
+		names(n_sseq, [&](uint32_t i) { return (const char*)g->sseq[i].name; }, &M->gafg.sseq_name, &M->gafg.sseq_name_off);
+		std::vector<int32_t> snid(n_seg), soff(n_seg), smin(n_sseq + 1), smax(n_sseq + 1), srank(n_sseq + 1);
+		for (uint32_t i = 0; i < n_seg; ++i) snid[i] = g->seg[i].snid, soff[i] = g->seg[i].soff;
+		for (uint32_t i = 0; i < n_sseq; ++i) smin[i] = g->sseq[i].min, smax[i] = g->sseq[i].max, srank[i] = g->sseq[i].rank;
+		auto put = [&](const std::vector<int32_t> &v, const int32_t **d) { *d = upload(v.data(), v.size()).release(), M->dev_ptrs.push_back((void*)*d); };
+		put(snid, &M->gafg.snid), put(soff, &M->gafg.soff), put(smin, &M->gafg.sseq_min), put(smax, &M->gafg.sseq_max), put(srank, &M->gafg.sseq_rank);
+		M->gafg.seg_len = M->g.seg_len;
+	}
 
 	// sketch every segment on the device (K1 reused), then build the table: on the device (the simulators: on the host)
 #ifdef MGB_HOSTSIM
@@ -1134,6 +1208,12 @@ static void fill_opt(MapOptDev &o, const mg_mapopt_t *opt, int k)
 	o.mask_level = opt->mask_level, o.sub_diff = opt->sub_diff, o.best_n = opt->best_n, o.pri_ratio = opt->pri_ratio, o.ref_bonus = opt->ref_bonus;
 }
 
+// dv:f of a graph chain (reference: gchain1.c:295; host libm log, SURVEY H3): mg_gchain_t::div here and in the GAF cells
+static float gc_div(int32_t n_mini, int32_t n_anchor, int32_t q_span)
+{
+	return n_mini >= n_anchor? (float)(log((double)n_mini / n_anchor) / q_span) : (float)(log((double)n_anchor / n_mini) / q_span);
+}
+
 static mg_gchains_t *build_result(const ReadOut &ro, const char *pool)
 {
 	const char *blob = pool + ro.blob_off;
@@ -1155,8 +1235,7 @@ static mg_gchains_t *build_result(const ReadOut &ro, const char *pool)
 		p->id = s->id, p->parent = s->parent, p->off = s->off, p->cnt = s->cnt, p->n_anchor = s->n_anchor, p->score = s->score;
 		p->qs = s->qs, p->qe = s->qe, p->plen = s->plen, p->ps = s->ps, p->pe = s->pe, p->blen = s->blen, p->mlen = s->mlen;
 		p->hash = s->hash, p->subsc = s->subsc, p->n_sub = s->n_sub, p->mapq = (uint32_t)s->mapq, p->flt = (uint32_t)s->flt;
-		// reference: gchain1.c:295 (host libm log, SURVEY H3)
-		p->div = s->n_mini >= s->n_anchor? (float)(log((double)s->n_mini / s->n_anchor) / s->q_span) : (float)(log((double)s->n_anchor / s->n_mini) / s->q_span);
+		p->div = gc_div(s->n_mini, s->n_anchor, s->q_span);
 		if (s->has_cigar) {
 			p->p = (mg_cigar_t*)calloc(1, (size_t)s->n_cigar * 8 + sizeof(mg_cigar_t));
 			p->p->n_cigar = s->n_cigar, p->p->mlen = s->c_mlen, p->p->blen = s->c_blen, p->p->aplen = s->c_aplen, p->p->ss = s->c_ss, p->p->ee = s->c_ee;
@@ -1220,9 +1299,155 @@ static void lab_after_batch(Model *M, unsigned int n_new)
 	h2d(M->d_lab_hdr, &hp, sizeof(Pool));
 }
 
-// Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).
+// mgb_map_batch_gaf(): the writer's flag, the segments of every read of the part, and where its text goes
+struct GafJob {
+	uint64_t flag;
+	const int *n_seg;          // segments per read, NULL: one (of length qlens[i] of the part)
+	const int64_t *seg_first;  // with n_seg: the first of a read's segment lengths in qlens
+	const int *qlens;
+	std::function<char*(size_t)> dest; // called once with the text's length; room for it and a closing 0, or NULL
+	size_t len;
+};
+
+// The GAF text of a mapped sub-batch, formatted on the device from the blobs in the output pool (mgb_gaf.cuh): requests for the dv:f
+// values, cells formatted by the host, count, scan, write; then the text goes to the host in pieces, each copied on to the caller's
+// buffer by the host threads while the next is on the wire.  Returns 0 or a negative code.
+static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int *qlens, const char *const *names, const ReadOut *routs,
+					const ReadOut *d_routs, const char *d_pool, int host_threads, mgb_stats_t &S, EvTimer &tm_d2h)
+{
+	auto pfor = [&](int64_t n, const std::function<void(int64_t)> &fn) {
+		if (n < 256 || host_threads <= 1) { for (int64_t i = 0; i < n; ++i) fn(i); return; }
+		sl.host_pool.run(n, host_threads, fn);
+	};
+	const size_t n = (size_t)n_reads;
+	const bool lchain = (J.flag & F_WRITE_LCHAIN) != 0;
+	size_t n_segs = 0, name_bytes = 0, n_req = 0;
+	for (size_t i = 0; i < n; ++i) {
+		n_segs += J.n_seg? (size_t)std::max(J.n_seg[i], 0) : 1;
+		name_bytes += names && names[i]? strlen(names[i]) : 1;
+		if (routs[i].n_gc > 0) n_req += (size_t)routs[i].n_gc + (lchain? (size_t)routs[i].n_lc : 0);
+	}
+	auto al = [](size_t x) { return (x + 15) & ~(size_t)15; };
+	// one block on both sides: name_off | req_off | n_seg | seg_first | seg_len | names (uploaded), then requests | cells | off | counters
+	const size_t o_req_off = al(8 * (n + 1)), o_nseg = o_req_off + al(8 * (n + 1)), o_first = o_nseg + al(4 * n), o_len = o_first + al(4 * n);
+	const size_t o_names = o_len + al(4 * n_segs), o_req = o_names + al(name_bytes), o_cells = o_req + al(sizeof(GafReq) * n_req);
+	const size_t o_off = o_cells + al((size_t)GAF_CELL * n_req), o_next = o_off + al(8 * (n + 1)), tot = o_next + 16;
+	char *h = (char*)sl.h_gaf.ensure(tot), *d = (char*)sl.d_gaf.ensure(tot);
+	{
+		int64_t *name_off = (int64_t*)h, *req_off = (int64_t*)(h + o_req_off);
+		int32_t *nseg = (int32_t*)(h + o_nseg), *first = (int32_t*)(h + o_first), *slen = (int32_t*)(h + o_len);
+		char *nm = h + o_names;
+		int64_t at = 0, rq = 0, sg = 0;
+		for (size_t i = 0; i < n; ++i) {
+			const char *s = names && names[i]? names[i] : "*";
+			const size_t l = strlen(s);
+			memcpy(nm + at, s, l);
+			name_off[i] = at, at += (int64_t)l;
+			req_off[i] = rq;
+			if (routs[i].n_gc > 0) rq += routs[i].n_gc + (lchain? routs[i].n_lc : 0);
+			const int ns = J.n_seg? std::max(J.n_seg[i], 0) : 1;
+			const int *ql = J.n_seg? J.qlens + J.seg_first[i] : qlens + i;
+			nseg[i] = ns, first[i] = (int32_t)sg;
+			for (int j = 0; j < ns; ++j) slen[sg++] = ql[j];
+		}
+		name_off[n] = at, req_off[n] = rq;
+	}
+	h2d(d, h, o_req);
+	GafArgs G;
+	G.g = M->gafg;
+	G.q.name = d + o_names, G.q.name_off = (const int64_t*)d, G.q.n_seg = (const int32_t*)(d + o_nseg), G.q.seg_first = (const int32_t*)(d + o_first);
+	G.q.seg_len = (const int32_t*)(d + o_len);
+	G.routs = d_routs, G.pool = d_pool, G.n = n_reads, G.flag = J.flag;
+	G.req_off = (const int64_t*)(d + o_req_off), G.req = (GafReq*)(d + o_req), G.cells = d + o_cells;
+	G.off = (uint64_t*)(d + o_off), G.text = 0, G.next = (unsigned int*)(d + o_next);
+#ifdef MGB_HOSTSIM
+	bool differ = false;
+	auto each_read = [&](const std::function<int(int, int)> &fn) { for (int r = 0; r < n_reads; ++r) sim_warp(-1, r, [&](int lane) { return fn(r, lane); }, &differ); };
+#endif
+	tm_d2h.start();
+	// dv:f values: the device lists what each needs, the host formats them with its libm (SURVEY H3)
+#ifdef MGB_HOSTSIM
+	each_read([&](int r, int lane) { gaf_requests(G, r, lane); return 0; });
+#else
+	if (n_req) { k_gaf_req<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G); CUDA_OK(cudaGetLastError()); }
+#endif
+	d2h(h + o_req, d + o_req, sizeof(GafReq) * n_req);
+	const GafReq *hreq = (const GafReq*)(h + o_req);
+	char *hcells = h + o_cells;
+	pfor((int64_t)n_req, [&](int64_t k) {
+		const GafReq &q = hreq[k];
+		char *c = hcells + (size_t)GAF_CELL * (size_t)k;
+		c[0] = 0;
+		if (q.kind == 0) { // format.c:204-209
+			const float div = gc_div(q.a, q.b, q.q_span);
+			if (div >= 0.0f && div <= 1.0f) { if (div == 0.0f) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div); }
+		} else if (q.kind == 1) { // format.c:256-263
+			const double div = q.a == q.b? 0.0 : (q.a > q.b? log((double)q.a / q.b) : log((double)q.b / q.a)) / q.q_span;
+			if (div == 0.0) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div);
+		}
+	});
+	h2d(d + o_cells, hcells, (size_t)GAF_CELL * n_req);
+	// text: sizes, offsets in read order, bytes
+	dzero(G.next, 2 * sizeof(unsigned int));
+#ifdef MGB_HOSTSIM
+	each_read([&](int r, int lane) { const uint64_t b = gaf_read(G, r, 0, lane); if (lane == 0) G.off[r] = b; return (int)b; });
+	uint64_t acc = 0;
+	for (size_t r = 0; r < n; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
+	G.off[n] = acc;
+#else
+	k_gaf_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	k_gaf_scan<<<1, 1024, 0, t_stream>>>(G);
+	CUDA_OK(cudaGetLastError());
+#endif
+	uint64_t *hoff = (uint64_t*)(h + o_off);
+	d2h(hoff, G.off, 8 * (n + 1));
+	const uint64_t total = hoff[n];
+	G.text = (char*)sl.d_gaf_text.ensure(total + 64);
+	char *htext = (char*)sl.h_out.ensure(total + 64);
+#ifdef MGB_HOSTSIM
+	each_read([&](int r, int lane) { return (int)gaf_read(G, r, G.text + G.off[r], lane); });
+	if (differ) { set_error("simulated warp: lanes returned different codes from the GAF formatter"); return MGB_E_INTERNAL; }
+#else
+	k_gaf_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	CUDA_OK(cudaGetLastError());
+#endif
+	S.n_launches += 4;
+	const int n_piece = n_reads >= 2048? 4 : 1;
+	for (int pc = 0; pc < n_piece; ++pc) {
+		const uint64_t b0 = hoff[n * pc / n_piece], b1 = hoff[n * (pc + 1) / n_piece];
+#ifndef MGB_HOSTSIM
+		if (b1 > b0) CUDA_OK(cudaMemcpyAsync(htext + b0, G.text + b0, b1 - b0, cudaMemcpyDeviceToHost, t_stream));
+		CUDA_OK(cudaEventRecord(sl.ev_piece[pc], t_stream));
+#else
+		if (b1 > b0) memcpy(htext + b0, G.text + b0, b1 - b0);
+#endif
+	}
+	tm_d2h.stop();
+	const double t_asm0 = now_ms();
+	char *dst = J.dest((size_t)total);
+	if (dst == 0) { dsync(); set_error("mgb_map_batch_gaf: out of host memory for the text"); return MGB_E_INTERNAL; }
+	const uint64_t chunk = 1 << 20;
+	for (int pc = 0; pc < n_piece; ++pc) {
+		const uint64_t b0 = hoff[n * pc / n_piece], b1 = hoff[n * (pc + 1) / n_piece];
+#ifndef MGB_HOSTSIM
+		CUDA_OK(cudaEventSynchronize(sl.ev_piece[pc]));
+#endif
+		pfor((int64_t)((b1 - b0 + chunk - 1) / chunk), [&](int64_t k) {
+			const uint64_t c0 = b0 + (uint64_t)k * chunk, c1 = std::min(b1, c0 + chunk);
+			memcpy(dst + c0, htext + c0, c1 - c0);
+		});
+	}
+	dst[total] = 0;
+	J.len = (size_t)total;
+	S.out_bytes = (int64_t)total;
+	S.t_asm_ms = now_ms() - t_asm0;
+	return 0;
+}
+
+// Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).  With gaf, the result is the batch's GAF text
+// (gaf_text) instead of mg_gchains_t objects.
 static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
-					 mg_gchains_t **gcs, int host_threads, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0)
+					 mg_gchains_t **gcs, int host_threads, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0, GafJob *gaf = 0)
 {
 	mgb_stats_t &S = sl.st;
 	memset(&S, 0, sizeof(S));
@@ -1395,6 +1620,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	char *hout = 0;
 	int rc_final = 0, n_piece = 1;
 	std::vector<uint64_t> pack_off;
+	const char *d_out_pool = 0; // the output pool of the last attempt: the GAF path formats from it
 	bool first_kernel = true;
 	(void)first_kernel;
 
@@ -1581,7 +1807,8 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		memcpy(hp, mail->pools, sizeof(hp));
 		if (use_lab) { unsigned int nn[2] = {mail->lab_n[0], mail->lab_n[1]}; S.n_lab_new = (int64_t)nn[0], S.n_lab_big = (int64_t)nn[1]; lab_after_batch(M, nn[0]); }
 		bool done = !pool_full;
-		if (done) { // blobs into read order, then to the host in pieces (the assembly below follows piece by piece)
+		d_out_pool = (const char*)d_buf[P_OUT];
+		if (done && !gaf) { // blobs into read order, then to the host in pieces (the assembly below follows piece by piece)
 			tm_d2h.start();
 			const size_t pool_bytes = (size_t)std::min<uint64_t>(hp[P_OUT].used, cap[P_OUT]);
 			PackArgs P;
@@ -1647,6 +1874,12 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		set_error(buf);
 		return st;
 	}
+	if (gaf) {
+		const int rc = gaf_text(M, sl, *gaf, n_reads, qlens, names, routs, d_routs, d_out_pool, host_threads, S, tm_d2h);
+		S.t_d2h_ms = tm_d2h.ms(); // the GAF kernels + the pieces of the copy
+		S.t_host_ms = now_ms() - t_host0;
+		return rc;
+	}
 	for (int pc = 0; pc < n_piece; ++pc) {
 		const int64_t r0 = (int64_t)n_reads * pc / n_piece, r1 = (int64_t)n_reads * (pc + 1) / n_piece;
 #ifndef MGB_HOSTSIM
@@ -1687,7 +1920,8 @@ static thread_local bool t_has_stats = false;
 // (callers beyond that wait), so a host that maps mini-batch i+1 on a second thread overlaps its packing, copies and result
 // assembly with the kernels of mini-batch i -- what the reference's kt_pipeline does with its step threads (gmap.c:176).
 static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
-						mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0)
+						mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
+						GafJob *gaf = 0)
 {
 	for (int i = 0; i < n_reads; ++i) gcs[i] = 0;
 	if (n_reads <= 0) return 0;
@@ -1729,7 +1963,7 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		}
 		int nt = (int)p_host_threads;
 		if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
-		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len);
+		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf);
 #ifndef MGB_HOSTSIM
 		t_stream = 0; // the slot's stream dies with the model; later calls on this thread (mg_index of another graph) use the default one
 #endif
@@ -1764,11 +1998,12 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 
 // The batch on every device of the index: contiguous parts of about equal bases, one host thread per device, results in input order.
 static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
-						  mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0)
+						  mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
+						  GafJob *gaf = 0)
 {
 	Model *M = (Model*)gi->B;
 	const int n_dev = 1 + (int)M->peers.size();
-	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len);
+	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len, gaf);
 	for (Model *P : M->peers) if (P == 0) { set_error("the index is missing on one of the MGB_DEVICES"); return MGB_E_INTERNAL; }
 	int64_t tot = 0;
 	for (int i = 0; i < n_reads; ++i) tot += qlens[i] > 0? qlens[i] : 0;
@@ -1782,15 +2017,34 @@ static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, con
 		}
 	}
 	std::vector<int> rcs((size_t)n_dev, 0);
+	std::vector<GafJob> parts(gaf? (size_t)n_dev : 0); // the GAF text of each part, joined in input order below
+	std::vector<std::vector<char>> texts(parts.size());
+	for (size_t d = 0; d < parts.size(); ++d) {
+		parts[d] = *gaf, parts[d].len = 0;
+		parts[d].dest = [&texts, d](size_t n) { texts[d].resize(n + 1); return texts[d].data(); };
+	}
 	std::vector<std::thread> th;
 	for (int d = 0; d < n_dev; ++d)
 		th.emplace_back([&, d]() {
 			const int b = bound[(size_t)d], e = bound[(size_t)d + 1];
-			if (e > b) rcs[(size_t)d] = map_batch_on(d == 0? M : M->peers[(size_t)d - 1], e - b, qlens + b, seqs + b, names? names + b : 0, gcs + b, opt);
+			if (e > b) rcs[(size_t)d] = map_batch_on(d == 0? M : M->peers[(size_t)d - 1], e - b, qlens + b, seqs + b, names? names + b : 0, gcs + b, opt,
+													  0, 0, gaf? &parts[(size_t)d] : 0);
 		});
 	for (auto &t : th) t.join();
 	int rc = 0;
 	for (int d = 0; d < n_dev; ++d) if (rcs[(size_t)d] < 0 && rc == 0) rc = rcs[(size_t)d];
+	if (rc == 0 && gaf) {
+		size_t tot = 0;
+		for (const GafJob &p : parts) tot += p.len;
+		char *o = gaf->dest(tot);
+		if (o == 0) { set_error("mgb_map_batch_gaf: out of host memory for the text"); rc = MGB_E_INTERNAL; }
+		else {
+			size_t at = 0;
+			for (size_t d = 0; d < parts.size(); ++d) { if (parts[d].len) memcpy(o + at, texts[d].data(), parts[d].len); at += parts[d].len; }
+			o[tot] = 0;
+			gaf->len = tot;
+		}
+	}
 	if (rc < 0) for (int i = 0; i < n_reads; ++i) if (gcs[i]) { mg_gchain_free(gcs[i]); gcs[i] = 0; } // no partial results are left behind
 #ifndef MGB_HOSTSIM
 	cudaSetDevice(M->device);
@@ -1804,6 +2058,34 @@ extern "C" int mg_map_batch(const mg_idx_t *gi, int n_reads, const int *qlens, c
 	return map_batch_impl(gi, n_reads, qlens, seqs, names, gcs, opt);
 }
 
+// Fragments of several segments as the kernels take them: each fragment's segments concatenated (qsum/sq), their lengths in seg_len
+// from seg_off[f], and first[f] = n_seg[0] + ... + n_seg[f-1], the fragment's first entry in the caller's arrays.
+struct FragBatch {
+	std::vector<std::string> cat;
+	std::vector<int> qsum;
+	std::vector<const char*> sq;
+	std::vector<int32_t> seg_off, seg_len;
+	std::vector<int64_t> first;
+	FragBatch(int n_frag, const int *n_seg, const int *qlens, const char *const *seqs)
+		: cat((size_t)n_frag), qsum((size_t)n_frag), sq((size_t)n_frag), seg_off((size_t)n_frag + 1), first((size_t)n_frag)
+	{
+		int64_t off = 0;
+		for (int f = 0; f < n_frag; ++f) {
+			seg_off[(size_t)f] = (int32_t)seg_len.size();
+			first[(size_t)f] = off;
+			const int ns = n_seg[f] > 0 && n_seg[f] <= 255? n_seg[f] : 0; // more than MG_MAX_SEG segments: no result (map-algo.c:359)
+			for (int j = 0; j < ns; ++j) {
+				const int l = qlens[off + j] > 0? qlens[off + j] : 0;
+				seg_len.push_back(l);
+				if (l > 0) cat[(size_t)f].append(seqs[off + j], (size_t)l);
+			}
+			qsum[(size_t)f] = (int)cat[(size_t)f].size(), sq[(size_t)f] = cat[(size_t)f].data();
+			off += n_seg[f] > 0? n_seg[f] : 0;
+		}
+		seg_off[(size_t)n_frag] = (int32_t)seg_len.size();
+	}
+};
+
 // Fragments of several segments (read pairs) in one go: fragment f has n_seg[f] consecutive entries of qlens/seqs/gcs starting at
 // seg_off[f] = n_seg[0] + ... + n_seg[f-1]; gcs[seg_off[f]] receives the result of the concatenated fragment and the other
 // entries NULL, exactly what worker_for() leaves behind without MG_M_INDEPEND_SEG (gmap.c:46-48).  names[f] is per fragment.
@@ -1816,29 +2098,59 @@ extern "C" int mg_map_batch_frag(const mg_idx_t *gi, int n_frag, const int *n_se
 	for (int f = 0; f < n_frag; ++f) { if (n_seg[f] != 1) single = false; n_tot += n_seg[f] > 0? n_seg[f] : 0; }
 	if (single) return map_batch_impl(gi, n_frag, qlens, seqs, names, gcs, opt);
 	for (int64_t i = 0; i < n_tot; ++i) gcs[i] = 0;
-	std::vector<std::string> cat((size_t)n_frag);
-	std::vector<int> qsum((size_t)n_frag);
-	std::vector<const char*> sq((size_t)n_frag);
-	std::vector<int32_t> seg_off((size_t)n_frag + 1), seg_len;
+	FragBatch fb(n_frag, n_seg, qlens, seqs);
 	std::vector<mg_gchains_t*> res((size_t)n_frag, (mg_gchains_t*)0);
-	seg_len.reserve((size_t)n_tot);
-	int64_t off = 0;
-	for (int f = 0; f < n_frag; ++f) {
-		seg_off[(size_t)f] = (int32_t)seg_len.size();
-		const int ns = n_seg[f] > 0 && n_seg[f] <= 255? n_seg[f] : 0; // more than MG_MAX_SEG segments: no result (map-algo.c:359)
-		for (int j = 0; j < ns; ++j) {
-			const int l = qlens[off + j] > 0? qlens[off + j] : 0;
-			seg_len.push_back(l);
-			if (l > 0) cat[(size_t)f].append(seqs[off + j], (size_t)l);
-		}
-		qsum[(size_t)f] = (int)cat[(size_t)f].size(), sq[(size_t)f] = cat[(size_t)f].data();
-		off += n_seg[f] > 0? n_seg[f] : 0;
-	}
-	seg_off[(size_t)n_frag] = (int32_t)seg_len.size();
-	int rc = map_batch_impl(gi, n_frag, qsum.data(), sq.data(), names, res.data(), opt, &seg_off, &seg_len);
+	int rc = map_batch_impl(gi, n_frag, fb.qsum.data(), fb.sq.data(), names, res.data(), opt, &fb.seg_off, &fb.seg_len);
 	if (rc < 0) return rc;
-	off = 0;
-	for (int f = 0; f < n_frag; ++f) { if (n_seg[f] > 0) gcs[off] = res[(size_t)f]; off += n_seg[f] > 0? n_seg[f] : 0; }
+	for (int f = 0; f < n_frag; ++f) if (n_seg[f] > 0) gcs[fb.first[(size_t)f]] = res[(size_t)f];
+	return 0;
+}
+
+// Map a batch and return its GAF text, formatted on the device (mgb_gaf.cuh, gaf_text).
+extern "C" int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, const int *qlens, const char *const *seqs, const char *const *names,
+								 const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap)
+{
+	const uint64_t F_CAL_COV = 0x4000, F_INDEPEND_SEG = 0x20000; // minigraph.h:19,22
+	char *fresh = 0;
+	auto dest = [&](size_t n) -> char* { // the caller's buffer, reused and grown, or a fresh block
+		if (out_cap == 0) return fresh = (char*)malloc(n + 1);
+		if (*out == 0 || *out_cap < n + 1) {
+			free(*out);
+			*out_cap = n + n / 8 + 1;
+			*out = (char*)malloc(*out_cap);
+			if (*out == 0) *out_cap = 0;
+		}
+		return *out;
+	};
+	auto fail = [&](int rc) { // no partial text
+		if (out_cap) { if (*out && *out_cap) (*out)[0] = 0; }
+		else { free(fresh); *out = 0; }
+		*out_len = 0;
+		return rc;
+	};
+	*out_len = 0;
+	if (opt->flag & (F_CAL_COV | F_INDEPEND_SEG)) { set_error("mgb_map_batch_gaf: --cov and independent segments print no per-fragment GAF record"); return fail(MGB_E_UNSUPPORTED); }
+	GafJob J;
+	J.flag = opt->flag, J.n_seg = 0, J.seg_first = 0, J.qlens = qlens, J.dest = dest, J.len = 0;
+	int rc = 0;
+	if (n_frag <= 0) {
+		char *o = dest(0);
+		if (o == 0) { set_error("mgb_map_batch_gaf: out of host memory"); return fail(MGB_E_INTERNAL); }
+		o[0] = 0;
+	} else {
+		bool single = true;
+		for (int f = 0; f < n_frag && n_seg; ++f) if (n_seg[f] != 1) single = false;
+		std::vector<mg_gchains_t*> gcs((size_t)n_frag, (mg_gchains_t*)0); // stays empty: the results go out as text
+		if (single) rc = map_batch_impl(gi, n_frag, qlens, seqs, names, gcs.data(), opt, 0, 0, &J);
+		else {
+			FragBatch fb(n_frag, n_seg, qlens, seqs);
+			J.n_seg = n_seg, J.seg_first = fb.first.data();
+			rc = map_batch_impl(gi, n_frag, fb.qsum.data(), fb.sq.data(), names, gcs.data(), opt, &fb.seg_off, &fb.seg_len, &J);
+		}
+		if (rc < 0) return fail(rc);
+	}
+	if (out_cap == 0) *out = fresh;
+	*out_len = J.len;
 	return 0;
 }
 
