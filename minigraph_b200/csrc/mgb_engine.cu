@@ -211,9 +211,6 @@ MG_HD inline int run_stage(const LaunchArgs &L, int item, Arena &A, int lane, in
 	if (S == S_FINISH) return stage_finish(L.c, L.routs, item, A, lane);
 	if (S == S_GWFA) return gwfa_job_run(A, L.c, L.job_start + item, lane, smem);
 	if (S == S_GCHAIN_GEN) return stage_gchain_gen(L.c, L.routs, item, A, lane);
-	if (S == S_WFA_SMALL) return wfa_job_run(A, L.c, L.job_start + item, lane, smem, 1);
-	if (S == S_WFA_MID) return wfa_job_run(A, L.c, L.c.jobq[0][item], lane, smem, 2);
-	if (S == S_WFA_BIG) return wfa_job_run(A, L.c, L.c.jobq[1][item], lane, smem, 3);
 	if (S == S_INDEX_SKETCH) { // sketch one graph segment for the index (reference: index.c:200-205)
 		AVec<u128> mv;
 		avec_init(mv);
@@ -249,6 +246,23 @@ MG_HD inline void stage_fail(const LaunchArgs &L, int item, int rc)
 	L.routs[rid].status = rc;
 }
 
+// The gap jobs of the WFA stages, as the traceback batch of a warp sees them (WfaBatch): the items of k_wfa_small are jobs from
+// job_start on, those of k_wfa_mid and k_wfa_big the queues tiers 1 and 2 filled.
+MG_HD constexpr bool is_wfa_stage(int S) { return S == S_WFA_SMALL || S == S_WFA_MID || S == S_WFA_BIG; }
+template<int S>
+struct WfaStageGaps {
+	const LaunchArgs &L;
+	int32_t *smem;
+	static constexpr int tier = S == S_WFA_SMALL? 1 : S == S_WFA_MID? 2 : 3;
+	MG_HD int run(int item, Arena &A, WfTbJob *tb, int lane) const
+	{
+		return wfa_job_run(A, L.c, tier == 1? L.job_start + item : (int64_t)L.c.jobq[tier - 2][item], lane, smem, tier, tb);
+	}
+	MG_HD int done(const WfTbJob &b, int lane) const { return wfa_job_finish(L.c, b, smem, tier, lane); }
+	MG_HD void fail(int item, int rc, int lane) const { if (lane == 0) stage_fail<S>(L, item, rc); }
+	MG_HD void traced(unsigned long long cyc, int lane) const { if (lane == 0) prof_add(L.c, PROF_WFA_TB_CYC, cyc); }
+};
+
 // What a warp of stage S does to its slice of shared memory before its first item (S < 0: nothing).  Warp-uniform.
 template<int S>
 MG_HD inline void stage_warp_init(int32_t *smem, int lane)
@@ -273,6 +287,9 @@ __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 	stage_warp_init<S>(smem, lane);
 	prof_block_begin();
 	const int n_work = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
+	const WfaStageGaps<S> gaps{L, smem};
+	WfaBatch<WfaStageGaps<S>> batch; // the WFA stages keep the arena across the gaps of a batch
+	if constexpr (is_wfa_stage(S)) batch.open(A);
 	int next_item = 0, have = 0;
 	for (;;) {
 		if (have == 0) {
@@ -284,7 +301,8 @@ __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 		--have;
 		if (item >= n_work) break;
 		if (L.rid_list) item = L.rid_list[item];
-		if (Spec::mode == ItemMode::WARP) {
+		if constexpr (is_wfa_stage(S)) batch.add(gaps, item, A, lane);
+		else if (Spec::mode == ItemMode::WARP) {
 			A.top = 0;
 			int rc = run_stage<S>(L, item, A, lane, smem);
 			if (rc < 0 && lane == 0) stage_fail<S>(L, item, rc);
@@ -295,6 +313,7 @@ __device__ __forceinline__ void stage_loop(const LaunchArgs &L)
 		}
 		__syncwarp();
 	}
+	if constexpr (is_wfa_stage(S)) batch.flush(gaps, A, lane);
 	if (lane == 0 && L.arena_peak) L.arena_peak[worker] = A.peak > L.arena_peak[worker]? A.peak : L.arena_peak[worker];
 	prof_block_end(L.c.prof);
 }
@@ -627,6 +646,26 @@ static int sim_warp(int stage, int item, const F &fn, bool *differ)
 	return fn(0);
 #endif
 }
+
+// One warp-uniform step fn(A, batch, lane) of a traceback batch (WfaBatch) on the simulated warp.  Every lane works on its own copy
+// of the arena header and the batch (in registers on the device); lane 0's copies are kept.  *differ is set when the lanes end
+// with different arena tops.
+template<typename B, typename F>
+static void sim_batch_step(int stage, int item, Arena &A, B &batch, const F &fn, bool *differ)
+{
+	Arena A0 = A;
+	B b0 = batch;
+	uint64_t peak = A.peak;
+	sim_warp(stage, item, [&](int lane) {
+		Arena Al = A;
+		B bl = batch;
+		fn(Al, bl, lane);
+		peak = std::max(peak, Al.peak);
+		if (lane == 0) A0 = Al, b0 = bl;
+		return (int)(Al.top >> 4) ^ bl.n << 24;
+	}, differ);
+	A = A0, A.peak = peak, batch = b0;
+}
 #endif
 
 template<int S>
@@ -643,6 +682,21 @@ static void launch_stage(LaunchArgs &L, const Workers &W)
 	bool differ = false;
 	sim_warp(S, -1, [&](int lane) { stage_warp_init<S>(smem, lane); return 0; }, &differ);
 	const int n_work_sim = L.n_work_dev? (int)*L.n_work_dev : L.n_work;
+	if constexpr (is_wfa_stage(S)) { // the warp's traceback batch, as on the device
+		const WfaStageGaps<S> gaps{L, smem};
+		WfaBatch<WfaStageGaps<S>> batch;
+		batch.open(A);
+		for (int it = 0; it <= n_work_sim; ++it) {
+			const int item = it == n_work_sim? -1 : L.rid_list? L.rid_list[it] : it;
+			sim_batch_step(S, item, A, batch, [&](Arena &Al, WfaBatch<WfaStageGaps<S>> &bl, int lane) {
+				if (item < 0) bl.flush(gaps, Al, lane);
+				else bl.add(gaps, item, Al, lane);
+			}, &differ);
+			if (differ) { set_error("simulated warp: lanes of a WFA stage's batch went apart"); abort(); }
+		}
+		if (W.peak && A.peak > W.peak[0]) W.peak[0] = A.peak;
+		return;
+	}
 	for (int it = 0; it < n_work_sim; ++it) {
 		int item = L.rid_list? L.rid_list[it] : it;
 		A.top = 0;
@@ -2261,9 +2315,16 @@ struct TestWfa {
 	MG_HD int operator()(int, int32_t *, Arena &A, int, int lane) const
 	{
 		WfResult r;
+		WfTbJob *tb = (WfTbJob*)arena_alloc(A, sizeof(WfTbJob)); // a batch of one
 		int rc = wfa_exact(A, tl, ts, ql, qs, max_iter, &r, lane, step);
-		if (rc == 0 && r.n_cigar <= cap) for (int32_t i = lane; i < r.n_cigar; i += MGB_W) cigar[i] = r.cigar[i];
-		if (lane == 0) out[0] = rc, out[1] = rc == 0? r.n_cigar : 0, out[2] = rc == 0? r.s : 0;
+		if (rc == 0) {
+			wfa_tb_keep(tb, r, tl, ts, ql, qs, 0, lane);
+			wfa_tb_batch(tb, 1, lane);
+			rc = tb->rc;
+		}
+		const int32_t n_cig = rc == 0? tb->n_cigar : 0;
+		if (rc == 0 && n_cig <= cap) for (int32_t i = lane; i < n_cig; i += MGB_W) cigar[i] = tb->cig[tb->first + i];
+		if (lane == 0) out[0] = rc, out[1] = n_cig, out[2] = rc == 0? r.s : 0;
 		return 0;
 	}
 };
@@ -2291,31 +2352,55 @@ extern "C" int mgb_test_wfa(const char *ts, int tl, const char *qs, int ql, int6
 
 // ---------------------------------------------------------------------------------------------------------------
 // test hook: a batch of gaps through one on-chip WFA tier, wfa_smem() with the template arguments of k_wfa_small (tier 1)
-// or k_wfa_mid (tier 2), launched as those kernels are (test_launch).  The junk in the slices is cells that are not -inf, so the
-// results also show that wfa_smem() clears the slices it reads.
+// or k_wfa_mid (tier 2), launched as those kernels are (test_launch), the tracebacks in the batches those kernels run (WfaBatch):
+// warp w takes gaps w, w + n_workers, ...  The junk in the slices is cells that are not -inf, so the results also show that
+// wfa_smem() clears the slices it reads.
 // ---------------------------------------------------------------------------------------------------------------
 struct TestTier {
-	int tier, cap;
+	int tier, cap, n, n_workers;
 	const char *ts, *qs;
 	const int64_t *t_off, *q_off;
 	const int32_t *tl, *ql;
 	int64_t *out;       // per gap: rc (0: aligned, 1: does not fit the tier), score, n_iter, n_cigar
 	uint32_t *cigar;    // per gap: cap entries
-	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
-	{
-		WfResult r;
-		A.top = 0;
-		const char *ts_i = ts + t_off[i], *qs_i = qs + q_off[i];
-		int64_t cont_cells = 0;
-		int rc = tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane)
-				: tier == 2? wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane)
-							: wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, tl[i], ts_i, ql[i], qs_i, &r, lane, &cont_cells);
-		if (rc == 0 && r.n_cigar > cap) rc = MGB_E_INTERNAL;
-		if (rc == 0) for (int32_t j = lane; j < r.n_cigar; j += MGB_W) cigar[(int64_t)i * cap + j] = r.cigar[j];
-		if (lane == 0) {
-			int64_t *o = out + 4 * (int64_t)i;
-			o[0] = rc, o[1] = rc == 0? r.s : -1, o[2] = rc == 0? r.n_iter : 0, o[3] = rc == 0? r.n_cigar : 0;
+	struct Gaps { // what the gaps are to the batch
+		const TestTier &t;
+		int32_t *smem;
+		MG_HD void put(int i, int64_t rc, int64_t s, int64_t n_iter, int64_t n_cigar, int lane) const
+		{
+			if (lane == 0) { int64_t *o = t.out + 4 * (int64_t)i; o[0] = rc, o[1] = s, o[2] = n_iter, o[3] = n_cigar; }
 		}
+		MG_HD int run(int i, Arena &A, WfTbJob *tb, int lane) const
+		{
+			WfResult r;
+			const char *ts_i = t.ts + t.t_off[i], *qs_i = t.qs + t.q_off[i];
+			int64_t cont_cells = 0;
+			const int rc = t.tier == 1? wfa_smem<WfTier1::W_, WfTier1::MAXLEN_, WfTier1::TBCAP_>(A, smem, t.tl[i], ts_i, t.ql[i], qs_i, &r, lane)
+					: t.tier == 2? wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_>(A, smem, t.tl[i], ts_i, t.ql[i], qs_i, &r, lane)
+								 : wfa_smem<WfTier2::W_, WfTier2::MAXLEN_, WfTier2::TBCAP_, true>(A, smem, t.tl[i], ts_i, t.ql[i], qs_i, &r, lane, &cont_cells);
+			if (rc == 1) put(i, 1, -1, 0, 0, lane);
+			if (rc != 0) return rc < 0? rc : 0;
+			wfa_tb_keep(tb, r, t.tl[i], ts_i, t.ql[i], qs_i, i, lane);
+			return 1;
+		}
+		MG_HD int done(const WfTbJob &b, int lane) const
+		{
+			if (b.rc < 0) return b.rc;
+			if (b.n_cigar > t.cap) return MGB_E_INTERNAL;
+			for (int32_t j = lane; j < b.n_cigar; j += MGB_W) t.cigar[b.job * t.cap + j] = b.cig[b.first + j];
+			put((int)b.job, 0, b.s, b.n_iter, b.n_cigar, lane);
+			return 0;
+		}
+		MG_HD void fail(int i, int rc, int lane) const { put(i, rc, -1, 0, 0, lane); }
+		MG_HD void traced(unsigned long long, int) const {}
+	};
+	MG_HD int operator()(int w, int32_t *smem, Arena &A, int, int lane) const
+	{
+		const Gaps g{*this, smem};
+		WfaBatch<Gaps> batch;
+		batch.open(A);
+		for (int i = w; i < n; i += n_workers) batch.add(g, i, A, lane);
+		batch.flush(g, A, lane);
 		warp_sync();
 		return 0;
 	}
@@ -2338,13 +2423,15 @@ static int test_wfa_tier_impl(int tier, int n, const char *ts, const int64_t *t_
 	DevBuf<int64_t> out_d(4 * (size_t)n);
 	DevBuf<uint32_t> cigar_d((size_t)n * cap + 1);
 	TestTier t;
-	t.tier = tier, t.cap = cap;
+	const int warps = tier == 1? StageSpec<S_WFA_SMALL>::warps : StageSpec<S_WFA_MID>::warps;
+	t.tier = tier, t.cap = cap, t.n = n, t.n_workers = (std::min(n, 64 * warps) + warps - 1) / warps * warps; // whole blocks, as launched
 	t.ts = ts_d, t.qs = qs_d, t.t_off = t_off_d, t.q_off = q_off_d, t.tl = tl_d, t.ql = ql_d, t.out = out_d, t.cigar = cigar_d;
 	// a tier-2 gap needs at most 8 KB of CIGAR and 70 KB of traceback rows; one carried on in the arena at most 230 KB of ring and
-	// 4.3 MB of traceback rows (scores below tl + ql + 30, rows of at most tl + ql + 1 bytes)
+	// 4.3 MB of traceback rows (scores below tl + ql + 30, rows of at most tl + ql + 1 bytes).  A batch is flushed once it keeps a
+	// quarter of the arena.
 	const uint64_t arena_bytes = tier == MGB_TEST_TIER2_CONT? (uint64_t)5 << 20 : (uint64_t)256 << 10;
-	const int rc = tier == 1? test_launch<S_WFA_SMALL>(n, std::min(n, 64 * StageSpec<S_WFA_SMALL>::warps), arena_bytes, t)
-							: test_launch<S_WFA_MID>(n, std::min(n, 64 * StageSpec<S_WFA_MID>::warps), arena_bytes, t);
+	const int rc = tier == 1? test_launch<S_WFA_SMALL>(t.n_workers, t.n_workers, arena_bytes, t)
+							: test_launch<S_WFA_MID>(t.n_workers, t.n_workers, arena_bytes, t);
 	if (rc) return rc;
 	d2h(out, out_d, sizeof(int64_t) * 4 * (size_t)n);
 	d2h(cigar, cigar_d, sizeof(uint32_t) * (size_t)n * cap);

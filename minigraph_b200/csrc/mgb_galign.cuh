@@ -61,13 +61,14 @@ static const unsigned long long CIG_CHUNK_BYTES = 2048; // a warp of a WFA kerne
 // Planning pass of mg_gchain_cigar() (reference: galign.c:39-124): walk the kept anchors of every graph chain, emit
 // literal CIGAR items for the trivial gaps (galign.c:98-100) and a WfaJob for the others.
 
-// K8a: align one gap.  Warp-uniform (all lanes enter with identical arguments).
+// K8a: the wavefronts of one gap.  Warp-uniform (all lanes enter with identical arguments).
 // tier 1: small gaps, wavefronts + traceback bytes in shared memory; tier 2: mid-size gaps, wavefronts in shared
 // memory, carried on in the worker arena when the window outgrows them (longer sides: in the arena from the start, while
 // wf_ring_always_fits); tier 3: anything, wavefronts in the worker arena.
 // A job that does not fit a tier is appended to the queue of the next one (jobq[tier-1]); the host launches the next tier
-// over that queue.
-MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int lane, int32_t *smem, int tier)
+// over that queue.  Returns 1 when the gap is aligned up to its traceback, which waits in *tb (and its rows, CIGAR store and
+// stitched target in the arena) for the rest of the warp's batch (WfaBatch); 0 when there is nothing to trace back.
+MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int lane, int32_t *smem, int tier, WfTbJob *tb)
 {
 	WfaJob *J = &c.jobs[job_idx];
 	if (J->rid < 0) return 0; // a slot no read wrote (its allocation ran over the end of the pool; the batch is re-run with a larger one)
@@ -167,12 +168,22 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 		return 0;
 	}
 	if (rst.s < 0) return MGB_E_INTERNAL;
+	wfa_tb_keep(tb, rst, tl, tseq, ql, qs, job_idx, lane);
+	return 1;
+}
+
+// K8a, after the traceback of the batch: the CIGAR of one gap into the pool.  Warp-uniform.
+MG_HD inline int wfa_job_finish(const PipeCtx &c, const WfTbJob &b, int32_t *smem, int tier, int lane)
+{
+	if (b.rc < 0) return b.rc;
+	const int32_t n_cigar = b.n_cigar;
+	const uint32_t *cigar = b.cig + b.first;
 	int64_t coff = 0;
 	if (lane == 0) {
 #if MGB_ON_DEVICE
 		unsigned long long *ck = wfa_cig_chunk(smem, tier); // the warp's slice of the pool
-		const unsigned long long need = ((unsigned long long)rst.n_cigar * 4 + 15) & ~15ULL;
-		if (ck == 0) coff = pool_alloc(c.pool_cig, (uint64_t)rst.n_cigar * 4);
+		const unsigned long long need = ((unsigned long long)n_cigar * 4 + 15) & ~15ULL;
+		if (ck == 0) coff = pool_alloc(c.pool_cig, (uint64_t)n_cigar * 4);
 		else if (ck[0] + need > ck[1]) {
 			const unsigned long long get = need > CIG_CHUNK_BYTES? need : CIG_CHUNK_BYTES;
 			const int64_t off = pool_alloc(c.pool_cig, get);
@@ -182,16 +193,68 @@ MG_HD inline int wfa_job_run(Arena &A, const PipeCtx &c, int64_t job_idx, int la
 		}
 		if (ck && coff >= 0) coff = (int64_t)ck[0], ck[0] += need;
 #else
-		coff = pool_alloc(c.pool_cig, (uint64_t)rst.n_cigar * 4);
+		coff = pool_alloc(c.pool_cig, (uint64_t)n_cigar * 4);
 #endif
 	}
 	coff = (int64_t)warp_bcast_u64((uint64_t)coff, 0);
 	if (coff < 0) return MGB_E_POOL;
 	uint32_t *dst = (uint32_t*)((char*)c.cig + coff);
-	for (int32_t x = lane; x < rst.n_cigar; x += MGB_W) dst[x] = rst.cigar[x];
-	if (lane == 0) J->n_cigar = rst.n_cigar, J->cig_off = coff;
+	for (int32_t x = lane; x < n_cigar; x += MGB_W) dst[x] = cigar[x];
+	if (lane == 0) { WfaJob *J = &c.jobs[b.job]; J->n_cigar = n_cigar, J->cig_off = coff; }
 	return 0;
 }
+
+// The traceback batch of a warp of a WFA kernel.  The warp computes the wavefronts of a gap with all lanes and keeps its traceback
+// rows in the arena; after MGB_W gaps, or once what the batch keeps passes a quarter of the arena, lane j traces gap j back
+// (wfa_tb_batch) and the warp hands the CIGARs on.  The records sit at the bottom of the arena, the gaps' memory above them.  G is
+// what the gaps are to the caller:
+//   int run(int item, Arena &, WfTbJob *, int lane)  the wavefronts (wfa_job_run): < 0 failed, 0 nothing to trace back, 1 kept
+//   int done(const WfTbJob &, int lane)              the traced CIGAR (wfa_job_finish), < 0 on failure
+//   void fail(int item, int rc, int lane)             record the failure of the item
+//   void traced(unsigned long long cyc, int lane)     lane 0's clock cycles of the batch's traceback
+// A gap that runs out of arena while the batch holds others is run again after the batch is flushed, so that what fails for lack
+// of arena is what fails on its own.  Warp-uniform; the state is the same on every lane.
+template<typename G>
+struct WfaBatch {
+	WfTbJob *rec;
+	int32_t n;
+	MG_HD void open(Arena &A)
+	{
+		A.top = 0, n = 0;
+		rec = (WfTbJob*)arena_alloc(A, (uint64_t)MGB_W * sizeof(WfTbJob)); // (the arena of a WFA kernel is far larger)
+	}
+	MG_HD void flush(const G &g, Arena &A, int lane)
+	{
+		if (n > 0) {
+			const unsigned long long t0 = prof_clock();
+			wfa_tb_batch(rec, n, lane);
+			g.traced(prof_clock() - t0, lane);
+			for (int32_t j = 0; j < n; ++j) {
+				const WfTbJob &b = rec[j];
+				const int rc = g.done(b, lane);
+				if (rc < 0) g.fail(b.item, rc, lane);
+			}
+			warp_sync();
+		}
+		open(A);
+	}
+	MG_HD void add(const G &g, int item, Arena &A, int lane)
+	{
+		uint64_t mark = A.top;
+		int rc = g.run(item, A, rec + n, lane);
+		if (rc == MGB_E_ARENA && n > 0) {
+			flush(g, A, lane);
+			mark = A.top;
+			rc = g.run(item, A, rec + n, lane);
+		}
+		if (rc < 0) g.fail(item, rc, lane);
+		if (rc == 1) {
+			if (lane == 0) rec[n].item = item;
+			++n;
+		} else A.top = mark;
+		if (n == MGB_W || A.top > A.cap / 4) flush(g, A, lane);
+	}
+};
 
 // Finishing pass of mg_gchain_cigar() (reference: galign.c:125-141): concatenate plan items and job CIGARs.
 

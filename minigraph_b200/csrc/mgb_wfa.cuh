@@ -5,7 +5,8 @@
 //
 // One warp aligns one gap.  Lanes own diagonals in the three data-parallel phases of a score step (exact-match
 // extension, recurrence, traceback-byte store); the scalar bookkeeping ([lo,hi] tracking, iteration counting) is
-// replicated on all lanes; the traceback walk is sequential on lane 0.  Two storage schemes share that skeleton:
+// replicated on all lanes; the traceback walk is sequential, so the job tiers keep the traceback rows of up to MGB_W gaps and walk
+// them back one gap per lane (wfa_tb_batch).  Two storage schemes share that skeleton:
 //   wfa_smem<W,..>  wavefront ring in shared memory for windows of at most W diagonals and scores below 255
 //   wfa_exact       ring in the worker arena (global memory), any size, incl. the band re-centring every 256 scores
 // Only one diagonal (d = ql - tl) can reach the end of both sequences, so "the first diagonal that finishes" of the
@@ -24,11 +25,16 @@ static const int WF_SEQ_PAD = 16;           // sentinel bytes after each staged 
 
 #define MGB_WF_MAX(a, b) ((a) >= (b)? (a) : (b))
 
+struct WfTbRow;
 struct WfResult {
 	int32_t s;        // score, -1 if the iteration cap was hit
 	int32_t n_cigar;
 	int64_t n_iter;
 	uint32_t *cigar;  // len<<4|op  (op: 7 '=', 8 'X', 1 'I', 2 'D'), allocated at the caller's mark
+	// The job tiers stop after the score loop: rows != 0 means that the traceback is still to run (wfa_tb_batch), from these rows,
+	// into cigar[0 .. tl + ql + 2); the rows stay in the arena above the caller's mark.  rows == 0: cigar[0 .. n_cigar) is final.
+	const WfTbRow *rows;
+	int32_t n_rows, last_state;
 };
 
 // ---- sequence staging: 4-byte aligned copies followed by sentinel bytes that match nothing ----
@@ -68,7 +74,7 @@ MG_HD inline int32_t wf_extend(const char *ts, const char *qs, int32_t k, int32_
 	}
 }
 
-// ---- traceback (reference: miniwfa.c:329-377 wf_traceback), lane 0 only ----
+// ---- traceback (reference: miniwfa.c:329-377 wf_traceback), one lane per gap ----
 // TB::get(s, d) returns the traceback byte of (score s, diagonal d) or -1 if out of range.  Operations are
 // accumulated in registers and written from the back of cig_store, so no reversal pass is needed.
 template<typename TB>
@@ -148,17 +154,6 @@ struct WfSmemLayout {
 template<int W>
 MG_HD inline int32_t wfs_col(int32_t d) { return (d + (1 << 20)) & (W - 1); }
 
-struct WfTbSmem { // traceback bytes in shared memory: row table {lo, width, off} is packed as lo, off; width from the next row
-	const int32_t *row; const uint8_t *x; int32_t n_rows, used;
-	MG_HD int32_t get(int32_t s, int32_t d) const
-	{
-		int32_t lo = row[2 * s], off = row[2 * s + 1];
-		int32_t end = s + 1 < n_rows? row[2 * s + 3] : used;
-		int32_t j = d - lo;
-		return (j < 0 || off + j >= end)? -1 : (int32_t)x[off + j];
-	}
-};
-
 struct WfTbRow { int32_t lo, hi; uint8_t *x; };
 struct WfTbArena { // traceback rows bump-allocated in the worker arena (reference: miniwfa.c:31-44 wf_tb_add)
 	const WfTbRow *row;
@@ -168,6 +163,44 @@ struct WfTbArena { // traceback rows bump-allocated in the worker arena (referen
 		return (j < 0 || j > row[s].hi - row[s].lo)? -1 : (int32_t)row[s].x[j];
 	}
 };
+
+// A gap whose wavefronts are done and whose traceback waits for the other gaps of its batch.  Its rows, its CIGAR store and a
+// stitched target stay in the worker arena until then; the read and the graph sequences are read where they live in global memory
+// (the staged copies in shared memory belong to the next gap by then).
+struct WfTbJob {
+	const WfTbRow *rows;      // 0: nothing to trace back, the CIGAR is cig[0 .. n_cigar) already
+	const char *ts, *qs;
+	uint32_t *cig;            // tl + ql + 2 entries, written from the back by the traceback
+	int64_t n_iter, first;    // first: where the CIGAR starts in cig
+	int64_t job;              // the caller's: which job this is
+	int32_t n_rows, last_state, tl, ql, s, item, rc, n_cigar;
+};
+
+MG_HD inline void wfa_tb_keep(WfTbJob *b, const WfResult &r, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t job, int lane)
+{
+	if (lane == 0) {
+		b->rows = r.rows, b->ts = ts, b->qs = qs, b->cig = r.cigar, b->n_iter = r.n_iter, b->first = 0, b->job = job;
+		b->n_rows = r.n_rows, b->last_state = r.last_state, b->tl = tl, b->ql = ql, b->s = r.s, b->item = 0, b->rc = 0, b->n_cigar = r.n_cigar;
+	}
+}
+
+// The tracebacks of a batch of n <= MGB_W gaps, lane j on gap j; rc, n_cigar and first of every record are set on return.
+// Warp-uniform.
+MG_HD inline void wfa_tb_batch(WfTbJob *rec, int32_t n, int lane)
+{
+	warp_sync(); // the records are complete
+	for (int32_t j = lane; j < n; j += MGB_W) {
+		WfTbJob &b = rec[j];
+		if (b.rows == 0) continue;
+		WfTbArena t;
+		t.row = b.rows;
+		int32_t n_cig = 0;
+		int64_t first = 0;
+		b.rc = wf_traceback(t, b.n_rows, b.tl, b.ts, b.ql, b.qs, b.last_state, b.cig, (int64_t)b.tl + b.ql + 2, &n_cig, &first);
+		b.n_cigar = n_cig, b.first = first;
+	}
+	warp_sync();
+}
 
 
 // =================================================================================================================
@@ -742,8 +775,7 @@ MG_HD inline int wfa_chain(Arena &A, int32_t tl, const char *ts, int32_t ql, con
 
 // Tier 3 entry (reference: miniwfa.c:824-834 mwf_wfa_auto): exact alignment capped at max_iter cells by the whole warp;
 // beyond the cap the chaining heuristic takes over on lane 0.
-MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
-							 uint32_t *cig_store, int64_t max_cigar, int lane); // mgb_wfa_tiers.cuh
+MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r, int lane); // mgb_wfa_tiers.cuh
 // the two rare continuations of tier 3, out of line: they are most of the kernel's code and would set its register count
 MG_HD MG_NOINLINE inline int wfa_core_cold(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r, uint32_t *cig_store, int64_t max_cigar, int lane)
 {
@@ -754,10 +786,12 @@ MG_HD MG_NOINLINE inline int wfa_chain_cold(Arena &A, int32_t tl, const char *ts
 	return wfa_chain(A, tl, ts_g, ql, qs_g, r, cig_store, max_cigar, step);
 }
 
+// With the 16-bit ring the traceback is left to the caller (WfResult::rows); the 32-bit ring and the chaining heuristic, both rare,
+// trace back on their own (the heuristic piece by piece) and return the CIGAR.
 MG_HD inline int wfa_exact(Arena &A, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, int64_t max_iter, WfResult *r, int lane, int32_t step = 5000)
 {
 	uint64_t mark = A.top;
-	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0;
+	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0, r->rows = 0, r->n_rows = 0, r->last_state = 0;
 	uint32_t *cig_store;
 	const int64_t max_cigar = (int64_t)tl + ql + 2;
 	MGB_ALLOC(A, cig_store, uint32_t, max_cigar);
@@ -769,8 +803,9 @@ MG_HD inline int wfa_exact(Arena &A, int32_t tl, const char *ts_g, int32_t ql, c
 	wf_stage_seq(qs, qs_g, ql, 0xff, lane);
 	warp_sync();
 	{
-		int rc = wfa_ring_g(A, tl, ts, ql, qs, max_iter, r, cig_store, max_cigar, lane);
+		int rc = wfa_ring_g(A, tl, ts, ql, qs, max_iter, r, lane);
 		if (rc < 0) return rc;
+		if (rc == 0 && r->s >= 0) { r->cigar = cig_store; return 0; } // the rows stay above mark_keep
 		if (rc == 1) { // (through a copy: an arena header whose address is taken would live in local memory for the whole kernel)
 			Arena B = A;
 			rc = wfa_core_cold(B, tl, ts, ql, qs, max_iter, r, cig_store, max_cigar, lane);

@@ -115,11 +115,12 @@ MG_HD inline uint32_t wf_ring_range(const WfTbRow *rows, int32_t sc)
 
 template<int W>
 MG_HD inline int wfa_smem_continue(Arena &A, uint64_t mark, const wf_cell_t *sm, int32_t tl, const char *ts, int32_t ql, const char *qs, WfResult *r,
-								   uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R);
+								   int lane, WfRing &R);
 
-// Returns 0 (aligned) or 1 (does not fit: the caller hands the gap to the next tier).  With CONT (tier 2 in its kernel), a gap whose
-// window outgrows the W columns before score 240 is not given up but carried on in the arena ring of tier 3 by the same warp
-// (wfa_smem_continue); *cont_cells then counts the cells computed there.
+// Returns 0 (aligned up to the traceback: see WfResult) or 1 (does not fit: the caller hands the gap to the next tier).  With CONT
+// (tier 2 in its kernel), a gap whose window outgrows the W columns before score 240 is not given up but carried on in the arena
+// ring of tier 3 by the same warp (wfa_smem_continue); *cont_cells then counts the cells computed there.  Tier 1 keeps its
+// traceback bytes in shared memory while it runs and copies them to the arena at the end, as the rows every tier traces back from.
 template<int W, int MAXLEN, int TBCAP, bool CONT = false>
 MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, WfResult *r, int lane, int64_t *cont_cells = 0)
 {
@@ -140,10 +141,10 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 	}
 	wf_stage_seq(ts, ts_g, tl, 0xfe, lane);
 	wf_stage_seq(qs, qs_g, ql, 0xff, lane);
-	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0;
+	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0, r->rows = 0, r->n_rows = 0, r->last_state = 0;
 	uint32_t *cig_store;
-	const int64_t max_cigar = (int64_t)tl + ql + 2;
-	MGB_ALLOC(A, cig_store, uint32_t, max_cigar);
+	MGB_ALLOC(A, cig_store, uint32_t, (int64_t)tl + ql + 2);
+	r->cigar = cig_store;
 	uint64_t mark_keep = A.top;
 	AVec<WfTbRow> rows; // TBCAP == 0 only
 	avec_init(rows);
@@ -171,15 +172,7 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 	for (;;) {
 		// invariant: the wavefront of score s is computed, extended along exact matches and visible to all lanes;
 		// a slice holds -inf everywhere outside the range it was last written with
-		if (hit) {
-			if (hit_noext) { // no extension on the last diagonal: the state comes from the traceback byte
-				int32_t x;
-				if (TBCAP > 0) { WfTbSmem t; t.row = tb_row, t.x = tb_x, t.n_rows = n_rows, t.used = tb_used; x = t.get(n_rows - 1, ql - tl); }
-				else { WfTbArena t; t.row = rows.a; x = t.get(n_rows - 1, ql - tl); }
-				last_state = x & 7;
-			}
-			break;
-		}
+		if (hit) break;
 		const int32_t lo = wlo > -tl? wlo - 1 : -tl;
 		const int32_t hi = whi < ql? whi + 1 : ql;
 		const int32_t width = hi - lo + 1;
@@ -187,7 +180,7 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 			if (CONT && s < 240) { // (then the window is what outgrew the ring)
 				WfRing R;
 				R.rows = rows, R.n_rows = n_rows, R.wlo = wlo, R.whi = whi, R.s = s, R.hs = hs, R.m3 = m3, R.m2 = m2, R.n_iter = n_iter;
-				const int rc = wfa_smem_continue<W>(A, mark_keep, H, tl, ts, ql, qs, r, cig_store, max_cigar, lane, R);
+				const int rc = wfa_smem_continue<W>(A, mark_keep, H, tl, ts, ql, qs, r, lane, R);
 				if (rc < 0) { A.top = mark; return rc; }
 				if (r->s < 0) { A.top = mark; return MGB_E_INTERNAL; } // (the cell cap cannot be reached, see wfa_smem_continue)
 				*cont_cells = r->n_iter - n_iter;
@@ -233,22 +226,22 @@ MG_HD inline int wfa_smem(Arena &A, int32_t *smem, int32_t tl, const char *ts_g,
 		n_iter += width;
 		warp_sync();
 	}
-	r->n_iter = n_iter;
-	r->s = s;
-	{
-		int rc = 0;
-		int32_t n_cig = 0;
-		int64_t first = 0;
-		if (lane == 0) {
-			if (TBCAP > 0) { WfTbSmem t; t.row = tb_row, t.x = tb_x, t.n_rows = n_rows, t.used = tb_used; rc = wf_traceback(t, n_rows, tl, ts, ql, qs, last_state, cig_store, max_cigar, &n_cig, &first); }
-			else { WfTbArena t; t.row = rows.a; rc = wf_traceback(t, n_rows, tl, ts, ql, qs, last_state, cig_store, max_cigar, &n_cig, &first); }
+	if (TBCAP > 0) { // the rows {lo, off} and bytes in shared memory become rows in the arena (row s ends where row s + 1 starts)
+		WfTbRow *ar;
+		uint8_t *ab;
+		MGB_ALLOC(A, ar, WfTbRow, n_rows);
+		MGB_ALLOC(A, ab, uint8_t, tb_used);
+		for (int32_t i = lane; i < tb_used; i += MGB_W) ab[i] = tb_x[i];
+		for (int32_t i = lane; i < n_rows; i += MGB_W) {
+			const int32_t lo = tb_row[2 * i], off = tb_row[2 * i + 1], end = i + 1 < n_rows? tb_row[2 * i + 3] : tb_used;
+			ar[i].lo = lo, ar[i].hi = lo + end - off - 1, ar[i].x = ab + off;
 		}
-		rc = warp_bcast_i32(rc, 0), n_cig = warp_bcast_i32(n_cig, 0), first = (int64_t)warp_bcast_u64((uint64_t)first, 0);
 		warp_sync();
-		if (rc < 0) { A.top = mark; return rc; }
-		r->n_cigar = n_cig, r->cigar = cig_store + first;
+		rows.a = ar;
 	}
-	A.top = mark_keep;
+	if (hit_noext) { WfTbArena t; t.row = rows.a; last_state = t.get(n_rows - 1, ql - tl) & 7; } // no extension on the last diagonal: the state comes from the traceback byte
+	r->n_iter = n_iter, r->s = s;
+	r->rows = rows.a, r->n_rows = n_rows, r->last_state = last_state;
 	return 0;
 }
 
@@ -293,9 +286,10 @@ static const int WF3_NSL = 17 + 3 + 3 + 2 + 2 + 1;
 		} \
 	} while (0)
 
-// the score loop of tier 3 from the state R, then the traceback into cig_store; A.top is set back to mark on return
+// the score loop of tier 3 from the state R.  Aligned: the traceback rows are in r (the ring and the rows stay allocated); stopped at
+// the cell cap or failed: A.top is set back to mark.
 MG_HD inline int wfa_ring_run(Arena &A, uint64_t mark, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
-							  uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R)
+							  int lane, WfRing &R)
 {
 	const int32_t W = R.W, mask = W - 1;
 	wf_cell_t *cells = R.cells;
@@ -392,25 +386,12 @@ MG_HD inline int wfa_ring_run(Arena &A, uint64_t mark, int32_t tl, const char *t
 #undef MGB_WF_GSET
 	r->n_iter = n_iter;
 	r->s = stopped? -1 : s;
-	if (!stopped) {
-		int rc = 0;
-		int32_t n_cig = 0;
-		int64_t first = 0;
-		if (lane == 0) {
-			WfTbArena t; t.row = rows.a;
-			rc = wf_traceback(t, n_rows, tl, ts, ql, qs, last_state, cig_store, max_cigar, &n_cig, &first);
-		}
-		rc = warp_bcast_i32(rc, 0), n_cig = warp_bcast_i32(n_cig, 0), first = (int64_t)warp_bcast_u64((uint64_t)first, 0);
-		warp_sync();
-		if (rc < 0) { A.top = mark; return rc; }
-		r->n_cigar = n_cig, r->cigar = cig_store + first;
-	}
-	A.top = mark;
+	if (stopped) A.top = mark;
+	else r->rows = rows.a, r->n_rows = n_rows, r->last_state = last_state;
 	return 0;
 }
 
-MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r,
-							uint32_t *cig_store, int64_t max_cigar, int lane)
+MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, const char *qs, int64_t max_iter, WfResult *r, int lane)
 {
 	if (tl + ql > 16000 || tl <= 0 || ql <= 0) return 1; // (scores stay below 2^15 too: deleting one sequence and inserting the other costs tl + ql + 30)
 	uint64_t mark = A.top;
@@ -444,7 +425,7 @@ MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, co
 	warp_sync();
 	R.cells = cells, R.W = W, R.flo = flo, R.fhi = fhi;
 	R.n_rows = 0, R.wlo = R.whi = R.s = 0, R.hs = R.m3 = R.m2 = 0, R.hit = hit, R.hit_noext = hit_noext, R.n_iter = 0;
-	return wfa_ring_run(A, mark, tl, ts, ql, qs, max_iter, r, cig_store, max_cigar, lane, R);
+	return wfa_ring_run(A, mark, tl, ts, ql, qs, max_iter, r, lane, R);
 }
 
 // Gaps of tier 2 with a side longer than its shared memory holds: the arena ring from score 0, when the gap is small enough that
@@ -453,21 +434,19 @@ MG_HD inline int wfa_ring_g(Arena &A, int32_t tl, const char *ts, int32_t ql, co
 MG_HD inline bool wf_ring_always_fits(int32_t tl, int32_t ql) { const int64_t n = (int64_t)tl + ql; return (n + 30) * (n + 1) <= 100000000LL; }
 MG_HD inline int wfa_ring_exact(Arena &A, int32_t tl, const char *ts_g, int32_t ql, const char *qs_g, WfResult *r, int lane)
 {
-	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0;
+	r->s = -1, r->n_cigar = 0, r->n_iter = 0, r->cigar = 0, r->rows = 0, r->n_rows = 0, r->last_state = 0;
 	uint32_t *cig_store;
-	const int64_t max_cigar = (int64_t)tl + ql + 2;
-	MGB_ALLOC(A, cig_store, uint32_t, max_cigar);
-	const uint64_t mark_keep = A.top;
+	MGB_ALLOC(A, cig_store, uint32_t, (int64_t)tl + ql + 2);
 	char *ts, *qs;
 	MGB_ALLOC(A, ts, char, tl + WF_SEQ_PAD + 4);
 	MGB_ALLOC(A, qs, char, ql + WF_SEQ_PAD + 4);
 	wf_stage_seq(ts, ts_g, tl, 0xfe, lane);
 	wf_stage_seq(qs, qs_g, ql, 0xff, lane);
 	warp_sync();
-	const int rc = wfa_ring_g(A, tl, ts, ql, qs, 100000000LL, r, cig_store, max_cigar, lane);
+	const int rc = wfa_ring_g(A, tl, ts, ql, qs, 100000000LL, r, lane);
 	if (rc < 0) return rc;
 	if (rc != 0 || r->s < 0) return MGB_E_INTERNAL; // (excluded by wf_ring_always_fits)
-	A.top = mark_keep;
+	r->cigar = cig_store;
 	return 0;
 }
 
@@ -480,7 +459,7 @@ MG_HD inline int wfa_ring_exact(Arena &A, int32_t tl, const char *ts_g, int32_t 
 // far below the cap of 10^8, so neither the 32-bit ring nor the chaining heuristic of tier 3 (wfa_exact) can be reached.
 template<int W>
 MG_HD inline int wfa_smem_continue(Arena &A, uint64_t mark, const wf_cell_t *sm, int32_t tl, const char *ts, int32_t ql, const char *qs, WfResult *r,
-								   uint32_t *cig_store, int64_t max_cigar, int lane, WfRing &R)
+								   int lane, WfRing &R)
 {
 	int32_t W2 = 64;
 	while (W2 < tl + ql + 2) W2 <<= 1;
@@ -501,7 +480,7 @@ MG_HD inline int wfa_smem_continue(Arena &A, uint64_t mark, const wf_cell_t *sm,
 #endif
 	R.hit = R.hit_noext = 0;
 	warp_sync();
-	return wfa_ring_run(A, mark, tl, ts, ql, qs, 100000000LL, r, cig_store, max_cigar, lane, R);
+	return wfa_ring_run(A, mark, tl, ts, ql, qs, 100000000LL, r, lane, R);
 }
 #undef MGB_WF_RG
 #undef MGB_WF2_CLEAN
