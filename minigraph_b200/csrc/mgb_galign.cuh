@@ -33,8 +33,6 @@ MG_HD inline int cigar_append(Arena &A, AVec<uint64_t> &c, int32_t n_cigar, cons
 	return 0;
 }
 
-struct CigarOut { uint64_t *cigar; int32_t n; };
-
 // One gap between two kept anchors that needs a real alignment.  Produced by the planning pass of K6/K7 (one lane
 // per read), consumed by the WFA kernel K8a (one warp per job), stitched back by the finishing pass.
 struct WfaJob {
@@ -256,271 +254,241 @@ struct WfaBatch {
 	}
 };
 
-// Finishing pass of mg_gchain_cigar() (reference: galign.c:125-141): concatenate plan items and job CIGARs.
+// ---- K8b: the stitched CIGAR and the ds:Z string of every chain, written once, straight into the result blob ----
 
-#if MGB_ON_DEVICE
-MG_D inline void lane_atomic_add_u64(uint64_t *p, uint64_t v) { atomicAdd((unsigned long long*)p, (unsigned long long)v); }
-#else
-inline void lane_atomic_add_u64(uint64_t *p, uint64_t v) { *p += v; } // lanes of the simulators never run concurrently
-#endif
-
-// gchain_cigar_finish() entered by all lanes of a warp (stage_finish<1>, parameter "fin_v2").  The reference appends item after
-// item and merges the first operation of an item into the last one written when they are of the same kind (galign.c:125-141 via
-// mg_cigar_push); nothing else is ever merged.  Here: (1) a prefix sum over the items gives every item its place in a flat list,
-// (2) the lanes copy the items there, the first operation of each item tagged, (3) a tagged operation that equals its left
-// neighbour continues that neighbour's run, every other operation starts a run; the runs are numbered by a ballot prefix
-// count and their lengths added up.  Same list as the sequential append, operation for operation.
-MG_HD inline int gchain_cigar_finish_w(Arena &A, const PipeCtx &c, GcSet &gt, CigarOut *out, int lane)
+MG_HD inline int mask_lowest(uint32_t m) // index of the lowest set bit of a non-zero mask
 {
-	const uint64_t FIRST = 1ULL << 62; // tag: first operation of an item (lengths stay far below 2^58)
-	for (int32_t i = 0; i < gt.n_gc; ++i) {
-		GChain *gc = &gt.gc[i];
-		const int32_t off_a0 = gt.lc[gc->off].off, n_plan = gc->n_plan;
-		const uint64_t *plan = c.plan + gc->plan_off;
-		int32_t *ioff;
-		MGB_ALLOC(A, ioff, int32_t, n_plan + 1);
-		int32_t tot = 0;
-		for (int32_t base = 0; base < n_plan; base += MGB_W) {
-			const int32_t t = base + lane;
-			int32_t cnt = 0;
-			if (t < n_plan) cnt = (plan[t] & PLAN_JOB)? c.jobs[plan[t] & ~PLAN_JOB].n_cigar : 1;
-			const int32_t incl = warp_incl_scan_i32(cnt, lane);
-			if (t < n_plan) ioff[t] = tot + incl - cnt;
-			tot += warp_bcast_i32(incl, MGB_W - 1);
-		}
-		uint64_t *F, *O;
-		int32_t *oidx;
-		MGB_ALLOC(A, F, uint64_t, tot + 1);
-		MGB_ALLOC(A, O, uint64_t, tot + 1);
-		MGB_ALLOC(A, oidx, int32_t, tot + 1);
-		warp_sync();
-		for (int32_t t = lane; t < n_plan; t += MGB_W) {
-			uint64_t *dst = F + ioff[t];
-			if (plan[t] & PLAN_JOB) {
-				const WfaJob *J = &c.jobs[plan[t] & ~PLAN_JOB];
-				const uint32_t *cig = (const uint32_t*)((const char*)c.cig + J->cig_off);
-				for (int32_t k = 0; k < J->n_cigar; ++k) dst[k] = (uint64_t)cig[k] | (k == 0? FIRST : 0);
-			} else dst[0] = plan[t] | FIRST;
-		}
-		warp_sync();
-		int32_t n_out = 0;
-		for (int32_t base = 0; base < tot; base += MGB_W) {
-			const int32_t j = base + lane;
-			int head = 0;
-			if (j < tot) head = j == 0 || !((F[j] & FIRST) && (F[j] & 0xf) == (F[j - 1] & 0xf));
-			const uint32_t mh = warp_ballot(head);
-			if (j < tot) {
-				const int32_t o = n_out + mask_rank(mh, lane) + head - 1;
-				oidx[j] = o;
-				if (head) O[o] = F[j] & 0xf;
+#if MGB_ON_DEVICE
+	return __ffs(m) - 1;
+#else
+	return __builtin_ctz(m);
+#endif
+}
+
+// Finishing pass of mg_gchain_cigar() (reference: galign.c:125-141): the stitched CIGAR of chain i, to *ops (n_cigar of them).
+// The reference appends item after item and merges the first operation of an item into the last one written when they are of
+// the same kind; nothing else is ever merged.  Here a prefix sum over the plan items gives every item its place in a flat list;
+// the warp walks that list MGB_W operations at a time, lane l on operation base+l: it finds its item by a binary search and reads
+// the operation (the lanes on one job read neighbouring words of its CIGAR).  An operation starts a run unless it is the first of
+// its item and of the same kind as its left neighbour.  The runs are numbered by a ballot and their lengths added up by a
+// segmented scan (the inclusive sum less the sum in front of the run's head); a run still open at the end of a group is written
+// as it stands and carried into the next group, which writes it again.  Same list as the sequential append, operation for
+// operation.  Warp-uniform.
+MG_HD inline int gchain_cigar_finish_w(Arena &A, const PipeCtx &c, GcSet &gt, int32_t i, uint64_t **ops, int lane)
+{
+	GChain *gc = &gt.gc[i];
+	const int32_t off_a0 = gt.lc[gc->off].off, n_plan = gc->n_plan;
+	const uint64_t *plan = c.plan + gc->plan_off;
+	int32_t *ioff;
+	MGB_ALLOC(A, ioff, int32_t, n_plan + 1);
+	int32_t tot = 0;
+	for (int32_t base = 0; base < n_plan; base += MGB_W) {
+		const int32_t t = base + lane;
+		int32_t cnt = 0;
+		if (t < n_plan) cnt = (plan[t] & PLAN_JOB)? c.jobs[plan[t] & ~PLAN_JOB].n_cigar : 1;
+		const int32_t incl = warp_incl_scan_i32(cnt, lane);
+		if (t < n_plan) ioff[t] = tot + incl - cnt;
+		tot += warp_bcast_i32(incl, MGB_W - 1);
+	}
+	uint64_t *O;
+	MGB_ALLOC(A, O, uint64_t, tot);
+	warp_sync();
+	int32_t n_out = 0, t_lo = 0, carry = 0, prev_op = 0, mlen = 0, blen = 0, aplen = 0, l = 0;
+	for (int32_t base = 0; base < tot; base += MGB_W) {
+		const int32_t j = base + lane;
+		int32_t t = t_lo, op = 0, len = 0, first = 0;
+		if (j < tot) {
+			for (int32_t hi = n_plan - 1; t < hi; ) { // the last item that starts at or before j (an item without operations starts where the next one does)
+				const int32_t mid = (t + hi + 1) >> 1;
+				if (ioff[mid] <= j) t = mid;
+				else hi = mid - 1;
 			}
-			n_out += mask_count(mh);
-		}
-		warp_sync();
-		for (int32_t j = lane; j < tot; j += MGB_W) lane_atomic_add_u64(&O[oidx[j]], (F[j] & ~FIRST) >> 4 << 4);
-		warp_sync();
-		int32_t mlen = 0, blen = 0, aplen = 0, l = 0;
-		for (int32_t j = lane; j < n_out; j += MGB_W) {
-			const int32_t op = (int32_t)(O[j] & 0xf), len = (int32_t)(O[j] >> 4);
+			uint64_t v = plan[t];
+			if (v & PLAN_JOB) {
+				const WfaJob *J = &c.jobs[v & ~PLAN_JOB];
+				v = ((const uint32_t*)((const char*)c.cig + J->cig_off))[j - ioff[t]];
+			}
+			op = (int32_t)(v & 0xf), len = (int32_t)(v >> 4), first = j == ioff[t];
 			if (op == 7) mlen += len;
 			blen += len;
 			if (op != 1) aplen += len;
 			if (op != 2) l += len;
 		}
-		mlen = warp_sum_i32(mlen), blen = warp_sum_i32(blen), aplen = warp_sum_i32(aplen), l = warp_sum_i32(l);
-		if (lane == 0) {
-			out[i].cigar = O, out[i].n = n_out;
-			gc->has_cigar = 1;
-			gc->n_cigar = n_out;
-			gc->c_ss = (int32_t)gt.a[off_a0].x + 1 - (int32_t)(gt.a[off_a0].y >> 32 & 0xff);
-			gc->c_ee = (int32_t)gt.a[off_a0 + gc->n_anchor - 1].x + 1;
-			gc->c_mlen = mlen, gc->c_blen = blen, gc->c_aplen = aplen;
-		}
-		if (!(l == gc->qe - gc->qs && aplen == gc->pe - gc->ps)) return MGB_E_INTERNAL;
-		warp_sync();
+		const int32_t up = (int32_t)warp_shfl_up1_u64((uint64_t)(uint32_t)op);
+		const int32_t left = lane > 0? up : prev_op;
+		const int head = j < tot && (j == 0 || !(first && op == left));
+		const uint32_t mh = warp_ballot(head);
+		const int32_t incl = warp_incl_scan_i32(len, lane);
+		const uint64_t hs = warp_incl_scan_max_u64(head? (uint64_t)(incl - len) + 1 : 0, lane); // 1 + the sum in front of the last head up to here
+		const int32_t run = hs? incl - (int32_t)(hs - 1) : carry + incl;
+		const int32_t o = n_out + mask_rank(mh, lane) + head - 1;
+		if (j < tot && (lane == MGB_W - 1 || j == tot - 1 || (mh >> (lane + 1) & 1))) O[o] = (uint64_t)(int64_t)run << 4 | (uint64_t)op;
+		carry = warp_bcast_i32(run, MGB_W - 1), prev_op = warp_bcast_i32(op, MGB_W - 1), t_lo = warp_bcast_i32(t, MGB_W - 1);
+		n_out += mask_count(mh);
 	}
+	mlen = warp_sum_i32(mlen), blen = warp_sum_i32(blen), aplen = warp_sum_i32(aplen), l = warp_sum_i32(l);
+	if (lane == 0) {
+		gc->has_cigar = 1;
+		gc->n_cigar = n_out;
+		gc->c_ss = (int32_t)gt.a[off_a0].x + 1 - (int32_t)(gt.a[off_a0].y >> 32 & 0xff);
+		gc->c_ee = (int32_t)gt.a[off_a0 + gc->n_anchor - 1].x + 1;
+		gc->c_mlen = mlen, gc->c_blen = blen, gc->c_aplen = aplen;
+	}
+	if (!(l == gc->qe - gc->qs && aplen == gc->pe - gc->ps)) return MGB_E_INTERNAL;
+	warp_sync();
+	*ops = O;
 	return 0;
 }
 
-// ---- ds:Z difference string ----
-
-struct DsOut { char *ds; int32_t len; int32_t *off; int32_t n_off; };
+// ---- ds:Z difference string (reference: galign.c:182-293 mg_gchain_gen_ds) ----
 
 MG_HD inline char ds_nt(const char *s, int64_t i) { return "acgtn"[nt4((uint8_t)s[i])]; }
+MG_HD inline int32_t ds_ndig(uint32_t x) { int32_t n = 1; while (x >= 10) x /= 10, ++n; return n; }
+MG_HD inline void ds_put_int(char *w, uint32_t x, int32_t n) { for (int32_t k = n - 1; k >= 0; --k) w[k] = (char)('0' + x % 10), x /= 10; }
 
-// ---- raw writers for the chunked ds generation: the caller has sized the buffers from per-operation upper bounds ----
-MG_HD inline char *ds_w_int(char *w, int32_t c)
+// The text of one alignment match of len bases at t[] on the walk and q[] on the read (reference: galign.c:234-254), at w[]
+// with its offsets, which count from b0, at off[]; w == 0: only counted.  Returns the bytes, *n_off the offsets.
+MG_HD inline int32_t ds_match(char *w, int32_t *off, int32_t b0, int32_t op, int32_t len, const char *t, const char *q, int32_t *n_off)
 {
-	char buf[16];
-	int l = 0;
-	uint32_t x = c >= 0? (uint32_t)c : (uint32_t)(-c);
-	do { buf[l++] = (char)(x % 10 + '0'); x /= 10; } while (x > 0);
-	if (c < 0) buf[l++] = '-';
-	for (int i = l - 1; i >= 0; --i) *w++ = buf[i];
-	return w;
+	int32_t nb = 0, no = 0, l = 0, z = 0;
+	if (op == 7) l = len, z = len; // '=' runs hold identical characters: nothing to look at
+	for (; z < len; ++z) {
+		const int cx = nt4((uint8_t)t[z]), cy = nt4((uint8_t)q[z]);
+		if (cx != cy) {
+			if (l > 0) {
+				const int32_t d = ds_ndig((uint32_t)l);
+				if (w) off[no] = b0 + nb, w[nb] = ':', ds_put_int(w + nb + 1, (uint32_t)l, d);
+				++no, nb += 1 + d;
+			}
+			if (w) off[no] = b0 + nb, w[nb] = '*', w[nb + 1] = "acgtn"[cx], w[nb + 2] = "acgtn"[cy];
+			++no, nb += 3, l = 0;
+		} else ++l;
+	}
+	if (l > 0) {
+		const int32_t d = ds_ndig((uint32_t)l);
+		if (w) off[no] = b0 + nb, w[nb] = ':', ds_put_int(w + nb + 1, (uint32_t)l, d);
+		++no, nb += 1 + d;
+	}
+	*n_off = no;
+	return nb;
 }
 
-// reference: galign.c:153-180 write_indel
-MG_HD inline char *ds_w_indel(char *w, int64_t len, const char *seq, int64_t ll, int64_t lr)
+// How far an indel of len bases at s[p] repeats into its flanks inside [lo, hi): ll bases to its right, lr to its left
+// (reference: galign.c:256-264 and 270-278).  One lane, and the same with the whole warp testing MGB_W positions at a time.
+MG_HD inline void ds_flanks(const char *s, int32_t p, int32_t len, int32_t lo, int32_t hi, int32_t *ll, int32_t *lr)
 {
-	int64_t i;
-	if (ll + lr >= len) {
-		*w++ = '[';
-		for (i = 0; i < len; ++i) *w++ = ds_nt(seq, i);
-		*w++ = ']';
-	} else {
-		int64_t k = 0;
-		if (ll > 0) {
-			*w++ = '[';
-			for (i = 0; i < ll; ++i) *w++ = ds_nt(seq, k + i);
-			*w++ = ']';
-			k += ll;
-		}
-		for (i = 0; i < len - lr - ll; ++i) *w++ = ds_nt(seq, k + i);
-		k += len - lr - ll;
-		if (lr > 0) {
-			*w++ = '[';
-			for (i = 0; i < lr; ++i) *w++ = ds_nt(seq, k + i);
-			*w++ = ']';
-		}
+	int32_t z;
+	for (z = 1; z <= len; ++z)
+		if (p - z < lo || s[p + len - z] != s[p - z]) break;
+	*lr = z - 1;
+	for (z = 0; z < len; ++z)
+		if (p + len + z >= hi || s[p + len + z] != s[p + z]) break;
+	*ll = z;
+}
+MG_HD inline void ds_flanks_w(const char *s, int32_t p, int32_t len, int32_t lo, int32_t hi, int32_t *ll, int32_t *lr, int lane)
+{
+	*lr = *ll = len;
+	for (int32_t z0 = 1; z0 <= len; z0 += MGB_W) {
+		const int32_t z = z0 + lane;
+		const uint32_t m = warp_ballot(z <= len && (p - z < lo || s[p + len - z] != s[p - z]));
+		if (m) { *lr = z0 + mask_lowest(m) - 1; break; }
 	}
-	return w;
+	for (int32_t z0 = 0; z0 < len; z0 += MGB_W) {
+		const int32_t z = z0 + lane;
+		const uint32_t m = warp_ballot(z < len && (p + len + z >= hi || s[p + len + z] != s[p + z]));
+		if (m) { *ll = z0 + mask_lowest(m); break; }
+	}
 }
 
-static const int DS_CHUNKS = 32;
-struct DsChunk { int64_t dx, dy; int32_t cap_b, cap_o, n_b, n_o; };
-
-// The ds:Z string of every chain (reference: galign.c:182-262 mg_gchain_gen_ds).  What one CIGAR operation contributes
-// depends only on the operation and on where it starts on the walk and on the read, so the operations are cut into
-// DS_CHUNKS runs that are written independently (by different lanes on the device) and then joined in order.
-// Warp-uniform: all lanes enter; out[] is filled identically on every lane.
-MG_HD inline int gchain_ds_w(Arena &A, const GraphDev &g, const char *qseq, GcSet &gt, const CigarOut *cg, DsOut *out, int lane)
+// The text of an indel (reference: galign.c:153-180 write_indel): its sign, then its bases, those that repeat in the flanks (ll
+// on the left, lr on the right) in brackets, all of them when ll + lr >= len.  Its length, and its byte r.
+MG_HD inline int32_t ds_indel_bytes(int32_t len, int32_t ll, int32_t lr) { return 1 + (ll + lr >= len? len + 2 : len + (ll > 0? 2 : 0) + (lr > 0? 2 : 0)); }
+MG_HD inline char ds_indel_char(int32_t r, int32_t op, int32_t len, const char *s, int32_t ll, int32_t lr)
 {
-	for (int32_t i = 0; i < gt.n_gc; ++i) {
-		GChain *gc = &gt.gc[i];
-		const uint64_t *cigar = cg[i].cigar;
-		const int32_t n_cigar = gc->n_cigar, aplen = gc->c_aplen;
-		char *seq;
-		int64_t seq_l = 0;
-		MGB_ALLOC(A, seq, char, aplen + 1);
-		for (int32_t j = 0; j < gc->cnt; ++j) { // the aligned part of the walk
-			const int32_t k = gc->off + j;
-			const uint32_t v = gt.lc[k].v;
-			const int32_t slen = g_vlen(g, v);
-			const int32_t st = j > 0? 0 : gc->c_ss;
-			const int32_t en = j < gc->cnt - 1? slen : gc->c_ee;
-			if (seq_l + (en - st) > aplen) return MGB_E_INTERNAL;
-			const char *s = g_vseq(g, v) + st;
-			for (int32_t t = lane; t < en - st; t += MGB_W) seq[seq_l + t] = s[t];
-			seq_l += en - st;
+	if (r == 0) return op == 1? '+' : '-';
+	r -= 1;
+	if (ll + lr >= len) return r == 0? '[' : r == len + 1? ']' : ds_nt(s, r - 1);
+	const int32_t a = ll > 0? ll + 2 : 0;
+	if (r < a) return r == 0? '[' : r == a - 1? ']' : ds_nt(s, r - 1);
+	r -= a;
+	if (r < len - ll - lr) return ds_nt(s, ll + r);
+	r -= len - ll - lr;
+	return r == 0? '[' : r == lr + 1? ']' : ds_nt(s, len - lr + r - 1);
+}
+
+static const int32_t DS_LONG_INDEL = 32; // an indel this long or longer is taken by the whole warp: its text and its flank scans grow with its length
+
+// One pass of the ds:Z string of a chain over its n_cigar merged operations ops[], MGB_W at a time, lane l on operation base+l.
+// What an operation writes depends only on its kind and length, on where it starts on the walk (x, in seq[0, aplen)) and on
+// the read (y, in qseq[qs, qe)) and on the two sequences: a scan of the operations' advances gives every one its x and y, a scan
+// of their sizes places their text.  Indels of DS_LONG_INDEL bases or more are taken by the whole warp, one after the other.
+//   sizing (WRITE false): at[j] = number of offsets << 32 | bytes in front of operation j; *ds_len and *n_off the totals;
+//   writing (WRITE true): the CIGAR to dc[], the text to ds[] and its offsets to dof[], each operation where the sizing pass
+//   placed it.
+// Warp-uniform.
+template<bool WRITE>
+MG_HD inline void gchain_ds_pass_w(const uint64_t *ops, int32_t n_cigar, uint64_t *at, const char *seq, int32_t aplen, const char *qseq, int32_t qs, int32_t qe,
+                                   uint64_t *dc, char *ds, int32_t *dof, int32_t *ds_len, int32_t *n_off, int lane)
+{
+	int32_t x0 = 0, y0 = qs, b_tot = 0, o_tot = 0;
+	for (int32_t base = 0; base < n_cigar; base += MGB_W) {
+		const int32_t j = base + lane;
+		int32_t op = -1, len = 0;
+		if (j < n_cigar) {
+			const uint64_t v = ops[j];
+			op = (int32_t)(v & 0xf), len = (int32_t)(v >> 4);
+			if (WRITE) dc[j] = v;
 		}
-		if (seq_l != aplen) return MGB_E_INTERNAL;
-		DsChunk *ch;
-		MGB_ALLOC(A, ch, DsChunk, DS_CHUNKS);
-		const int32_t per = (n_cigar + DS_CHUNKS - 1) / DS_CHUNKS;
-		// pass 0: how far each run advances, and how much it can write at most
-		for (int c = lane; c < DS_CHUNKS; c += MGB_W) {
-			const int32_t j0 = c * per < n_cigar? c * per : n_cigar, j1 = j0 + per < n_cigar? j0 + per : n_cigar;
-			DsChunk d;
-			d.dx = d.dy = 0, d.cap_b = d.cap_o = d.n_b = d.n_o = 0;
-			for (int32_t j = j0; j < j1; ++j) {
-				const int64_t op = (int64_t)(cigar[j] & 0xf), len = (int64_t)(cigar[j] >> 4);
-				if (op == 7) d.dx += len, d.dy += len, d.cap_b += 12, d.cap_o += 1;
-				else if (op == 0 || op == 8) d.dx += len, d.dy += len, d.cap_b += (int32_t)(14 * len + 12), d.cap_o += (int32_t)(2 * len + 1);
-				else if (op == 1) d.dy += len, d.cap_b += (int32_t)(len + 6), d.cap_o += 1;
-				else if (op == 2) d.dx += len, d.cap_b += (int32_t)(len + 6), d.cap_o += 1;
-			}
-			ch[c] = d;
+		const int match = op == 0 || op == 7 || op == 8, indel = op == 1 || op == 2;
+		const int32_t dx = match || op == 2? len : 0, dy = match || op == 1? len : 0;
+		const int32_t ix = warp_incl_scan_i32(dx, lane), iy = warp_incl_scan_i32(dy, lane);
+		const int32_t x = x0 + ix - dx, y = y0 + iy - dy;
+		x0 += warp_bcast_i32(ix, MGB_W - 1), y0 += warp_bcast_i32(iy, MGB_W - 1);
+		const char *s = op == 1? qseq : seq;
+		const int32_t p = op == 1? y : x, lo = op == 1? qs : 0, hi = op == 1? qe : aplen;
+		const int is_long = indel && len >= DS_LONG_INDEL;
+		const uint32_t m_long = warp_ballot(is_long);
+		int32_t ll = 0, lr = 0;
+		for (uint32_t m = m_long; m; m &= m - 1) {
+			const int src = mask_lowest(m);
+			const int32_t sop = warp_bcast_i32(op, src), slen = warp_bcast_i32(len, src), sp = warp_bcast_i32(p, src);
+			int32_t a, b;
+			ds_flanks_w(sop == 1? qseq : seq, sp, slen, sop == 1? qs : 0, sop == 1? qe : aplen, &a, &b, lane);
+			if (lane == src) ll = a, lr = b;
 		}
-		warp_sync();
-		int64_t tot_cb = 0, tot_co = 0;
-		for (int c = 0; c < DS_CHUNKS; ++c) tot_cb += ch[c].cap_b, tot_co += ch[c].cap_o;
-		char *tmp_b;
-		int32_t *tmp_o;
-		MGB_ALLOC(A, tmp_b, char, tot_cb);
-		MGB_ALLOC(A, tmp_o, int32_t, tot_co);
-		// pass 1: every run writes its text and its (run-relative) offsets
-		int bad = 0;
-		for (int c = lane; c < DS_CHUNKS; c += MGB_W) {
-			const int32_t j0 = c * per < n_cigar? c * per : n_cigar, j1 = j0 + per < n_cigar? j0 + per : n_cigar;
-			int64_t x = 0, y = gc->qs, cb = 0, co = 0;
-			for (int q = 0; q < c; ++q) x += ch[q].dx, y += ch[q].dy, cb += ch[q].cap_b, co += ch[q].cap_o;
-			char *const w0 = tmp_b + cb;
-			char *w = w0;
-			int32_t *const o0 = tmp_o + co;
-			int32_t *o = o0;
-			for (int32_t j = j0; j < j1; ++j) {
-				const int64_t op = (int64_t)(cigar[j] & 0xf), len = (int64_t)(cigar[j] >> 4);
-				if (op == 0 || op == 7 || op == 8) {
-					int64_t z;
-					int32_t l = 0;
-					if (op == 7) l = (int32_t)len, z = len; // '=' runs hold identical characters: nothing to look at
-					else z = 0;
-					for (; z < len; ++z) {
-						const uint8_t cx = (uint8_t)nt4((uint8_t)seq[x + z]);
-						const uint8_t cy = (uint8_t)nt4((uint8_t)qseq[y + z]);
-						if (cx != cy) {
-							if (l > 0) { *o++ = (int32_t)(w - w0); *w++ = ':'; w = ds_w_int(w, l); }
-							*o++ = (int32_t)(w - w0);
-							*w++ = '*', *w++ = "acgtn"[cx], *w++ = "acgtn"[cy];
-							l = 0;
-						} else ++l;
-					}
-					if (l > 0) { *o++ = (int32_t)(w - w0); *w++ = ':'; w = ds_w_int(w, l); }
-					x += len, y += len;
-				} else if (op == 1) {
-					int64_t z, ll, lr;
-					for (z = 1; z <= len; ++z)
-						if (y - z < gc->qs || qseq[y + len - z] != qseq[y - z]) break;
-					lr = z - 1;
-					for (z = 0; z < len; ++z)
-						if (y + len + z >= gc->qe || qseq[y + len + z] != qseq[y + z]) break;
-					ll = z;
-					*o++ = (int32_t)(w - w0);
-					*w++ = '+';
-					w = ds_w_indel(w, len, &qseq[y], ll, lr);
-					y += len;
-				} else if (op == 2) {
-					int64_t z, ll, lr;
-					for (z = 1; z <= len; ++z)
-						if (x - z < 0 || seq[x + len - z] != seq[x - z]) break;
-					lr = z - 1;
-					for (z = 0; z < len; ++z)
-						if (x + len + z >= aplen || seq[x + z] != seq[x + len + z]) break;
-					ll = z;
-					*o++ = (int32_t)(w - w0);
-					*w++ = '-';
-					w = ds_w_indel(w, len, &seq[x], ll, lr);
-					x += len;
-				}
-			}
-			ch[c].n_b = (int32_t)(w - w0), ch[c].n_o = (int32_t)(o - o0);
-			if (ch[c].n_b > ch[c].cap_b || ch[c].n_o > ch[c].cap_o) bad = 1; // cannot happen: the bounds are per operation
+		if (indel && !is_long) ds_flanks(s, p, len, lo, hi, &ll, &lr);
+		int32_t b0, o0;
+		if (!WRITE) {
+			int32_t nb = 0, no = 0;
+			if (indel) nb = ds_indel_bytes(len, ll, lr), no = 1;
+			else if (match) nb = ds_match(0, 0, 0, op, len, seq + x, qseq + y, &no);
+			const int32_t ib = warp_incl_scan_i32(nb, lane), io = warp_incl_scan_i32(no, lane);
+			b0 = b_tot + ib - nb, o0 = o_tot + io - no;
+			if (j < n_cigar) at[j] = (uint64_t)(uint32_t)o0 << 32 | (uint32_t)b0;
+			b_tot += warp_bcast_i32(ib, MGB_W - 1), o_tot += warp_bcast_i32(io, MGB_W - 1);
+			continue;
 		}
-		if (warp_any(bad)) return MGB_E_INTERNAL;
-		warp_sync();
-		// join
-		int64_t tot_b = 0, tot_o = 0;
-		for (int c = 0; c < DS_CHUNKS; ++c) tot_b += ch[c].n_b, tot_o += ch[c].n_o;
-		char *str;
-		int32_t *off;
-		MGB_ALLOC(A, str, char, tot_b + 1);
-		MGB_ALLOC(A, off, int32_t, tot_o);
-		{
-			int64_t cb = 0, co = 0, ab = 0, ao = 0;
-			for (int c = 0; c < DS_CHUNKS; ++c) {
-				const char *sb = tmp_b + cb;
-				const int32_t *so = tmp_o + co;
-				for (int32_t t = lane; t < ch[c].n_b; t += MGB_W) str[ab + t] = sb[t];
-				for (int32_t t = lane; t < ch[c].n_o; t += MGB_W) off[ao + t] = so[t] + (int32_t)ab;
-				cb += ch[c].cap_b, co += ch[c].cap_o, ab += ch[c].n_b, ao += ch[c].n_o;
-			}
+		b0 = o0 = 0;
+		if (j < n_cigar) { const uint64_t v = at[j]; b0 = (int32_t)(uint32_t)v, o0 = (int32_t)(v >> 32); }
+		if (indel && !is_long) {
+			const int32_t nb = ds_indel_bytes(len, ll, lr);
+			dof[o0] = b0;
+			for (int32_t r = 0; r < nb; ++r) ds[b0 + r] = ds_indel_char(r, op, len, s + p, ll, lr);
+		} else if (match) {
+			int32_t no;
+			ds_match(ds + b0, dof + o0, b0, op, len, seq + x, qseq + y, &no);
 		}
-		warp_sync();
-		out[i].ds = str, out[i].len = (int32_t)tot_b, out[i].off = off, out[i].n_off = (int32_t)tot_o;
-		if (lane == 0) gc->ds_len = (int32_t)tot_b, gc->n_dsoff = (int32_t)tot_o;
+		for (uint32_t m = m_long; m; m &= m - 1) {
+			const int src = mask_lowest(m);
+			const int32_t sop = warp_bcast_i32(op, src), slen = warp_bcast_i32(len, src), sp = warp_bcast_i32(p, src), sb0 = warp_bcast_i32(b0, src);
+			const int32_t sll = warp_bcast_i32(ll, src), slr = warp_bcast_i32(lr, src);
+			const char *ss = (sop == 1? qseq : seq) + sp;
+			const int32_t nb = ds_indel_bytes(slen, sll, slr);
+			for (int32_t r = lane; r < nb; r += MGB_W) ds[sb0 + r] = ds_indel_char(r, sop, slen, ss, sll, slr);
+			if (lane == src) dof[o0] = b0;
+		}
 	}
-	return 0;
+	*ds_len = b_tot, *n_off = o_tot;
 }
 
 // per-read result header, one per read, in an array parallel to ReadMeta
@@ -844,8 +812,12 @@ MG_HD inline int stage_gchain_gen(const PipeCtx &c, ReadOut *routs, int rid, Are
 	return 0;
 }
 
-// K8b for one read: stitch CIGARs, ds strings, part 2 of the result (one lane).
-// Warp-uniform: all lanes enter.  The CIGAR stitching runs on lane 0, the ds strings and the copies on all lanes.
+// What K8b keeps of a chain between its passes, in the worker's arena: the merged CIGAR, where the ds:Z text of each of its
+// operations goes (gchain_ds_pass_w) and the aligned part of the walk.
+struct FinChain { uint64_t *ops, *at; char *seq; };
+
+// K8b for one read: stitch the CIGARs, size the ds:Z strings, take part 2 of the result from the pool in one piece and write
+// every chain's CIGAR, ds text and ds offsets straight to their place in it.  Warp-uniform: all lanes enter.
 MG_HD inline int stage_finish(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, int lane)
 {
 	ReadMeta &m = c.meta[rid];
@@ -853,6 +825,7 @@ MG_HD inline int stage_finish(const PipeCtx &c, ReadOut *routs, int rid, Arena &
 	if (m.status != 0) { if (lane == 0) ro.status = m.status; return 0; }
 	if (!(c.opt.flag & F_CIGAR) || ro.n_gc == 0 || batch_n_seg(c.b, rid) != 1) return 0;
 	uint64_t mark = A.top;
+	const GraphDev &g = c.g;
 	const char *qseq = c.b.seq + c.b.seq_off[rid];
 	char *blob = c.out + ro.blob_off;
 	GcSet gs;
@@ -860,37 +833,60 @@ MG_HD inline int stage_finish(const PipeCtx &c, ReadOut *routs, int rid, Arena &
 	gs.gc = (GChain*)blob;
 	gs.lc = (LLChain*)(blob + align8((uint64_t)gs.n_gc * sizeof(GChain)));
 	gs.a = (u128*)((char*)gs.lc + align8((uint64_t)gs.n_lc * sizeof(LLChain)));
-	CigarOut *cg;
-	DsOut *ds;
-	MGB_ALLOC(A, cg, CigarOut, gs.n_gc);
-	MGB_ALLOC(A, ds, DsOut, gs.n_gc);
+	FinChain *fc;
+	MGB_ALLOC(A, fc, FinChain, gs.n_gc);
 	unsigned long long pt0 = prof_clock();
-	MGB_TRY(gchain_cigar_finish_w(A, c, gs, cg, lane));
+	for (int32_t i = 0; i < gs.n_gc; ++i) {
+		uint64_t *ops;
+		MGB_TRY(gchain_cigar_finish_w(A, c, gs, i, &ops, lane));
+		if (lane == 0) fc[i].ops = ops;
+	}
 	unsigned long long pt1 = prof_clock();
-	MGB_TRY(gchain_ds_w(A, c.g, qseq, gs, cg, ds, lane));
-	if (lane == 0) prof_add(c, PROF_FIN_CIGAR_CYC, pt1 - pt0), prof_add(c, PROF_FIN_DS_CYC, prof_clock() - pt1);
 	uint64_t sz = 0;
-	for (int32_t i = 0; i < gs.n_gc; ++i)
-		sz += align8((uint64_t)cg[i].n * 8) + align8((uint64_t)ds[i].len + 1) + align8((uint64_t)ds[i].n_off * 4);
+	for (int32_t i = 0; i < gs.n_gc; ++i) { // sizing pass
+		GChain *gc = &gs.gc[i];
+		const int32_t aplen = gc->c_aplen, n_cigar = gc->n_cigar;
+		char *seq;
+		uint64_t *at;
+		MGB_ALLOC(A, seq, char, aplen + 1);
+		MGB_ALLOC(A, at, uint64_t, n_cigar);
+		int64_t seq_l = 0;
+		for (int32_t j = 0; j < gc->cnt; ++j) { // the aligned part of the walk (reference: galign.c:197-207)
+			const uint32_t v = gs.lc[gc->off + j].v;
+			const int32_t st = j > 0? 0 : gc->c_ss;
+			const int32_t en = j < gc->cnt - 1? g_vlen(g, v) : gc->c_ee;
+			if (seq_l + (en - st) > aplen) return MGB_E_INTERNAL;
+			const char *s = g_vseq(g, v) + st;
+			for (int32_t t = lane; t < en - st; t += MGB_W) seq[seq_l + t] = s[t];
+			seq_l += en - st;
+		}
+		if (seq_l != aplen) return MGB_E_INTERNAL;
+		warp_sync();
+		int32_t ds_len, n_off;
+		gchain_ds_pass_w<false>(fc[i].ops, n_cigar, at, seq, aplen, qseq, gc->qs, gc->qe, 0, 0, 0, &ds_len, &n_off, lane);
+		sz += align8((uint64_t)n_cigar * 8) + align8((uint64_t)ds_len + 1) + align8((uint64_t)n_off * 4);
+		warp_sync();
+		if (lane == 0) fc[i].at = at, fc[i].seq = seq, gc->ds_len = ds_len, gc->n_dsoff = n_off;
+	}
 	int64_t boff = 0;
 	if (lane == 0) boff = pool_alloc(c.pool_out, sz);
 	boff = (int64_t)warp_bcast_u64((uint64_t)boff, 0);
 	if (boff < 0) return MGB_E_POOL;
+	warp_sync();
 	uint64_t at = (uint64_t)boff;
-	for (int32_t i = 0; i < gs.n_gc; ++i) {
+	for (int32_t i = 0; i < gs.n_gc; ++i) { // writing pass
 		GChain *gc = &gs.gc[i];
-		const int64_t cigar_off = (int64_t)at; at += align8((uint64_t)cg[i].n * 8);
-		const int64_t ds_off = (int64_t)at; at += align8((uint64_t)ds[i].len + 1);
-		const int64_t dsoff_off = (int64_t)at; at += align8((uint64_t)ds[i].n_off * 4);
-		if (lane == 0) gc->cigar_off = cigar_off, gc->ds_off = ds_off, gc->dsoff_off = dsoff_off;
-		uint64_t *dc = (uint64_t*)(c.out + cigar_off);
-		for (int32_t k = lane; k < cg[i].n; k += MGB_W) dc[k] = cg[i].cigar[k];
+		const int32_t n_cigar = gc->n_cigar, ds_len = gc->ds_len, n_off = gc->n_dsoff;
+		const int64_t cigar_off = (int64_t)at; at += align8((uint64_t)n_cigar * 8);
+		const int64_t ds_off = (int64_t)at; at += align8((uint64_t)ds_len + 1);
+		const int64_t dsoff_off = (int64_t)at; at += align8((uint64_t)n_off * 4);
 		char *dd = c.out + ds_off;
-		for (int32_t k = lane; k < ds[i].len; k += MGB_W) dd[k] = ds[i].ds[k];
-		if (lane == 0) dd[ds[i].len] = 0;
-		int32_t *dof = (int32_t*)(c.out + dsoff_off);
-		for (int32_t k = lane; k < ds[i].n_off; k += MGB_W) dof[k] = ds[i].off[k];
+		int32_t wl, wo;
+		gchain_ds_pass_w<true>(fc[i].ops, n_cigar, fc[i].at, fc[i].seq, gc->c_aplen, qseq, gc->qs, gc->qe, (uint64_t*)(c.out + cigar_off), dd, (int32_t*)(c.out + dsoff_off), &wl, &wo, lane);
+		warp_sync();
+		if (lane == 0) gc->cigar_off = cigar_off, gc->ds_off = ds_off, gc->dsoff_off = dsoff_off, dd[ds_len] = 0;
 	}
+	if (lane == 0) prof_add(c, PROF_FIN_CIGAR_CYC, pt1 - pt0), prof_add(c, PROF_FIN_DS_CYC, prof_clock() - pt1);
 	if (lane == 0) ro.blob2_off = boff, ro.blob2_size = (uint32_t)sz;
 	A.top = mark;
 	return 0;
