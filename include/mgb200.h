@@ -298,6 +298,28 @@ typedef struct {
 int mgb_test_lchain(int mode, int n, const mg128_t *a, const int64_t *off, const int32_t *cnt, const mgb_lchain_opt_t *opt, int32_t *out,
 					uint64_t *u, mg128_t *a_out);
 
+/* test hook: the (w,k)-minimizers (sketch.c mg_sketch) of n sequences seq[off[i]..+len[i]) (bytes, not strings: 0..3 are bases),
+ * sequence i with rid i, on a warp launched as the seeding kernel is.  mode 0: the sketch of the seeding kernel, cut into chunks
+ * over the lanes where it can be, the window rings in the warp's slice of shared memory and, for a sequence that is all A/C/G/T,
+ * the bases read from the 2-bit words of the batch upload; mode 1: the sequential sketch of the index build, on lane 0.
+ * out[3i..3i+2] = rc, n, path (mode 0: MGB_SKETCH_PATH_*; mode 1: -1); the list goes to mz[mz_off[i]..+n) if it fits before
+ * mz_off[i+1].  Returns 0, or a negative code (nothing run) for bad k, w, mode or an empty sequence. */
+#define MGB_SKETCH_PATH_SMEM_PK 0 /* chunks, rings in shared memory, 2-bit words */
+#define MGB_SKETCH_PATH_SMEM 1    /* chunks, rings in shared memory, ASCII */
+#define MGB_SKETCH_PATH_ARENA 2   /* chunks, rings in the worker arena (w > 12) */
+#define MGB_SKETCH_PATH_SEQ 3     /* the sequential scan on lane 0 */
+int mgb_test_sketch(int k, int w, int n, const char *seq, const int64_t *off, const int32_t *len, int mode, int32_t *out, mg128_t *mz, const int64_t *mz_off);
+
+/* test hook: the seeding stage itself (minimizers, index lookup with the occurrence filter, seed expansion, seed sort or the heap
+ * merge of MG_M_HEAP_SORT) on n reads with the graph and index of gi and the options flag, occ_max1 and max_qlen, the batch
+ * packed as mg_map_batch packs it.  seg_off == NULL: single-segment reads; otherwise read i is the concatenation of the
+ * non-empty segments seg_len[seg_off[i]..seg_off[i+1]) (qlens[i] their sum).  names (may be NULL) decide MG_M_NO_DIAG.
+ * out[5i..5i+4] = status (0; 1: not mapped, empty or longer than max_qlen; < 0: error), n_mz, rep_len, n_a, n_mp; the seeds of
+ * the reads with status 0 follow each other in a[] in read order, as the stage leaves them, and so do their mini_pos.  Returns 0,
+ * MGB_E_POOL when they do not fit a_cap / mp_cap (out[] is filled), or a negative code (nothing run) for bad reads. */
+int mgb_test_seed(const mg_idx_t *gi, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off, const int32_t *seg_len,
+				  const char *const *names, uint64_t flag, int occ_max1, int max_qlen, int32_t *out, mg128_t *a, int64_t a_cap, int32_t *mini_pos, int64_t mp_cap);
+
 const char *mgb_last_error(void);
 void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st);
 /* knobs: "arena_mb" (per worker), "workers_per_sm", "device"; returns 0 if the key is known */

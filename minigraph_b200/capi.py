@@ -110,6 +110,8 @@ WFA_TIER2_CONT = 4
 # mgb_test_lchain(): modes (k_chain DP, k_chain RMQ, k_chain_rescue) and fill paths (mgb200.h)
 LCHAIN_DP, LCHAIN_RMQ, LCHAIN_RESCUE = 0, 1, 2
 LCHAIN_PATH_DP, LCHAIN_PATH_RMQ_W, LCHAIN_PATH_RMQ_TIE, LCHAIN_PATH_RMQ_CAP = 0, 1, 2, 3
+# mgb_test_sketch(): the ways the seeding kernel's sketch makes a list (mgb200.h MGB_SKETCH_PATH_*)
+SKETCH_PATH_SMEM_PK, SKETCH_PATH_SMEM, SKETCH_PATH_ARENA, SKETCH_PATH_SEQ = 0, 1, 2, 3
 
 
 class mgb_lchain_opt_t(C.Structure):
@@ -197,6 +199,11 @@ def bind_engine_api(lib):
     lib.mgb_test_radix128.argtypes = [C.POINTER(mg128_t), C.c_int64, C.c_int, C.c_int]
     lib.mgb_test_lchain.restype = C.c_int
     lib.mgb_test_lchain.argtypes = [C.c_int, C.c_int, C.POINTER(mg128_t), i64p, i32p, C.POINTER(mgb_lchain_opt_t), i32p, C.POINTER(C.c_uint64), C.POINTER(mg128_t)]
+    lib.mgb_test_sketch.restype = C.c_int
+    lib.mgb_test_sketch.argtypes = [C.c_int, C.c_int, C.c_int, C.c_char_p, i64p, i32p, C.c_int, i32p, C.POINTER(mg128_t), i64p]
+    lib.mgb_test_seed.restype = C.c_int
+    lib.mgb_test_seed.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_char_p), i32p, i32p, C.POINTER(C.c_char_p),
+                                  C.c_uint64, C.c_int, C.c_int, i32p, C.POINTER(mg128_t), C.c_int64, i32p, C.c_int64]
     lib.mg_map_batch_frag.restype = C.c_int
     lib.mg_map_batch_frag.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
                                       C.POINTER(C.POINTER(mg_gchains_t)), C.POINTER(mg_mapopt_t)]

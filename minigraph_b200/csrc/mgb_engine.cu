@@ -1498,6 +1498,15 @@ static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int
 	return 0;
 }
 
+// MG_M_NO_DIAG: which segment name, if any, is each read's own (BatchDev::self_id; exact string match on the host)
+static std::vector<int32_t> read_self_ids(const Model *M, int n_reads, const char *const *names)
+{
+	std::vector<int32_t> self((size_t)n_reads, -1);
+	for (int i = 0; i < n_reads; ++i)
+		if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[(size_t)i] = it->second; }
+	return self;
+}
+
 // Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).  With gaf, the result is the batch's GAF text
 // (gaf_text) instead of mg_gchains_t objects.
 static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
@@ -1638,10 +1647,8 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	}
 	tm_h2d.stop();
 	const bool no_diag = (o.flag & F_NO_DIAG) != 0;
-	if (no_diag) { // which segment name, if any, is the read's own (exact string match on the host)
-		std::vector<int32_t> self((size_t)n_reads, -1);
-		for (int i = 0; i < n_reads; ++i)
-			if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[(size_t)i] = it->second; }
+	if (no_diag) {
+		const std::vector<int32_t> self = read_self_ids(M, n_reads, names);
 		h2d(d_self_id, self.data(), sizeof(int32_t) * (size_t)n_reads);
 	}
 	int32_t *d_seg_off = 0, *d_seg_len = 0; // multi-segment fragments only (mg_map_frag with n_segs > 1)
@@ -2646,6 +2653,201 @@ extern "C" int mgb_test_lchain(int mode, int n, const mg128_t *a, const int64_t 
 							   uint64_t *u, mg128_t *a_out)
 {
 	try { return test_lchain_impl(mode, n, (const u128*)a, off, cnt, opt, out, u, (u128*)a_out); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: the minimizer sketch of n sequences, launched as k_seed is (test_launch).  mode 0: sketch_seq_w() on the warp, the
+// window rings in the warp's slice and, for a sequence that is all A/C/G/T, the 2-bit words of the host packer of the batch upload
+// (stage_seed); mode 1: sketch_seq() on lane 0 (k_index_sketch).  Sequence i is sketched with rid i.
+// ---------------------------------------------------------------------------------------------------------------
+struct TestSketch {
+	int k, w, mode;
+	const char *seq;
+	const int64_t *off, *pk_off, *mz_off; // pk_off[i] < 0: sequence i has other letters and no 2-bit words
+	const int32_t *len;
+	const uint64_t *pk;
+	int32_t *out;         // per sequence: rc, n, path
+	u128 *mz;             // list i at mz[mz_off[i]..mz_off[i+1])
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
+	{
+		A.top = 0;
+		AVec<u128> mv;
+		avec_init(mv);
+		const char *s = seq + off[i];
+		int rc = 0, path = -1;
+		if (mode == 0) rc = sketch_seq_w(A, s, len[i], w, k, (uint32_t)i, mv, lane, (u128*)smem, pk_off[i] >= 0? pk + pk_off[i] : 0, &path);
+		else if (lane == 0) rc = sketch_seq(A, s, len[i], w, k, (uint32_t)i, mv); // the list is lane 0's alone
+		rc = warp_bcast_i32(rc, 0);
+		const int64_t n = rc == 0? (int64_t)warp_bcast_u64((uint64_t)mv.n, 0) : 0;
+		if (n <= mz_off[i + 1] - mz_off[i]) {
+			if (mode == 0) for (int64_t j = lane; j < n; j += MGB_W) mz[mz_off[i] + j] = mv.a[j];
+			else if (lane == 0) for (int64_t j = 0; j < n; ++j) mz[mz_off[i] + j] = mv.a[j];
+		}
+		if (lane == 0) out[3 * (int64_t)i] = rc, out[3 * (int64_t)i + 1] = (int32_t)n, out[3 * (int64_t)i + 2] = path;
+		warp_sync();
+		return 0;
+	}
+};
+
+static int test_sketch_impl(int k, int w, int n, const char *seq, const int64_t *off, const int32_t *len, int mode, int32_t *out, u128 *mz, const int64_t *mz_off)
+{
+	static_assert(SKETCH_PATH_SMEM_PK == MGB_SKETCH_PATH_SMEM_PK && SKETCH_PATH_SMEM == MGB_SKETCH_PATH_SMEM && SKETCH_PATH_ARENA == MGB_SKETCH_PATH_ARENA
+				  && SKETCH_PATH_SEQ == MGB_SKETCH_PATH_SEQ, "the sketch paths of mgb200.h are mgb_seed.cuh's");
+	if (k < 1 || k > 28 || w < 1 || w > 255 || (mode != 0 && mode != 1) || n < 0) {
+		set_error("mgb_test_sketch: 1 <= k <= 28, 1 <= w <= 255, mode 0 or 1 and n at least 0");
+		return MGB_E_UNSUPPORTED;
+	}
+	int32_t max_len = 0;
+	for (int i = 0; i < n; ++i) { // the sketch of an empty sequence is not defined (sketch.c:63 asserts)
+		if (len[i] < 1 || off[i] < 0 || mz_off[i] < 0 || mz_off[i + 1] < mz_off[i]) {
+			set_error("mgb_test_sketch: sequence " + std::to_string(i) + " is empty or has a bad offset");
+			return MGB_E_UNSUPPORTED;
+		}
+		max_len = std::max(max_len, len[i]);
+	}
+	if (n == 0) return 0;
+	if (int e = test_no_device()) return e;
+	std::vector<int64_t> pk_off((size_t)n);
+	std::vector<uint64_t> hpk;
+	for (int i = 0; i < n; ++i) { // the words of the batch upload (map_range): one more than the bases need
+		pk_off[(size_t)i] = (int64_t)hpk.size();
+		hpk.resize(hpk.size() + (size_t)(len[i] + 31) / 32 + 1, 0);
+		if (!pack_read(seq + off[i], len[i], hpk.data() + pk_off[(size_t)i])) pk_off[(size_t)i] = -1;
+	}
+	auto seq_d = upload(seq, test_seq_bytes(n, off, len));
+	auto off_d = upload(off, n), pk_off_d = upload(pk_off.data(), n), mz_off_d = upload(mz_off, (size_t)n + 1);
+	auto len_d = upload(len, n);
+	auto pk_d = upload(hpk.data(), hpk.size());
+	DevBuf<int32_t> out_d(3 * (size_t)n);
+	DevBuf<u128> mz_d((size_t)mz_off[n] + 1);
+	TestSketch t;
+	t.k = k, t.w = w, t.mode = mode, t.seq = seq_d, t.off = off_d, t.pk_off = pk_off_d, t.mz_off = mz_off_d, t.len = len_d, t.pk = pk_d;
+	t.out = out_d, t.mz = mz_d;
+	// the chunk lists and rings (about 16 bytes per base and window slot), or the sequential list grown in the arena
+	const uint64_t arena_bytes = (uint64_t)max_len * 256 + ((uint64_t)1 << 20);
+	if (int e = test_launch<S_SEED>(n, std::min(n, 2 * StageSpec<S_SEED>::warps), arena_bytes, t)) return e;
+	d2h(out, out_d, sizeof(int32_t) * 3 * (size_t)n);
+	d2h(mz, mz_d, sizeof(u128) * (size_t)mz_off[n]);
+	return 0;
+}
+
+extern "C" int mgb_test_sketch(int k, int w, int n, const char *seq, const int64_t *off, const int32_t *len, int mode, int32_t *out, mg128_t *mz, const int64_t *mz_off)
+{
+	try { return test_sketch_impl(k, w, n, seq, off, len, mode, out, (u128*)mz, mz_off); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: stage_seed() itself on a batch packed as mg_map_batch packs it (the 2-bit words of every read that is all A/C/G/T;
+// fragments of several segments as ASCII only), with the graph and index of gi and the options flag, occ_max1 and max_qlen,
+// launched as k_seed is (test_launch).  The seeds and mini_pos of each read are read back from the pools.
+// ---------------------------------------------------------------------------------------------------------------
+struct TestSeed {
+	PipeCtx c;
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
+	{
+		A.top = 0;
+		const int rc = stage_seed(c, i, A, lane, smem);
+		if (rc < 0 && lane == 0) c.meta[i].status = rc; // as stage_fail records a failed read
+		warp_sync();
+		return 0;
+	}
+};
+
+static int test_seed_impl(const mg_idx_t *gi, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off, const int32_t *seg_len,
+						  const char *const *names, uint64_t flag, int occ_max1, int max_qlen, int32_t *out, u128 *a, int64_t a_cap, int32_t *mini_pos, int64_t mp_cap)
+{
+	if (gi == 0 || n < 0 || a_cap < 0 || mp_cap < 0) { set_error("mgb_test_seed: an index, n and the capacities at least 0"); return MGB_E_UNSUPPORTED; }
+	for (int i = 0; i < n; ++i) {
+		int64_t sum = 0;
+		if (seg_off) {
+			if (seg_off[i] < 0 || seg_off[i + 1] <= seg_off[i]) { set_error("mgb_test_seed: read " + std::to_string(i) + " has no segment"); return MGB_E_UNSUPPORTED; }
+			for (int32_t j = seg_off[i]; j < seg_off[i + 1]; ++j) {
+				if (seg_len[j] < 1) { set_error("mgb_test_seed: read " + std::to_string(i) + " has an empty segment"); return MGB_E_UNSUPPORTED; } // map-algo.c:34-45 sketches every one
+				sum += seg_len[j];
+			}
+		}
+		if (qlens[i] < 0 || (seg_off && sum != qlens[i]) || (qlens[i] > 0 && seqs[i] == 0)) {
+			set_error("mgb_test_seed: read " + std::to_string(i) + " has a bad length");
+			return MGB_E_UNSUPPORTED;
+		}
+	}
+	if (n == 0) return 0;
+	const Model *M = model_of(gi);
+	if (int e = test_no_device(M->device)) return e;
+	// the batch as map_range lays it out: ASCII with slack, 2-bit words per read (pk_off ~0: the read has other letters)
+	std::vector<uint64_t> seq_off((size_t)n), pk_off((size_t)n), hpk;
+	std::vector<uint32_t> name_hash((size_t)n);
+	uint64_t tot = 0;
+	int64_t n_bases = 0;
+	for (int i = 0; i < n; ++i) {
+		seq_off[(size_t)i] = tot, tot = (tot + (uint64_t)qlens[i] + 8 + 15) & ~(uint64_t)15;
+		name_hash[(size_t)i] = names && names[i]? hash_str(names[i]) : 0;
+		pk_off[(size_t)i] = hpk.size();
+		hpk.resize(hpk.size() + (size_t)(qlens[i] + 31) / 32 + 1, 0);
+		if (qlens[i] > 0 && !pack_read(seqs[i], qlens[i], hpk.data() + pk_off[(size_t)i])) pk_off[(size_t)i] = ~0ULL;
+		n_bases += qlens[i];
+	}
+	std::vector<char> hseq((size_t)tot + 16, 0);
+	for (int i = 0; i < n; ++i) if (qlens[i] > 0) memcpy(hseq.data() + seq_off[(size_t)i], seqs[i], (size_t)qlens[i]);
+	auto seq_d = upload(hseq.data(), hseq.size());
+	auto seq_off_d = upload(seq_off.data(), n), pk_off_d = upload(pk_off.data(), n), pk_d = upload(hpk.data(), hpk.size());
+	auto len_d = upload((const int32_t*)qlens, n);
+	auto hash_d = upload(name_hash.data(), n);
+	const std::vector<int32_t> self = read_self_ids(M, n, names);
+	auto self_d = upload(self.data(), n);
+	const int n_seg_tot = seg_off? seg_off[n] : 0;
+	auto seg_off_d = upload(seg_off? seg_off : (const int32_t*)self.data(), seg_off? (size_t)n + 1 : 0);
+	auto seg_len_d = upload(seg_len? seg_len : (const int32_t*)self.data(), seg_off? (size_t)n_seg_tot : 0);
+	DevBuf<ReadMeta> meta_d((size_t)n);
+	DevBuf<Pool> pools_d(2);
+	TestSeed t;
+	memset(&t.c, 0, sizeof(t.c));
+	t.c.g = M->g, t.c.ix = M->ix;
+	t.c.opt.flag = flag, t.c.opt.occ_max1 = occ_max1, t.c.opt.max_qlen = max_qlen;
+	t.c.b.n_reads = n, t.c.b.seq = seq_d, t.c.b.seq_off = seq_off_d, t.c.b.seq_len = len_d, t.c.b.name_hash = hash_d;
+	t.c.b.self_id = (flag & F_NO_DIAG)? (const int32_t*)self_d : 0;
+	t.c.b.seg_off = seg_off? (const int32_t*)seg_off_d : 0, t.c.b.seg_len = seg_off? (const int32_t*)seg_len_d : 0;
+	t.c.b.pk = seg_off? 0 : (const uint64_t*)pk_d, t.c.b.pk_off = seg_off? 0 : (const uint64_t*)pk_off_d;
+	t.c.meta = meta_d, t.c.pool_anchor = pools_d, t.c.pool_minipos = pools_d + 1;
+	// pools as map_range sizes them at first, doubled while a read runs out of them (the batch's retry)
+	uint64_t cap_a = std::max<uint64_t>((uint64_t)n_bases / 4 * sizeof(u128), (uint64_t)1 << 22), cap_mp = std::max<uint64_t>((uint64_t)n_bases * sizeof(int32_t) / 2, (uint64_t)1 << 20);
+	std::vector<ReadMeta> meta((size_t)n);
+	for (;;) {
+		DevBuf<u128> anchor_d(cap_a / sizeof(u128));
+		DevBuf<int32_t> mp_d(cap_mp / sizeof(int32_t));
+		Pool hp[2];
+		hp[0].used = 0, hp[0].cap = cap_a, hp[1].used = 0, hp[1].cap = cap_mp;
+		h2d(pools_d, hp, sizeof(hp));
+		dzero(meta_d, sizeof(ReadMeta) * (size_t)n);
+		t.c.anchor = anchor_d, t.c.minipos = mp_d;
+		// a read's lists in the arena: minimizers and matches (~120 bytes per base at w = 1), the sort's scratch when off chip
+		int32_t max_len = 0;
+		for (int i = 0; i < n; ++i) max_len = std::max(max_len, qlens[i]);
+		const uint64_t arena_bytes = (uint64_t)max_len * 256 + ((uint64_t)16 << 20);
+		if (int e = test_launch<S_SEED>(n, std::min(n, 2 * StageSpec<S_SEED>::warps), arena_bytes, t)) return e;
+		d2h(meta.data(), meta_d, sizeof(ReadMeta) * (size_t)n);
+		bool pool_full = false;
+		for (int i = 0; i < n; ++i) pool_full |= meta[(size_t)i].status == MGB_E_POOL;
+		if (pool_full) { cap_a *= 2, cap_mp *= 2; continue; }
+		int64_t sum_a = 0, sum_mp = 0;
+		for (int i = 0; i < n; ++i) {
+			const ReadMeta &m = meta[(size_t)i];
+			int32_t *o = out + 5 * (int64_t)i;
+			o[0] = m.status, o[1] = m.n_mz, o[2] = m.rep_len, o[3] = m.n_a, o[4] = m.n_mp;
+			if (m.status != 0) continue;
+			if (sum_a + m.n_a <= a_cap) d2h(a + sum_a, (const u128*)anchor_d + m.a_off, sizeof(u128) * (size_t)m.n_a);
+			if (sum_mp + m.n_mp <= mp_cap) d2h(mini_pos + sum_mp, (const int32_t*)mp_d + m.mp_off, sizeof(int32_t) * (size_t)m.n_mp);
+			sum_a += m.n_a, sum_mp += m.n_mp;
+		}
+		if (sum_a > a_cap || sum_mp > mp_cap) { set_error("mgb_test_seed: the seeds or mini_pos do not fit a_cap / mp_cap"); return MGB_E_POOL; }
+		return 0;
+	}
+}
+
+extern "C" int mgb_test_seed(const mg_idx_t *gi, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off, const int32_t *seg_len,
+							 const char *const *names, uint64_t flag, int occ_max1, int max_qlen, int32_t *out, mg128_t *a, int64_t a_cap, int32_t *mini_pos, int64_t mp_cap)
+{
+	try { return test_seed_impl(gi, n, qlens, seqs, seg_off, seg_len, names, flag, occ_max1, max_qlen, out, (u128*)a, a_cap, mini_pos, mp_cap); } catch (const MgbError &e) { return e.code; }
 }
 
 extern "C" void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st) { *st = t_has_stats? t_last_stats : model_of(gi)->stats; } // the calling thread's last batch

@@ -155,9 +155,15 @@ MG_HD inline int sketch_chunk(const char *str, const uint64_t *pk, int w, int k,
 static const int SKETCH_SMEM_W = 12; // widest window whose rings fit the shared-memory variant ("seed_v2")
 static const int SKETCH_SMEM_BYTES = SKETCH_SMEM_W * 32 * 16; // per warp
 
+// The ways sketch_seq_w() makes the list: chunks with the rings in shared memory reading the 2-bit words or ASCII, chunks with the
+// rings in the arena (w > SKETCH_SMEM_W or no slice), the sequential scan on lane 0
+enum { SKETCH_PATH_SMEM_PK = 0, SKETCH_PATH_SMEM = 1, SKETCH_PATH_ARENA = 2, SKETCH_PATH_SEQ = 3 };
+
 // sring: NULL, or SKETCH_SMEM_BYTES of shared memory of this warp for the window rings
 // pk: NULL, or the sequence 2 bits per base (see sketch_chunk); str is always there (the sequential scan below reads it)
-MG_HD inline int sketch_seq_w(Arena &A, const char *str, int len, int w, int k, uint32_t rid, AVec<u128> &out, int lane, u128 *sring = 0, const uint64_t *pk = 0)
+// path: NULL, or where the way the list was made goes (SKETCH_PATH_*)
+MG_HD inline int sketch_seq_w(Arena &A, const char *str, int len, int w, int k, uint32_t rid, AVec<u128> &out, int lane, u128 *sring = 0, const uint64_t *pk = 0,
+							  int *path = 0)
 {
 	if (!(len > 0 && w > 0 && w < 256 && k > 0 && k <= 28)) return MGB_E_INTERNAL;
 	const int min_chunk = w + 2 * k > 64? w + 2 * k : 64;
@@ -192,19 +198,23 @@ MG_HD inline int sketch_seq_w(Arena &A, const char *str, int len, int w, int k, 
 			int64_t off = cnt[0];
 			for (int c = 1; c < n_ch; ++c) {
 				const u128 *src = tmp + (int64_t)c * cap;
-				for (int j0 = 0; j0 < cnt[c]; j0 += MGB_W) {
+				// read once, before the moves: past the last warp_sync below a lane may already be on to the caller, whose allocations
+				// take the arena behind the list (cnt[] included) while another lane would still test its loop bound there
+				const int32_t n_c = cnt[c];
+				for (int j0 = 0; j0 < n_c; j0 += MGB_W) {
 					const int j = j0 + lane;
 					u128 e = {0, 0};
-					if (j < cnt[c]) e = src[j];
+					if (j < n_c) e = src[j];
 					warp_sync();
-					if (j < cnt[c]) dst[off + j] = e;
+					if (j < n_c) dst[off + j] = e;
 					warp_sync();
 				}
-				off += cnt[c];
+				off += n_c;
 			}
 			A.top = mark + ((((uint64_t)tot + 16) * sizeof(u128) + 15) & ~(uint64_t)15);
 			if (A.top > A.peak) A.peak = A.top;
 			out.a = dst, out.n = tot, out.m = tot + 16;
+			if (path) *path = !(sring && w <= SKETCH_SMEM_W)? SKETCH_PATH_ARENA : pk? SKETCH_PATH_SMEM_PK : SKETCH_PATH_SMEM;
 			return 0;
 		}
 		A.top = mark;
@@ -221,6 +231,7 @@ MG_HD inline int sketch_seq_w(Arena &A, const char *str, int len, int w, int k, 
 		A.top = warp_bcast_u64(B.top, 0);
 		A.peak = warp_bcast_u64(B.peak, 0);
 		warp_sync();
+		if (path) *path = SKETCH_PATH_SEQ;
 		return rc;
 	}
 }
