@@ -10,6 +10,8 @@
 #include <string.h>
 #include <math.h>
 #include <vector>
+#include <array>
+#include <memory>
 #include <algorithm>
 #include <string>
 #include <chrono>
@@ -70,23 +72,30 @@ extern "C" int mgb_set_param(const char *key, int64_t value)
 // device memory shim
 // ---------------------------------------------------------------------------------------------------------------
 
-#ifdef MGB_HOSTSIM
+static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// A failed CUDA call (out of memory, a fault in a kernel) unwinds to the C entry point, which returns NULL / a negative code with
+// the reason in mgb_last_error(); the library never ends the host process on its own.
 struct MgbError { int code; };
+#ifdef MGB_HOSTSIM
 static bool dev_ok(int dev = -1) { (void)dev; return true; }
 static void *dmalloc(size_t n) { void *p = malloc(n? n : 16); return p; }
 static void dfree(void *p) { free(p); }
-static void h2d(void *d, const void *h, size_t n) { if (n) memcpy(d, h, n); }
-static void d2h(void *h, const void *d, size_t n) { if (n) memcpy(h, d, n); }
 static void dzero(void *d, size_t n) { if (n) memset(d, 0, n); }
 static void d2d(void *d, const void *s, size_t n) { if (n) memcpy(d, s, n); }
 static void dfill(void *d, int v, size_t n) { if (n) memset(d, v, n); }
 static void dsync() {}
 static int dev_sm_count() { return 2; }
 static size_t dev_free_mem() { return (size_t)8 << 30; }
+typedef int DevStream;
+typedef double DevEvent; // the host clock when it was recorded
+static void dev_bind(int dev, DevStream s) { (void)dev, (void)s; }
+static void h2d_async(void *d, const void *h, size_t n) { if (n) memcpy(d, h, n); }
+static void d2h_async(void *h, const void *d, size_t n) { if (n) memcpy(h, d, n); }
+static void ev_record(DevEvent &e) { e = now_ms(); }
+static void ev_wait(DevEvent &e) { (void)e; }
+static double ev_ms(DevEvent &a, DevEvent &b) { return b - a; }
 #else
-// A failed CUDA call (out of memory, a fault in a kernel) unwinds to the C entry point, which returns NULL / a negative code with
-// the reason in mgb_last_error(); the library never ends the host process on its own.
-struct MgbError { int code; };
 #define CUDA_OK(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { set_error(std::string(#call) + ": " + cudaGetErrorString(_e)); throw MgbError{MGB_E_INTERNAL}; } } while (0)
 // every host thread that drives a slot of the batch pipeline works on its own stream
 static thread_local cudaStream_t t_stream = 0;
@@ -100,14 +109,26 @@ static bool dev_ok(int dev = -1)
 static void *dmalloc(size_t n) { void *p = 0; CUDA_OK(cudaMalloc(&p, n? n : 16)); return p; }
 static void dfree(void *p) { if (p) cudaFree(p); }
 static void dsync() { CUDA_OK(cudaStreamSynchronize(t_stream)); }
-static void h2d(void *d, const void *h, size_t n) { if (n) { CUDA_OK(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, t_stream)); dsync(); } }
-static void d2h(void *h, const void *d, size_t n) { if (n) { CUDA_OK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, t_stream)); dsync(); } }
 static void dzero(void *d, size_t n) { if (n) CUDA_OK(cudaMemsetAsync(d, 0, n, t_stream)); }
 static void d2d(void *d, const void *s, size_t n) { if (n) CUDA_OK(cudaMemcpyAsync(d, s, n, cudaMemcpyDeviceToDevice, t_stream)); }
 static void dfill(void *d, int v, size_t n) { if (n) CUDA_OK(cudaMemsetAsync(d, v, n, t_stream)); }
 static int dev_sm_count() { static int v = 0; if (v == 0) { int d = 0; CUDA_OK(cudaGetDevice(&d)); CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d)); } return v; } // (the devices of one box are alike)
 static size_t dev_free_mem() { size_t f = 0, t = 0; CUDA_OK(cudaMemGetInfo(&f, &t)); return f; }
+typedef cudaStream_t DevStream;
+typedef cudaEvent_t DevEvent;
+// the calling thread's device and stream (0: the device's default stream)
+static void dev_bind(int dev, DevStream s) { cudaSetDevice(dev); t_stream = s; }
+// copies that do not wait: the host memory must be page-locked and stay untouched until the stream gets past them
+static void h2d_async(void *d, const void *h, size_t n) { if (n) CUDA_OK(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, t_stream)); }
+static void d2h_async(void *h, const void *d, size_t n) { if (n) CUDA_OK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, t_stream)); }
+static void ev_record(DevEvent &e) { CUDA_OK(cudaEventRecord(e, t_stream)); }
+static void ev_wait(DevEvent &e) { CUDA_OK(cudaEventSynchronize(e)); }
+static double ev_ms(DevEvent &a, DevEvent &b) { float t = 0; return cudaEventElapsedTime(&t, a, b) == cudaSuccess? t : 0; }
 #endif
+static void h2d(void *d, const void *h, size_t n) { if (n) h2d_async(d, h, n), dsync(); }
+static void d2h(void *h, const void *d, size_t n) { if (n) d2h_async(h, d, n), dsync(); }
+// kernels launched by the calling thread (every launcher counts its own): map_batch_on() counts those of a batch
+static thread_local int64_t t_launches = 0;
 
 // n elements of device memory, freed when the holder goes out of scope (also when a CUDA call throws) unless release()d
 template<typename T> struct DevBuf {
@@ -128,10 +149,13 @@ template<typename T> static DevBuf<T> upload(const T *h, size_t n)
 	return d;
 }
 
-// grow-only buffers kept across batches: device memory, or page-locked host memory for fast H2D/D2H
+// grow-only buffers kept across batches: device memory, or page-locked host memory for fast H2D/D2H; freed with their owner
 struct GrowBuf {
 	void *p; size_t cap; bool host;
 	GrowBuf(bool host_ = false) : p(0), cap(0), host(host_) {}
+	GrowBuf(const GrowBuf &) = delete;
+	GrowBuf &operator=(const GrowBuf &) = delete;
+	~GrowBuf() { release(); }
 	void release()
 	{
 		if (p == 0) return;
@@ -157,16 +181,11 @@ struct GrowBuf {
 	}
 };
 
-namespace {
-static mgb::HostPool g_host_pool; // packing, result assembly, index build (one caller at a time)
-template<typename F> void parallel_for(int64_t n, F fn)
+// fn(0) .. fn(n - 1) on nt threads of pool; on the calling thread when there is little to do
+static void pfor(mgb::HostPool &pool, int nt, int64_t n, const std::function<void(int64_t)> &fn)
 {
-	int nt = (int)p_host_threads;
-	if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
-	if (n < 64 || nt == 1) { for (int64_t i = 0; i < n; ++i) fn(i); return; }
-	const std::function<void(int64_t)> f = fn;
-	g_host_pool.run(n, nt, f);
-}
+	if (n < 256 || nt <= 1) { for (int64_t i = 0; i < n; ++i) fn(i); return; }
+	pool.run(n, nt, fn);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -424,6 +443,7 @@ static void make_job_order(const LaunchArgs &L, int kind, const int32_t *q, int 
 	for (int b = 0; b < 64; ++b) cnt[b + 1] += cnt[b];
 	for (int i = 0; i < n; ++i) order[cnt[order_bin(order_key(L, kind, q, i))]++] = i;
 #endif
+	++t_launches;
 }
 
 // ---- result blobs in read order ----
@@ -489,6 +509,7 @@ static void pack_results(const PackArgs &P)
 	P.off[P.n] = acc;
 	for (int r = 0; r < P.n; ++r) pack_read(P, r, 0, 1);
 #endif
+	t_launches += 2;
 }
 
 // ---- reads cross PCIe 2 bits per base ----
@@ -574,6 +595,16 @@ __global__ void __launch_bounds__(256) k_unpack(UnpackArgs U)
 	}
 }
 #endif
+static void unpack_reads(const UnpackArgs &U)
+{
+#ifndef MGB_HOSTSIM
+	k_unpack<<<dev_sm_count() * 8, 256, 0, t_stream>>>(U);
+	CUDA_OK(cudaGetLastError());
+#else
+	for (int r = 0; r < U.n_reads; ++r) if (U.pk_off[r] != ~0ULL) for (int64_t wd = 0; wd * 32 < U.seq_len[r]; ++wd) unpack_word(U, r, wd);
+#endif
+	++t_launches;
+}
 
 // ---- the few words the host needs between two kernels (pool fill levels, queue lengths) ----
 // They do not travel by cudaMemcpy: a copy of 16 bytes queues behind whatever another call in flight has put on the copy engines
@@ -605,8 +636,19 @@ MG_HD inline void job_counts(const Pool *pools, int i_gjobs, int i_jobs, unsigne
 #ifndef MGB_HOSTSIM
 __global__ void k_job_counts(const Pool *pools, int i_gjobs, int i_jobs, unsigned int gjobs_done, unsigned int jobs_done, unsigned int *cnt) { job_counts(pools, i_gjobs, i_jobs, gjobs_done, jobs_done, cnt); }
 #endif
+static void count_jobs(const Pool *pools, int i_gjobs, int i_jobs, unsigned int gjobs_done, unsigned int jobs_done, unsigned int *cnt)
+{
+#ifndef MGB_HOSTSIM
+	k_job_counts<<<1, 1, 0, t_stream>>>(pools, i_gjobs, i_jobs, gjobs_done, jobs_done, cnt);
+	CUDA_OK(cudaGetLastError());
+#else
+	job_counts(pools, i_gjobs, i_jobs, gjobs_done, jobs_done, cnt);
+#endif
+	++t_launches;
+}
 static void fetch_mail(const MailSrc &m, Mail *mail)
 {
+	++t_launches;
 #ifndef MGB_HOSTSIM
 	k_mail<<<1, 32, 0, t_stream>>>(m, mail);
 	CUDA_OK(cudaGetLastError());
@@ -674,6 +716,7 @@ static void launch_stage(LaunchArgs &L, const Workers &W)
 	typedef StageSpec<S> Spec;
 	L.arena_base = W.arena, L.arena_bytes = W.arena_bytes, L.arena_peak = W.peak;
 	dzero(L.c.next_read, sizeof(unsigned int)); // in stream order: no host round trip per launch
+	++t_launches;
 #ifdef MGB_HOSTSIM
 	Arena A;
 	arena_init(A, W.arena, Spec::mode == ItemMode::THREAD? (W.arena_bytes / 32) & ~(uint64_t)15 : W.arena_bytes); // one item per thread: a thread's share, as on the device
@@ -764,7 +807,131 @@ __global__ void __launch_bounds__(256) k_gaf_write(GafArgs G)
 	const int lane = threadIdx.x & 31;
 	for (int r = gaf_next_read(G.next + 1, lane); r < G.n; r = gaf_next_read(G.next + 1, lane)) gaf_read(G, r, G.text + G.off[r], lane);
 }
+#else
+// fn(r, lane) on every read, a simulated warp each
+template<typename F>
+static void sim_each_read(int n, const F &fn)
+{
+	bool differ = false;
+	for (int r = 0; r < n; ++r) sim_warp(-1, r, [&](int lane) { return fn(r, lane); }, &differ);
+	if (differ) { set_error("simulated warp: lanes returned different codes from the GAF formatter"); throw MgbError{MGB_E_INTERNAL}; }
+}
 #endif
+// what the dv:f values of every read need (G.req)
+static void gaf_list_requests(const GafArgs &G)
+{
+#ifndef MGB_HOSTSIM
+	k_gaf_req<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	CUDA_OK(cudaGetLastError());
+#else
+	sim_each_read(G.n, [&](int r, int lane) { gaf_requests(G, r, lane); return 0; });
+#endif
+	++t_launches;
+}
+// the length of every read's text and where it starts, in read order (G.off; G.off[n]: the whole text); G.next[0] zeroed
+static void gaf_offsets(const GafArgs &G)
+{
+#ifndef MGB_HOSTSIM
+	k_gaf_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	k_gaf_scan<<<1, 1024, 0, t_stream>>>(G);
+	CUDA_OK(cudaGetLastError());
+#else
+	sim_each_read(G.n, [&](int r, int lane) { const uint64_t b = gaf_read(G, r, 0, lane); if (lane == 0) G.off[r] = b; return (int)b; });
+	uint64_t acc = 0;
+	for (int r = 0; r < G.n; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
+	G.off[G.n] = acc;
+#endif
+	t_launches += 2;
+}
+// the text (G.text); G.next[1] zeroed
+static void gaf_write(const GafArgs &G)
+{
+#ifndef MGB_HOSTSIM
+	k_gaf_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	CUDA_OK(cudaGetLastError());
+#else
+	sim_each_read(G.n, [&](int r, int lane) { return (int)gaf_read(G, r, G.text + G.off[r], lane); });
+#endif
+	++t_launches;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// a batch on the device: where its reads go, its output pools, the timers of its spans
+// ---------------------------------------------------------------------------------------------------------------
+
+// Where the reads of a batch lie: the ASCII copy the kernels read (each read 16-byte aligned, with 8 bytes of slack behind it) and
+// the 2-bit words in which they cross PCIe (a read's words start at pk_off[i], with one spare word behind them)
+struct BatchLayout {
+	std::vector<uint64_t> seq_off, pk_off;
+	uint64_t seq_bytes = 0, n_words = 0;
+	int64_t n_bases = 0;
+	BatchLayout(int n, const int32_t *len) : seq_off((size_t)n), pk_off((size_t)n)
+	{
+		for (int i = 0; i < n; ++i) {
+			const uint64_t l = len[i] > 0? (uint64_t)len[i] : 0;
+			seq_off[(size_t)i] = seq_bytes, seq_bytes = (seq_bytes + l + 8 + 15) & ~(uint64_t)15;
+			pk_off[(size_t)i] = n_words, n_words += (l + 31) / 32 + 1;
+			n_bases += (int64_t)l;
+		}
+		seq_bytes += 16;
+	}
+};
+
+// The page-locked host copies and the device copies of a batch's reads and per-read tables (upload_batch)
+struct Staging {
+	GrowBuf h_tables{true}, h_seq{true}, h_pk{true}, d_tables, d_seq, d_pk, d_segs;
+};
+
+// The output pools of a batch (PipeCtx); an attempt at the batch that overflows one is run again with that pool grown
+enum PoolId { P_ANCHOR, P_MINIPOS, P_LCHAIN, P_OUT, P_PLAN, P_JOBS, P_CIG, P_GSTATE, P_GJOBS, P_WALK, N_POOLS };
+// their capacities at the first attempt
+static std::array<uint64_t, N_POOLS> pool_caps(int n_reads, int64_t n_bases, int n_workers)
+{
+	std::array<uint64_t, N_POOLS> cap;
+	cap[P_ANCHOR] = std::max<uint64_t>((uint64_t)n_bases / 4 * sizeof(u128), (uint64_t)1 << 22);
+	cap[P_MINIPOS] = std::max<uint64_t>((uint64_t)n_bases * sizeof(int32_t) / 2, (uint64_t)1 << 20);
+	cap[P_LCHAIN] = std::max<uint64_t>((uint64_t)n_reads * 64 * sizeof(LChain), (uint64_t)1 << 20);
+	cap[P_OUT] = std::max<uint64_t>((uint64_t)n_bases * 4, (uint64_t)1 << 22);
+	cap[P_PLAN] = std::max<uint64_t>((uint64_t)n_bases / 8 * 8, (uint64_t)1 << 20);
+	cap[P_JOBS] = std::max<uint64_t>((uint64_t)n_bases / 40 * sizeof(WfaJob), (uint64_t)1 << 20);
+	cap[P_CIG] = std::max<uint64_t>((uint64_t)n_bases, (uint64_t)1 << 20) + (uint64_t)n_workers * CIG_CHUNK_BYTES * 4; // + the unused ends of the warps' slices (three tier kernels per pass)
+	cap[P_GSTATE] = std::max<uint64_t>((uint64_t)n_reads * 2048, (uint64_t)1 << 20);
+	cap[P_GJOBS] = std::max<uint64_t>((uint64_t)n_reads * 24 * sizeof(GwfaJob), (uint64_t)1 << 20);
+	cap[P_WALK] = std::max<uint64_t>((uint64_t)n_reads * 256, (uint64_t)1 << 20);
+	return cap;
+}
+
+#ifndef MGB_HOSTSIM
+struct EvTimer {
+	cudaEvent_t a, b; bool used;
+	EvTimer() : used(false) { cudaEventCreate(&a); cudaEventCreate(&b); }
+	~EvTimer() { cudaEventDestroy(a); cudaEventDestroy(b); }
+	void start() { cudaEventRecord(a, t_stream); used = true; }
+	void stop() { cudaEventRecord(b, t_stream); }
+	double ms() { if (!used) return 0; float t = 0; cudaEventSynchronize(b); cudaEventElapsedTime(&t, a, b); return t; }
+	void clear() { used = false; }
+};
+#else
+struct EvTimer { double t0 = 0, t1 = 0; void start() { t0 = now_ms(); } void stop() { t1 = now_ms(); } double ms() { return t1 - t0; } void clear() { t0 = t1 = 0; } };
+#endif
+
+struct SlotTimers {
+	EvTimer h2d, seed, chain, align, wfa, fin, d2h, lab, k[10];
+	void reset() { EvTimer *all[] = {&h2d, &seed, &chain, &align, &wfa, &fin, &d2h, &lab}; for (EvTimer *t : all) t->clear(); for (int i = 0; i < 10; ++i) k[i].clear(); }
+	void to_stats(mgb_stats_t &S) // all but t_d2h_ms, which ends with the batch
+	{
+		S.t_h2d_ms = h2d.ms(), S.t_seed_ms = seed.ms(), S.t_chain_ms = chain.ms(), S.t_align_ms = align.ms();
+		S.t_wfa_ms = wfa.ms(), S.t_finish_ms = fin.ms(), S.t_lab_ms = lab.ms();
+		for (int i = 0; i < 10; ++i) S.t_kernel_ms[i] = k[i].ms();
+	}
+};
+
+// t times the launches of one scope; NULL: an untimed scope
+struct Span {
+	EvTimer *t;
+	explicit Span(EvTimer *t_) : t(t_) { if (t) t->start(); }
+	~Span() { if (t) t->stop(); }
+};
 
 // ---------------------------------------------------------------------------------------------------------------
 // model: flattened graph + minimizer index, host copy and device image
@@ -800,17 +967,15 @@ struct Model {
 	// the batch pipeline: a batch is cut into sub-batches, each driven by its own host thread on its own stream ("slot"),
 	// so that kernels, copies and host-side result assembly of different sub-batches overlap
 	struct Slot {
-		GrowBuf h_seq{true}, h_out{true}, h_small{true}, h_pk{true}, h_mail{true}, h_routs{true}, d_pk, d_seq, d_meta, d_routs, d_small, d_jobq, d_order, d_packed, d_packoff, d_segs, d_lab_new, d_pool[10];
+		Staging stage;
+		GrowBuf h_out{true}, h_mail{true}, h_routs{true}, d_meta, d_routs, d_scratch, d_jobq, d_order, d_packed, d_packoff, d_lab_new, d_pool[N_POOLS];
 		GrowBuf h_gaf{true}, d_gaf, d_gaf_text; // mgb_map_batch_gaf(): the reads' names and segments, requests and cells; the text
 		mgb::HostPool host_pool; // packing and result assembly of the batch on this slot
 		Workers W;
 		mgb_stats_t st;
-		double ev_first_ms, ev_last_ms; // first kernel start / last kernel end relative to the batch reference event
-#ifndef MGB_HOSTSIM
-		cudaStream_t stream;
-		cudaEvent_t ev_first, ev_last, ev_piece[4];
-#endif
-		struct SlotTimers *timers = 0;
+		DevStream stream;
+		DevEvent ev_first, ev_last, ev_piece[4]; // first kernel start and last kernel end of the batch; the end of each piece's download
+		std::unique_ptr<SlotTimers> timers; // the event pairs live in the slot: creating and destroying three dozen events per call contends on the driver's lock with the other calls in flight
 		bool ready;
 		Slot() : ready(false) { memset(&W, 0, sizeof(W)); }
 	};
@@ -829,8 +994,6 @@ struct Model {
 	uint64_t lab_cap = 0; int32_t lab_max_dist_g = -1; int64_t lab_sources = 0;
 };
 
-struct SlotTimers;
-static void timers_free(SlotTimers *t);
 static void model_free(Model *M)
 {
 	for (Model *P : M->peers) model_free(P);
@@ -847,17 +1010,13 @@ static void model_free(Model *M)
 	dfree(M->d_lab_off), dfree(M->d_lab_hdr), dfree(M->d_lab_pool), dfree(M->d_occ_sorted);
 	for (int k = 0; k < Model::MAX_SLOTS; ++k) {
 		Model::Slot &sl = M->slots[k];
-		sl.h_seq.release(), sl.h_out.release(), sl.h_small.release(), sl.h_pk.release(), sl.h_mail.release(), sl.h_routs.release(), sl.d_pk.release(), sl.d_seq.release(), sl.d_meta.release(), sl.d_routs.release(), sl.d_small.release(), sl.d_jobq.release(), sl.d_order.release(), sl.d_packed.release(), sl.d_packoff.release(), sl.d_segs.release(), sl.d_lab_new.release();
-		sl.h_gaf.release(), sl.d_gaf.release(), sl.d_gaf_text.release();
-		for (int i = 0; i < 10; ++i) sl.d_pool[i].release();
-		if (sl.timers) timers_free(sl.timers);
 		if (sl.W.arena) dfree(sl.W.arena);
 		if (sl.W.peak) dfree(sl.W.peak);
 #ifndef MGB_HOSTSIM
 		if (sl.ready) { cudaStreamDestroy(sl.stream); cudaEventDestroy(sl.ev_first); cudaEventDestroy(sl.ev_last); for (int i = 0; i < 4; ++i) cudaEventDestroy(sl.ev_piece[i]); }
 #endif
 	}
-	delete M;
+	delete M; // (with it the slots' buffers and timers, on this device)
 }
 
 // reference: gfa-base.c:509-526 gfa_comp_table.  Filled once: with MGB_DEVICES, mg_index() builds the models of the further devices
@@ -898,6 +1057,24 @@ static int default_workers()
 #else
 	return dev_sm_count() * (int)p_workers_per_sm;
 #endif
+}
+
+// The slot on the model's device: its stream and events made at its first batch, its arenas sized; then the calling thread works on
+// its stream
+static void slot_prepare(Model *M, Model::Slot &sl, int n_workers)
+{
+#ifndef MGB_HOSTSIM
+	cudaSetDevice(M->device);
+	if (!sl.ready) {
+		CUDA_OK(cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
+		CUDA_OK(cudaEventCreate(&sl.ev_first));
+		CUDA_OK(cudaEventCreate(&sl.ev_last));
+		for (int i = 0; i < 4; ++i) CUDA_OK(cudaEventCreateWithFlags(&sl.ev_piece[i], cudaEventDisableTiming));
+	}
+#endif
+	sl.ready = true;
+	ensure_workers(sl.W, n_workers, (uint64_t)p_arena_mb << 20);
+	dev_bind(M->device, sl.stream);
 }
 
 static Model *model_build(gfa_t *g, int k, int w)
@@ -1221,29 +1398,6 @@ extern "C" void mgb_free_batch(int n_reads, mg_gchains_t **gcs)
 // batch dispatcher
 // ---------------------------------------------------------------------------------------------------------------
 
-static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-#ifndef MGB_HOSTSIM
-struct EvTimer {
-	cudaEvent_t a, b; bool used;
-	EvTimer() : used(false) { cudaEventCreate(&a); cudaEventCreate(&b); }
-	~EvTimer() { cudaEventDestroy(a); cudaEventDestroy(b); }
-	void start() { cudaEventRecord(a, t_stream); used = true; }
-	void stop() { cudaEventRecord(b, t_stream); }
-	double ms() { if (!used) return 0; float t = 0; cudaEventSynchronize(b); cudaEventElapsedTime(&t, a, b); return t; }
-	void clear() { used = false; }
-};
-#else
-struct EvTimer { double t0 = 0, t1 = 0; void start() { t0 = now_ms(); } void stop() { t1 = now_ms(); } double ms() { return t1 - t0; } void clear() { t0 = t1 = 0; } };
-#endif
-
-struct SlotTimers {
-	EvTimer h2d, seed, chain, align, wfa, fin, d2h, lab, k[10];
-	void reset() { EvTimer *all[] = {&h2d, &seed, &chain, &align, &wfa, &fin, &d2h, &lab}; for (EvTimer *t : all) t->clear(); for (int i = 0; i < 10; ++i) k[i].clear(); }
-};
-
-static void timers_free(SlotTimers *t) { delete t; }
-
 static void fill_opt(MapOptDev &o, const mg_mapopt_t *opt, int k)
 {
 	memset(&o, 0, sizeof(o));
@@ -1363,16 +1517,35 @@ struct GafJob {
 	size_t len;
 };
 
+// A batch of 2048 reads or more goes up and comes back in 4 pieces, so that the host threads pack or assemble one piece while
+// another is on the wire.  Piece pc holds reads [r0(pc), r0(pc + 1)).
+struct Pieces {
+	int n_reads, n;
+	explicit Pieces(int n_reads_) : n_reads(n_reads_), n(n_reads_ >= 2048? 4 : 1) {}
+	int64_t r0(int pc) const { return (int64_t)n_reads * pc / n; }
+};
+
+// Bytes [off[r0], off[r1]) of each piece of the reads from d to h, each piece followed by the event the host waits for before it
+// reads them
+static void download_in_pieces(Model::Slot &sl, int n_reads, const uint64_t *off, char *h, const char *d)
+{
+	const Pieces pcs(n_reads);
+	for (int pc = 0; pc < pcs.n; ++pc) {
+		const uint64_t b0 = off[pcs.r0(pc)], b1 = off[pcs.r0(pc + 1)];
+		d2h_async(h + b0, d + b0, b1 - b0);
+		ev_record(sl.ev_piece[pc]);
+	}
+}
+
+// a read's outcome: the code of the stage that failed it, or else ReadOut::status (1: not mapped)
+static int read_status(const ReadMeta &m, const ReadOut &o) { return m.status < 0? m.status : o.status; }
+
 // The GAF text of a mapped sub-batch, formatted on the device from the blobs in the output pool (mgb_gaf.cuh): requests for the dv:f
 // values, cells formatted by the host, count, scan, write; then the text goes to the host in pieces, each copied on to the caller's
 // buffer by the host threads while the next is on the wire.  Returns 0 or a negative code.
 static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int *qlens, const char *const *names, const ReadOut *routs,
 					const ReadOut *d_routs, const char *d_pool, int host_threads, mgb_stats_t &S, EvTimer &tm_d2h)
 {
-	auto pfor = [&](int64_t n, const std::function<void(int64_t)> &fn) {
-		if (n < 256 || host_threads <= 1) { for (int64_t i = 0; i < n; ++i) fn(i); return; }
-		sl.host_pool.run(n, host_threads, fn);
-	};
 	const size_t n = (size_t)n_reads;
 	const bool lchain = (J.flag & F_WRITE_LCHAIN) != 0;
 	size_t n_segs = 0, name_bytes = 0, n_req = 0;
@@ -1414,79 +1587,47 @@ static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int
 	G.routs = d_routs, G.pool = d_pool, G.n = n_reads, G.flag = J.flag;
 	G.req_off = (const int64_t*)(d + o_req_off), G.req = (GafReq*)(d + o_req), G.cells = d + o_cells;
 	G.off = (uint64_t*)(d + o_off), G.text = 0, G.next = (unsigned int*)(d + o_next);
-#ifdef MGB_HOSTSIM
-	bool differ = false;
-	auto each_read = [&](const std::function<int(int, int)> &fn) { for (int r = 0; r < n_reads; ++r) sim_warp(-1, r, [&](int lane) { return fn(r, lane); }, &differ); };
-#endif
-	tm_d2h.start();
-	// dv:f values: the device lists what each needs, the host formats them with its libm (SURVEY H3)
-#ifdef MGB_HOSTSIM
-	each_read([&](int r, int lane) { gaf_requests(G, r, lane); return 0; });
-#else
-	if (n_req) { k_gaf_req<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G); CUDA_OK(cudaGetLastError()); }
-#endif
-	d2h(h + o_req, d + o_req, sizeof(GafReq) * n_req);
-	const GafReq *hreq = (const GafReq*)(h + o_req);
-	char *hcells = h + o_cells;
-	pfor((int64_t)n_req, [&](int64_t k) {
-		const GafReq &q = hreq[k];
-		char *c = hcells + (size_t)GAF_CELL * (size_t)k;
-		c[0] = 0;
-		if (q.kind == 0) { // format.c:204-209
-			const float div = gc_div(q.a, q.b, q.q_span);
-			if (div >= 0.0f && div <= 1.0f) { if (div == 0.0f) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div); }
-		} else if (q.kind == 1) { // format.c:256-263
-			const double div = q.a == q.b? 0.0 : (q.a > q.b? log((double)q.a / q.b) : log((double)q.b / q.a)) / q.q_span;
-			if (div == 0.0) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div);
-		}
-	});
-	h2d(d + o_cells, hcells, (size_t)GAF_CELL * n_req);
-	// text: sizes, offsets in read order, bytes
-	dzero(G.next, 2 * sizeof(unsigned int));
-#ifdef MGB_HOSTSIM
-	each_read([&](int r, int lane) { const uint64_t b = gaf_read(G, r, 0, lane); if (lane == 0) G.off[r] = b; return (int)b; });
-	uint64_t acc = 0;
-	for (size_t r = 0; r < n; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
-	G.off[n] = acc;
-#else
-	k_gaf_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
-	k_gaf_scan<<<1, 1024, 0, t_stream>>>(G);
-	CUDA_OK(cudaGetLastError());
-#endif
-	uint64_t *hoff = (uint64_t*)(h + o_off);
-	d2h(hoff, G.off, 8 * (n + 1));
-	const uint64_t total = hoff[n];
-	G.text = (char*)sl.d_gaf_text.ensure(total + 64);
-	char *htext = (char*)sl.h_out.ensure(total + 64);
-#ifdef MGB_HOSTSIM
-	each_read([&](int r, int lane) { return (int)gaf_read(G, r, G.text + G.off[r], lane); });
-	if (differ) { set_error("simulated warp: lanes returned different codes from the GAF formatter"); return MGB_E_INTERNAL; }
-#else
-	k_gaf_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
-	CUDA_OK(cudaGetLastError());
-#endif
-	S.n_launches += 4;
-	const int n_piece = n_reads >= 2048? 4 : 1;
-	for (int pc = 0; pc < n_piece; ++pc) {
-		const uint64_t b0 = hoff[n * pc / n_piece], b1 = hoff[n * (pc + 1) / n_piece];
-#ifndef MGB_HOSTSIM
-		if (b1 > b0) CUDA_OK(cudaMemcpyAsync(htext + b0, G.text + b0, b1 - b0, cudaMemcpyDeviceToHost, t_stream));
-		CUDA_OK(cudaEventRecord(sl.ev_piece[pc], t_stream));
-#else
-		if (b1 > b0) memcpy(htext + b0, G.text + b0, b1 - b0);
-#endif
+	const Pieces pcs(n_reads);
+	const uint64_t *hoff = (const uint64_t*)(h + o_off);
+	char *htext;
+	{
+		Span span(&tm_d2h);
+		// dv:f values: the device lists what each needs, the host formats them with its libm (SURVEY H3)
+		if (n_req) gaf_list_requests(G);
+		d2h(h + o_req, d + o_req, sizeof(GafReq) * n_req);
+		const GafReq *hreq = (const GafReq*)(h + o_req);
+		char *hcells = h + o_cells;
+		pfor(sl.host_pool, host_threads, (int64_t)n_req, [&](int64_t k) {
+			const GafReq &q = hreq[k];
+			char *c = hcells + (size_t)GAF_CELL * (size_t)k;
+			c[0] = 0;
+			if (q.kind == 0) { // format.c:204-209
+				const float div = gc_div(q.a, q.b, q.q_span);
+				if (div >= 0.0f && div <= 1.0f) { if (div == 0.0f) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div); }
+			} else if (q.kind == 1) { // format.c:256-263
+				const double div = q.a == q.b? 0.0 : (q.a > q.b? log((double)q.a / q.b) : log((double)q.b / q.a)) / q.q_span;
+				if (div == 0.0) c[0] = '0', c[1] = 0; else snprintf(c, GAF_CELL, "%.4f", div);
+			}
+		});
+		h2d(d + o_cells, hcells, (size_t)GAF_CELL * n_req);
+		// text: sizes, offsets in read order, bytes
+		dzero(G.next, 2 * sizeof(unsigned int));
+		gaf_offsets(G);
+		d2h(h + o_off, G.off, 8 * (n + 1));
+		G.text = (char*)sl.d_gaf_text.ensure(hoff[n] + 64);
+		htext = (char*)sl.h_out.ensure(hoff[n] + 64);
+		gaf_write(G);
+		download_in_pieces(sl, n_reads, hoff, htext, G.text);
 	}
-	tm_d2h.stop();
+	const uint64_t total = hoff[n];
 	const double t_asm0 = now_ms();
 	char *dst = J.dest((size_t)total);
 	if (dst == 0) { dsync(); set_error("mgb_map_batch_gaf: out of host memory for the text"); return MGB_E_INTERNAL; }
 	const uint64_t chunk = 1 << 20;
-	for (int pc = 0; pc < n_piece; ++pc) {
-		const uint64_t b0 = hoff[n * pc / n_piece], b1 = hoff[n * (pc + 1) / n_piece];
-#ifndef MGB_HOSTSIM
-		CUDA_OK(cudaEventSynchronize(sl.ev_piece[pc]));
-#endif
-		pfor((int64_t)((b1 - b0 + chunk - 1) / chunk), [&](int64_t k) {
+	for (int pc = 0; pc < pcs.n; ++pc) {
+		const uint64_t b0 = hoff[pcs.r0(pc)], b1 = hoff[pcs.r0(pc + 1)];
+		ev_wait(sl.ev_piece[pc]);
+		pfor(sl.host_pool, host_threads, (int64_t)((b1 - b0 + chunk - 1) / chunk), [&](int64_t k) {
 			const uint64_t c0 = b0 + (uint64_t)k * chunk, c1 = std::min(b1, c0 + chunk);
 			memcpy(dst + c0, htext + c0, c1 - c0);
 		});
@@ -1498,13 +1639,261 @@ static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int
 	return 0;
 }
 
-// MG_M_NO_DIAG: which segment name, if any, is each read's own (BatchDev::self_id; exact string match on the host)
-static std::vector<int32_t> read_self_ids(const Model *M, int n_reads, const char *const *names)
+// Copies a batch laid out as lay says to the device and returns what the kernels read of it.  The reads go up 2 bits per base (a
+// quarter of the bytes) and k_unpack writes their ASCII copy on the device; a read with any byte other than A/C/G/T goes up as
+// ASCII, and so does the whole batch when such reads are many or the fragments have segments (seg_off, seg_len: as BatchDev has
+// them, or NULL).  t (or NULL) times the reads, the per-read tables and k_unpack.
+static BatchDev upload_batch(Staging &B, const BatchLayout &lay, const Model *M, int n_reads, const int *qlens, const char *const *seqs,
+							 const char *const *names, bool no_diag, const int32_t *seg_off, const int32_t *seg_len, mgb::HostPool &pool, int nt,
+							 EvTimer *t, mgb_stats_t &S)
 {
-	std::vector<int32_t> self((size_t)n_reads, -1);
-	for (int i = 0; i < n_reads; ++i)
-		if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[(size_t)i] = it->second; }
-	return self;
+	const size_t n = (size_t)n_reads;
+	uint64_t *seq_off = (uint64_t*)B.h_tables.ensure(n * 16 + 256); // seq_off, seq_len and name_hash: one copy
+	int32_t *seq_len = (int32_t*)(seq_off + n);
+	uint32_t *name_hash = (uint32_t*)(seq_len + n);
+	memcpy(seq_off, lay.seq_off.data(), n * 8);
+	for (size_t i = 0; i < n; ++i) seq_len[i] = qlens[i], name_hash[i] = names && names[i]? hash_str(names[i]) : 0;
+	char *hseq = (char*)B.h_seq.ensure(lay.seq_bytes), *d_seq = (char*)B.d_seq.ensure(lay.seq_bytes);
+	const Pieces pcs(n_reads);
+	BatchDev b;
+	memset(&b, 0, sizeof(b));
+	{
+		Span span(t);
+		// put(r) for the reads of each piece, then the piece's copy; returns the host's time
+		auto in_pieces = [&](const std::function<void(int64_t)> &put, char *d, const char *h, const uint64_t *off, uint64_t end, uint64_t unit) {
+			double t_pack = 0;
+			for (int pc = 0; pc < pcs.n; ++pc) {
+				const int64_t r0 = pcs.r0(pc), r1 = pcs.r0(pc + 1);
+				const double tp0 = now_ms();
+				pfor(pool, nt, r1 - r0, [&](int64_t i) { put(r0 + i); });
+				t_pack += now_ms() - tp0;
+				const uint64_t b0 = off[r0] * unit, b1 = (r1 < n_reads? off[r1] : end) * unit;
+				h2d_async(d + b0, h + b0, b1 - b0);
+			}
+			return t_pack;
+		};
+		bool packed = seg_off == 0;
+		uint64_t *pk_off = 0, *d_pk = 0, *d_pk_off = 0;
+		if (packed) {
+			const size_t n8 = (n + 7) & ~(size_t)7;
+			pk_off = (uint64_t*)B.h_pk.ensure(n * 8 + 64 + (size_t)(lay.n_bases / 4) + n * 16);
+			memcpy(pk_off, lay.pk_off.data(), n * 8);
+			uint64_t *hpk = pk_off + n8;
+			d_pk_off = (uint64_t*)B.d_pk.ensure((n8 + lay.n_words + 8) * 8);
+			d_pk = d_pk_off + n8;
+			std::vector<uint8_t> raw(n, 0);
+			const double t_pack = in_pieces([&](int64_t r) { if (qlens[r] > 0 && !pack_read(seqs[r], qlens[r], hpk + pk_off[r])) raw[(size_t)r] = 1; },
+											(char*)d_pk, (const char*)hpk, pk_off, lay.n_words, 8);
+			int64_t n_raw = 0;
+			for (size_t i = 0; i < n; ++i) n_raw += raw[i];
+			if (n_raw > 64) packed = false; // not worth a copy per read
+			else {
+				S.t_pack_ms = t_pack;
+				S.h2d_bytes = (int64_t)(lay.n_words * 8);
+				for (size_t i = 0; i < n; ++i)
+					if (raw[i]) {
+						memcpy(hseq + seq_off[i], seqs[i], (size_t)qlens[i]);
+						h2d_async(d_seq + seq_off[i], hseq + seq_off[i], (size_t)qlens[i]);
+						pk_off[i] = ~0ULL, S.h2d_bytes += qlens[i];
+					}
+				h2d(d_pk_off, pk_off, n * 8);
+			}
+		}
+		if (!packed) {
+			S.t_pack_ms += in_pieces([&](int64_t r) { if (qlens[r] > 0) memcpy(hseq + seq_off[r], seqs[r], (size_t)qlens[r]); }, d_seq, hseq, seq_off, lay.seq_bytes, 1);
+			dsync();
+			S.h2d_bytes = (int64_t)lay.seq_bytes;
+		}
+		uint64_t *d_seq_off = (uint64_t*)B.d_tables.ensure(n * 20 + 64); // seq_off, seq_len, name_hash, self_id
+		h2d(d_seq_off, seq_off, n * 16);
+		S.h2d_bytes += (int64_t)n * 16;
+		b.n_reads = n_reads, b.seq = d_seq, b.seq_off = d_seq_off, b.seq_len = (const int32_t*)(d_seq_off + n), b.name_hash = (const uint32_t*)(b.seq_len + n);
+		b.pk = packed? d_pk : 0, b.pk_off = packed? d_pk_off : 0;
+		if (packed) unpack_reads(UnpackArgs{d_pk, d_pk_off, d_seq_off, b.seq_len, d_seq, n_reads});
+	}
+	if (no_diag) { // which segment name, if any, is each read's own (exact string match on the host)
+		std::vector<int32_t> self(n, -1);
+		for (size_t i = 0; i < n; ++i)
+			if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[i] = it->second; }
+		int32_t *d_self_id = (int32_t*)(b.name_hash + n);
+		h2d(d_self_id, self.data(), sizeof(int32_t) * n);
+		b.self_id = d_self_id;
+	}
+	if (seg_off) {
+		const size_t n_len = (size_t)seg_off[n];
+		int32_t *d_segs = (int32_t*)B.d_segs.ensure(sizeof(int32_t) * (n + 1 + n_len));
+		h2d(d_segs, seg_off, sizeof(int32_t) * (n + 1));
+		h2d(d_segs + n + 1, seg_len, sizeof(int32_t) * n_len);
+		b.seg_off = d_segs, b.seg_len = d_segs + n + 1;
+	}
+	return b;
+}
+
+// The slot's device scratch for a batch: the read list of the retry pass, the reads k_chain hands to k_chain_rescue, work counters,
+// profile counters, pool headers and the tier histogram
+struct PassScratch {
+	int32_t *list, *rescue;
+	unsigned int *next, *jobq_n, *rescue_n, *cnt, *tier_hist; // cnt: [0] bridging jobs, [1] gap jobs the next job kernel has to take
+	unsigned long long *prof;
+	Pool *pools;
+	PassScratch(GrowBuf &buf, int n_reads)
+	{
+		list = (int32_t*)buf.ensure((size_t)n_reads * 8 + 4096 + 1024), rescue = list + n_reads;
+		char *dsm = (char*)(((uintptr_t)(rescue + n_reads) + 255) & ~(uintptr_t)255);
+		next = (unsigned int*)dsm, jobq_n = next + 4, rescue_n = next + 8, cnt = next + 10;
+		prof = (unsigned long long*)(dsm + 64);
+		pools = (Pool*)(dsm + 64 + sizeof(unsigned long long) * PROF_N);
+		tier_hist = (unsigned int*)((char*)(pools + 16) + 64); // 32 x 4 counters behind the pool headers
+	}
+};
+
+// One attempt at a batch: its pools, emptied, and one pass of the pipeline over its reads (run), or over the list of the
+// large-arena retry.  Every kernel after k_gchain reads its number of items on the device, so a pass is queued without a host round
+// trip, and nothing another thread does in the driver (large copies, blocking waits) can open gaps between its kernels; the mailbox
+// at its end is its one wait.
+struct Pass {
+	Model::Slot &sl;
+	const PassScratch &D;
+	LaunchArgs L;
+	int64_t max_jobs, jobs_done = 0, gjobs_done = 0;
+	int32_t *jobq, *order; // the queues of tiers 2 and 3 (max_jobs each); the order of a job list
+	unsigned int *lab_n;   // the sources k_chain listed for the label searches; NULL: no label table
+	MailSrc msrc;
+	Mail *mail;
+	Pass(Model *M, Model::Slot &sl_, const MapOptDev &o, const BatchDev &b, const PassScratch &D_, const std::array<uint64_t, N_POOLS> &cap,
+		 unsigned int *lab_n_, int32_t skip1) : sl(sl_), D(D_), lab_n(lab_n_)
+	{
+		void *buf[N_POOLS];
+		Pool hp[N_POOLS];
+		for (int i = 0; i < N_POOLS; ++i) buf[i] = sl.d_pool[i].ensure(cap[i]), hp[i].used = 0, hp[i].cap = cap[i];
+		h2d(D.pools, hp, sizeof(hp));
+		dfill(buf[P_GJOBS], 0xff, cap[P_GJOBS]); // reserved-but-unused bridging job slots read as rid == -1
+		dfill(buf[P_JOBS], 0xff, cap[P_JOBS]);   // the same for gap jobs: slots of an allocation that overflowed the pool are never written
+		memset(&L, 0, sizeof(L));
+		L.c.g = M->g, L.c.ix = M->ix, L.c.opt = o, L.c.b = b;
+		L.c.meta = (ReadMeta*)sl.d_meta.p, L.routs = (ReadOut*)sl.d_routs.p;
+		L.c.pool_anchor = &D.pools[P_ANCHOR], L.c.anchor = (u128*)buf[P_ANCHOR];
+		L.c.pool_minipos = &D.pools[P_MINIPOS], L.c.minipos = (int32_t*)buf[P_MINIPOS];
+		L.c.pool_lchain = &D.pools[P_LCHAIN], L.c.lchain = (LChain*)buf[P_LCHAIN];
+		L.c.pool_out = &D.pools[P_OUT], L.c.out = (char*)buf[P_OUT];
+		L.c.pool_plan = &D.pools[P_PLAN], L.c.plan = (uint64_t*)buf[P_PLAN];
+		L.c.pool_jobs = &D.pools[P_JOBS], L.c.jobs = (WfaJob*)buf[P_JOBS];
+		L.c.pool_cig = &D.pools[P_CIG], L.c.cig = (uint32_t*)buf[P_CIG];
+		L.c.pool_gstate = &D.pools[P_GSTATE], L.c.gstate = (char*)buf[P_GSTATE];
+		L.c.pool_gjobs = &D.pools[P_GJOBS], L.c.gjobs = (GwfaJob*)buf[P_GJOBS];
+		L.c.pool_walk = &D.pools[P_WALK], L.c.walk = (int32_t*)buf[P_WALK];
+		L.c.next_read = D.next;
+		L.c.rescue_list = D.rescue, L.c.rescue_n = D.rescue_n;
+		if (lab_n) {
+			L.c.lab.src_off = M->d_lab_off, L.c.lab.pool_hdr = M->d_lab_hdr, L.c.lab.pool = M->d_lab_pool, L.c.lab.new_src = (int32_t*)(lab_n + 4), L.c.lab.n_new = lab_n;
+			L.c.lab.max_dist_g = M->lab_max_dist_g, L.c.lab.cap_new = M->g.n_seg * 2;
+			dzero(lab_n, 2 * sizeof(unsigned int));
+		}
+		L.c.prof = D.prof;
+		L.c.tier_hist = D.tier_hist, L.c.skip1_len = skip1;
+		L.c.jobq_n = D.jobq_n;
+		max_jobs = (int64_t)(cap[P_JOBS] / sizeof(WfaJob)) + 1;
+		const int64_t max_gjobs = (int64_t)(cap[P_GJOBS] / sizeof(GwfaJob)) + 1;
+		jobq = (int32_t*)sl.d_jobq.ensure(sizeof(int32_t) * 2 * (size_t)max_jobs);
+		order = (int32_t*)sl.d_order.ensure(sizeof(int32_t) * (size_t)std::max<int64_t>(std::max<int64_t>(max_jobs, max_gjobs), b.n_reads));
+		msrc.pools = D.pools, msrc.jobq_n = D.jobq_n, msrc.lab_n = lab_n, msrc.prof = D.prof, msrc.tier_hist = D.tier_hist, msrc.peak = sl.W.peak, msrc.n_workers = sl.W.n_workers;
+		mail = (Mail*)sl.h_mail.p;
+	}
+	// list: the reads to run (NULL: all n_list of the batch); T: the timers of the spans (NULL: untimed)
+	void run(const int32_t *list, int32_t n_list, const Workers &W, SlotTimers *T)
+	{
+		auto tk = [&](int s) { return T? &T->k[s] : (EvTimer*)0; };
+		auto tm = [&](EvTimer SlotTimers::*m) { return T? &(T->*m) : (EvTimer*)0; };
+		L.rid_list = list, L.n_work = n_list;
+		{ Span t(tm(&SlotTimers::seed)), k(tk(S_SEED)); launch_stage<S_SEED>(L, W); }
+		{
+			Span t(tm(&SlotTimers::chain)), k(tk(S_CHAIN));
+			dzero(D.rescue_n, sizeof(unsigned int));
+			launch_stage<S_CHAIN>(L, W);
+			L.n_work_dev = D.rescue_n, L.rid_list = 0; // the reads k_chain put on the rescue list (count known on the device only)
+			launch_stage<S_CHAIN_RESCUE>(L, W);
+			L.n_work_dev = 0, L.rid_list = list;
+		}
+		{
+			Span t(tm(&SlotTimers::align));
+			if (lab_n) { // labels of the sources k_chain listed (count known on the device only)
+				L.n_work_dev = lab_n, L.rid_list = 0;
+				Span tl(tm(&SlotTimers::lab));
+				launch_stage<S_LABELS>(L, W);
+				L.n_work_dev = lab_n + 1;
+				launch_stage<S_LABELS_BIG>(L, W);
+				L.n_work_dev = 0, L.rid_list = list;
+			}
+			{
+				Span k(tk(S_GCHAIN));
+				if (list == 0 && n_list >= 1024) { // whole batch: reads with many linear chains first (a few of them set the time of this kernel)
+					make_job_order(L, 2, 0, n_list, order);
+					L.rid_list = order;
+				}
+				launch_stage<S_GCHAIN>(L, W);
+				L.rid_list = list;
+			}
+			// bridging jobs planned by k_gchain, then materialisation
+			count_jobs(D.pools, (int)P_GJOBS, (int)P_JOBS, (unsigned int)gjobs_done, (unsigned int)jobs_done, D.cnt);
+			L.rid_list = 0, L.job_start = gjobs_done, L.n_work = 0, L.n_work_dev = D.cnt;
+			{ Span k(tk(S_GWFA)); make_job_order(L, 0, 0, 0, order, D.cnt); L.rid_list = order; launch_stage<S_GWFA>(L, W); }
+			L.rid_list = list, L.n_work = n_list, L.n_work_dev = 0;
+			{ Span k(tk(S_GCHAIN_GEN)); launch_stage<S_GCHAIN_GEN>(L, W); }
+		}
+		{ // three tiers; a job that does not fit one tier is queued for the next
+			Span t(tm(&SlotTimers::wfa));
+			count_jobs(D.pools, (int)P_GJOBS, (int)P_JOBS, (unsigned int)gjobs_done, (unsigned int)jobs_done, D.cnt);
+			L.c.jobq[0] = jobq, L.c.jobq[1] = jobq + max_jobs;
+			dzero(D.jobq_n, 2 * sizeof(unsigned int));
+			L.rid_list = 0, L.job_start = jobs_done, L.n_work = 0, L.n_work_dev = D.cnt + 1;
+			{ Span k(tk(S_WFA_SMALL)); launch_stage<S_WFA_SMALL>(L, W); }
+			L.n_work_dev = D.jobq_n;
+			{ // longest first: the long gaps, which run on one warp each, start early
+				Span k(tk(S_WFA_MID));
+				make_job_order(L, 1, L.c.jobq[0], 0, order, D.jobq_n);
+				L.rid_list = order;
+				launch_stage<S_WFA_MID>(L, W);
+			}
+			L.rid_list = 0, L.n_work_dev = D.jobq_n + 1;
+			{ Span k(tk(S_WFA_BIG)); make_job_order(L, 1, L.c.jobq[1], 0, order, D.jobq_n + 1); L.rid_list = order; launch_stage<S_WFA_BIG>(L, W); }
+			L.rid_list = 0, L.n_work_dev = 0;
+		}
+		L.rid_list = list, L.n_work = n_list;
+		{ Span t(tm(&SlotTimers::fin)), k(tk(S_FINISH)); launch_stage<S_FINISH>(L, W); }
+		ev_record(sl.ev_last);
+		fetch_mail(msrc, mail); // (also the one wait of the pass)
+		gjobs_done = (int64_t)(std::min<uint64_t>(mail->pools[P_GJOBS].used, mail->pools[P_GJOBS].cap) / sizeof(GwfaJob));
+		jobs_done = (int64_t)(std::min<uint64_t>(mail->pools[P_JOBS].used, mail->pools[P_JOBS].cap) / sizeof(WfaJob));
+	}
+};
+
+// The result blobs of a batch closed up in read order (pack_results), then to the host in pieces, each followed by the event the
+// assembly of its reads waits for.  routs gets the blobs' new places.  Returns the host copy.
+static const char *download_blobs(Model::Slot &sl, int n_reads, ReadOut *routs, const char *d_out, uint64_t out_used, EvTimer &tm_d2h, mgb_stats_t &S)
+{
+	Span span(&tm_d2h);
+	const size_t n = (size_t)n_reads;
+	PackArgs P;
+	P.routs = (ReadOut*)sl.d_routs.p, P.meta = (const ReadMeta*)sl.d_meta.p, P.n = n_reads, P.pool = d_out;
+	P.packed = (char*)sl.d_packed.ensure(out_used + 64), P.off = (uint64_t*)sl.d_packoff.ensure(sizeof(uint64_t) * (n + 1));
+	pack_results(P);
+	d2h(routs, P.routs, sizeof(ReadOut) * n);
+	std::vector<uint64_t> off(n + 1);
+	d2h(off.data(), P.off, sizeof(uint64_t) * (n + 1));
+	char *hout = (char*)sl.h_out.ensure(off[n] + 64);
+	download_in_pieces(sl, n_reads, off.data(), hout, P.packed);
+	S.out_bytes = (int64_t)off[n];
+	return hout;
+}
+
+// Tier-1 routing for the batches to come: the first length bucket in which the sampled gaps mostly ended beyond tier 1
+static void learn_tier_routing(Model *M, const unsigned int *h)
+{
+	int32_t t1 = INT32_MAX;
+	for (int b = 0; b < 32 && t1 == INT32_MAX; ++b) { unsigned int in = h[b * 4 + 1], out = h[b * 4 + 2] + h[b * 4 + 3]; if (in + out >= 8 && in < out) t1 = b * 16; }
+	unsigned int tot = 0;
+	for (int i = 0; i < 128; ++i) tot += h[i];
+	if (tot >= 64) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1; }
 }
 
 // Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).  With gaf, the result is the batch's GAF text
@@ -1514,338 +1903,53 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 {
 	mgb_stats_t &S = sl.st;
 	memset(&S, 0, sizeof(S));
-	sl.ev_first_ms = sl.ev_last_ms = 0;
 	if (n_reads <= 0) return 0;
+	const size_t n = (size_t)n_reads;
 	const int32_t L_skip1 = M->skip1_len; // threshold this batch runs with
-	double t_host0 = now_ms();
-	// ---- pack the sub-batch into page-locked memory ----
-	uint64_t tot = 0;
-	uint64_t *seq_off; int32_t *seq_len; uint32_t *name_hash;
-	{
-		size_t small = (size_t)n_reads * (8 + 4 + 4) + 256;
-		char *hs = (char*)sl.h_small.ensure(small);
-		seq_off = (uint64_t*)hs, seq_len = (int32_t*)(seq_off + n_reads), name_hash = (uint32_t*)(seq_len + n_reads);
-	}
-	for (int i = 0; i < n_reads; ++i) {
-		seq_off[i] = tot, seq_len[i] = qlens[i];
-		tot += (uint64_t)(qlens[i] > 0? qlens[i] : 0) + 8;
-		tot = (tot + 15) & ~(uint64_t)15;
-		name_hash[i] = names && names[i]? hash_str(names[i]) : 0;
-		S.n_bases += qlens[i] > 0? qlens[i] : 0;
-	}
-	S.n_reads = n_reads;
-	const size_t hseq_bytes = tot + 16;
-	char *hseq = (char*)sl.h_seq.ensure(hseq_bytes);
-	auto pfor = [&](int64_t n, const std::function<void(int64_t)> &fn) {
-		if (n < 256 || host_threads <= 1) { for (int64_t i = 0; i < n; ++i) fn(i); return; }
-		sl.host_pool.run(n, host_threads, fn);
-	};
-	// the event pairs live in the slot: creating and destroying three dozen events per call contends on the driver's lock with the other calls in flight
-	if (sl.timers == 0) sl.timers = new SlotTimers();
+	const double t_host0 = now_ms();
+	if (!sl.timers) sl.timers.reset(new SlotTimers());
 	SlotTimers &TM = *sl.timers;
 	TM.reset();
-	EvTimer &tm_h2d = TM.h2d, &tm_seed = TM.seed, &tm_chain = TM.chain, &tm_align = TM.align, &tm_wfa = TM.wfa, &tm_fin = TM.fin, &tm_d2h = TM.d2h, &tm_lab = TM.lab;
-	EvTimer *tm_k = TM.k; // one per kernel (first pass only)
+	const BatchLayout lay(n_reads, qlens);
+	S.n_reads = n_reads, S.n_bases = lay.n_bases;
+	const BatchDev b = upload_batch(sl.stage, lay, M, n_reads, qlens, seqs, names, (o.flag & F_NO_DIAG) != 0, seg_off? seg_off->data() : 0,
+									seg_len? seg_len->data() : 0, sl.host_pool, host_threads, &TM.h2d, S);
 	// ---- device buffers (all persistent: cudaMalloc/cudaFree would serialise the slots) ----
-	enum { P_ANCHOR, P_MINIPOS, P_LCHAIN, P_OUT, P_PLAN, P_JOBS, P_CIG, P_GSTATE, P_GJOBS, P_WALK, N_POOLS };
-	char *d_seq = (char*)sl.d_seq.ensure(hseq_bytes);
-	tm_h2d.start();
-	// The reads go up 2 bits per base (a quarter of the bytes) and k_unpack writes their ASCII copy on the device; a read with any
-	// byte other than A/C/G/T goes up as ASCII, and so does the whole batch when such reads are many or the fragments have segments.
-	uint64_t *pk_off = 0, *d_pk = 0, *d_pk_off = 0;
-	bool packed_mode = seg_off == 0;
-	if (packed_mode) {
-		pk_off = (uint64_t*)sl.h_pk.ensure((size_t)n_reads * 8 + 64 + (size_t)(S.n_bases / 4) + (size_t)n_reads * 16);
-		uint64_t wtot = 0;
-		for (int i = 0; i < n_reads; ++i) { pk_off[i] = wtot; wtot += (uint64_t)((qlens[i] > 0? qlens[i] : 0) + 31) / 32 + 1; }
-		uint64_t *hpk = pk_off + (((size_t)n_reads + 7) & ~(size_t)7);
-		d_pk_off = (uint64_t*)sl.d_pk.ensure(((((size_t)n_reads + 7) & ~(size_t)7) + wtot + 8) * 8);
-		d_pk = d_pk_off + (((size_t)n_reads + 7) & ~(size_t)7);
-		std::vector<uint8_t> raw((size_t)n_reads, 0);
-		const int n_piece = n_reads >= 2048? 4 : 1;
-		double t_pack = 0;
-		for (int pc = 0; pc < n_piece; ++pc) {
-			const int64_t r0 = (int64_t)n_reads * pc / n_piece, r1 = (int64_t)n_reads * (pc + 1) / n_piece;
-			if (r0 >= r1) continue;
-			const double tp0 = now_ms();
-			pfor(r1 - r0, [&](int64_t i) { const int64_t r = r0 + i; if (qlens[r] > 0 && !pack_read(seqs[r], qlens[r], hpk + pk_off[r])) raw[(size_t)r] = 1; });
-			t_pack += now_ms() - tp0;
-			const uint64_t w0 = pk_off[r0], w1 = r1 < n_reads? pk_off[r1] : wtot;
-#ifndef MGB_HOSTSIM
-			CUDA_OK(cudaMemcpyAsync(d_pk + w0, hpk + w0, (w1 - w0) * 8, cudaMemcpyHostToDevice, t_stream));
-#else
-			memcpy(d_pk + w0, hpk + w0, (w1 - w0) * 8);
-#endif
-		}
-		int64_t n_raw = 0;
-		for (int i = 0; i < n_reads; ++i) n_raw += raw[(size_t)i];
-		if (n_raw > 64) packed_mode = false; // not worth a copy per read
-		else {
-			S.t_pack_ms = t_pack;
-			S.h2d_bytes = (int64_t)(wtot * 8);
-			for (int i = 0; i < n_reads; ++i)
-				if (raw[(size_t)i]) {
-					memcpy(hseq + seq_off[i], seqs[i], (size_t)qlens[i]);
-#ifndef MGB_HOSTSIM
-					CUDA_OK(cudaMemcpyAsync(d_seq + seq_off[i], hseq + seq_off[i], (size_t)qlens[i], cudaMemcpyHostToDevice, t_stream));
-#else
-					memcpy(d_seq + seq_off[i], hseq + seq_off[i], (size_t)qlens[i]);
-#endif
-					pk_off[i] = ~0ULL, S.h2d_bytes += qlens[i];
-				}
-			h2d(d_pk_off, pk_off, (size_t)n_reads * 8);
-		}
-	}
-	if (!packed_mode) { // pack and upload in a few pieces: the copy of one piece runs while the host threads pack the next
-		const int n_piece = n_reads >= 2048? 4 : 1;
-		double t_pack = 0;
-		for (int pc = 0; pc < n_piece; ++pc) {
-			const int64_t r0 = (int64_t)n_reads * pc / n_piece, r1 = (int64_t)n_reads * (pc + 1) / n_piece;
-			if (r0 >= r1) continue;
-			const double tp0 = now_ms();
-			pfor(r1 - r0, [&](int64_t i) { if (qlens[r0 + i] > 0) memcpy(hseq + seq_off[r0 + i], seqs[r0 + i], (size_t)qlens[r0 + i]); });
-			t_pack += now_ms() - tp0;
-			const uint64_t b0 = seq_off[r0], b1 = r1 < n_reads? seq_off[r1] : (uint64_t)hseq_bytes;
-#ifndef MGB_HOSTSIM
-			CUDA_OK(cudaMemcpyAsync(d_seq + b0, hseq + b0, b1 - b0, cudaMemcpyHostToDevice, t_stream));
-#else
-			memcpy(d_seq + b0, hseq + b0, b1 - b0);
-#endif
-		}
-		dsync();
-		S.t_pack_ms += t_pack;
-		S.h2d_bytes = (int64_t)hseq_bytes;
-	}
-	size_t small_dev = (size_t)n_reads * (8 + 4 + 4 + 4 + 4 + 4) + 4096 + 1024;
-	char *ds = (char*)sl.d_small.ensure(small_dev);
-	uint64_t *d_seq_off = (uint64_t*)ds;
-	int32_t *d_seq_len = (int32_t*)(d_seq_off + n_reads);
-	uint32_t *d_name_hash = (uint32_t*)(d_seq_len + n_reads);
-	int32_t *d_list_buf = (int32_t*)(d_name_hash + n_reads); // n_reads entries: read list of the retry pass
-	int32_t *d_self_id = d_list_buf + n_reads; // n_reads entries, MG_M_NO_DIAG only
-	int32_t *d_rescue = d_self_id + n_reads; // n_reads entries: reads handed from k_chain to k_chain_rescue
-	char *dsm = (char*)(((uintptr_t)(d_rescue + n_reads) + 255) & ~(uintptr_t)255);
-	unsigned int *d_next = (unsigned int*)dsm;
-	unsigned int *d_jobq_n = d_next + 4;
-	unsigned int *d_rescue_n = d_next + 8;
-	unsigned int *d_cnt = d_next + 10; // [0] bridging jobs, [1] gap jobs the next job kernel has to take
-	unsigned long long *d_prof = (unsigned long long*)(dsm + 64);
-	Pool *d_pools = (Pool*)(dsm + 64 + sizeof(unsigned long long) * PROF_N);
-	unsigned int *d_tier_hist = (unsigned int*)((char*)(d_pools + 16) + 64); // 32 x 4 counters behind the pool headers
-	h2d(d_seq_off, seq_off, (size_t)n_reads * 16); // seq_off, seq_len and name_hash are contiguous on both sides
-	S.h2d_bytes += (int64_t)n_reads * 16;
-	if (packed_mode) {
-		UnpackArgs U;
-		U.pk = d_pk, U.pk_off = d_pk_off, U.seq_off = d_seq_off, U.seq_len = d_seq_len, U.seq = d_seq, U.n_reads = n_reads;
-#ifndef MGB_HOSTSIM
-		k_unpack<<<dev_sm_count() * 8, 256, 0, t_stream>>>(U);
-		CUDA_OK(cudaGetLastError());
-#else
-		for (int r = 0; r < n_reads; ++r) if (pk_off[r] != ~0ULL) for (int64_t wd = 0; wd * 32 < qlens[r]; ++wd) unpack_word(U, r, wd);
-#endif
-		S.n_launches += 1;
-	}
-	tm_h2d.stop();
-	const bool no_diag = (o.flag & F_NO_DIAG) != 0;
-	if (no_diag) {
-		const std::vector<int32_t> self = read_self_ids(M, n_reads, names);
-		h2d(d_self_id, self.data(), sizeof(int32_t) * (size_t)n_reads);
-	}
-	int32_t *d_seg_off = 0, *d_seg_len = 0; // multi-segment fragments only (mg_map_frag with n_segs > 1)
-	if (seg_off && seg_len) {
-		d_seg_off = (int32_t*)sl.d_segs.ensure(sizeof(int32_t) * (seg_off->size() + seg_len->size()));
-		d_seg_len = d_seg_off + seg_off->size();
-		h2d(d_seg_off, seg_off->data(), sizeof(int32_t) * seg_off->size());
-		h2d(d_seg_len, seg_len->data(), sizeof(int32_t) * seg_len->size());
-	}
-	ReadMeta *d_meta = (ReadMeta*)sl.d_meta.ensure(sizeof(ReadMeta) * (size_t)n_reads);
-	ReadOut *d_routs = (ReadOut*)sl.d_routs.ensure(sizeof(ReadOut) * (size_t)n_reads);
-	dzero(d_meta, sizeof(ReadMeta) * (size_t)n_reads);
-	dzero(d_routs, sizeof(ReadOut) * (size_t)n_reads);
-	dzero(d_prof, sizeof(unsigned long long) * PROF_N);
-	dzero(d_tier_hist, sizeof(unsigned int) * 128);
-	uint64_t cap[N_POOLS];
-	cap[P_ANCHOR] = std::max<uint64_t>((uint64_t)S.n_bases / 4 * sizeof(u128), (uint64_t)1 << 22);
-	cap[P_MINIPOS] = std::max<uint64_t>((uint64_t)S.n_bases * sizeof(int32_t) / 2, (uint64_t)1 << 20);
-	cap[P_LCHAIN] = std::max<uint64_t>((uint64_t)n_reads * 64 * sizeof(LChain), (uint64_t)1 << 20);
-	cap[P_OUT] = std::max<uint64_t>((uint64_t)S.n_bases * 4, (uint64_t)1 << 22);
-	cap[P_PLAN] = std::max<uint64_t>((uint64_t)S.n_bases / 8 * 8, (uint64_t)1 << 20);
-	cap[P_JOBS] = std::max<uint64_t>((uint64_t)S.n_bases / 40 * sizeof(WfaJob), (uint64_t)1 << 20);
-	cap[P_CIG] = std::max<uint64_t>((uint64_t)S.n_bases, (uint64_t)1 << 20) + (uint64_t)sl.W.n_workers * CIG_CHUNK_BYTES * 4; // + the unused ends of the warps' slices (three tier kernels per pass)
-	cap[P_GSTATE] = std::max<uint64_t>((uint64_t)n_reads * 2048, (uint64_t)1 << 20);
-	cap[P_GJOBS] = std::max<uint64_t>((uint64_t)n_reads * 24 * sizeof(GwfaJob), (uint64_t)1 << 20);
-	cap[P_WALK] = std::max<uint64_t>((uint64_t)n_reads * 256, (uint64_t)1 << 20);
+	const PassScratch D(sl.d_scratch, n_reads);
+	void *d_meta = sl.d_meta.ensure(sizeof(ReadMeta) * n), *d_routs = sl.d_routs.ensure(sizeof(ReadOut) * n);
+	dzero(d_meta, sizeof(ReadMeta) * n);
+	dzero(d_routs, sizeof(ReadOut) * n);
+	dzero(D.prof, sizeof(unsigned long long) * PROF_N);
+	dzero(D.tier_hist, sizeof(unsigned int) * 128);
+	std::array<uint64_t, N_POOLS> cap = pool_caps(n_reads, lay.n_bases, sl.W.n_workers);
 	for (int i = 0; i < N_POOLS; ++i) if (sl.d_pool[i].cap > cap[i]) cap[i] = sl.d_pool[i].cap & ~(size_t)4095; // keep what earlier batches needed
-	ReadOut *routs = (ReadOut*)sl.h_routs.ensure((sizeof(ReadOut) + sizeof(ReadMeta)) * (size_t)n_reads + 64); // page-locked: a pageable destination makes the copy a blocking, staged one
+	ReadOut *routs = (ReadOut*)sl.h_routs.ensure((sizeof(ReadOut) + sizeof(ReadMeta)) * n + 64); // page-locked: a pageable destination makes the copy a blocking, staged one
 	ReadMeta *meta = (ReadMeta*)(routs + n_reads);
-	char *hout = 0;
-	int rc_final = 0, n_piece = 1;
-	std::vector<uint64_t> pack_off;
-	const char *d_out_pool = 0; // the output pool of the last attempt: the GAF path formats from it
-	bool first_kernel = true;
-	(void)first_kernel;
-
 	const bool use_lab = p_lab_cache && lab_prepare(M, o.bw_long);
-	int32_t *d_lab_new = 0; unsigned int *d_lab_n = 0; // this call's list of sources to search
 	Mail *mail = (Mail*)sl.h_mail.ensure(sizeof(Mail));
-	if (use_lab) { d_lab_n = (unsigned int*)sl.d_lab_new.ensure(((size_t)M->g.n_seg * 2 + 4) * sizeof(int32_t)); d_lab_new = (int32_t*)(d_lab_n + 4); }
-	MailSrc msrc;
-	msrc.pools = d_pools, msrc.jobq_n = d_jobq_n, msrc.lab_n = d_lab_n, msrc.prof = d_prof, msrc.tier_hist = d_tier_hist, msrc.peak = sl.W.peak, msrc.n_workers = sl.W.n_workers;
-	for (int attempt = 0; attempt < 8; ++attempt) {
-		void *d_buf[N_POOLS];
-		Pool hp[N_POOLS];
-		for (int i = 0; i < N_POOLS; ++i) d_buf[i] = sl.d_pool[i].ensure(cap[i]), hp[i].used = 0, hp[i].cap = cap[i];
-		h2d(d_pools, hp, sizeof(hp));
-		dfill(d_buf[P_GJOBS], 0xff, cap[P_GJOBS]); // reserved-but-unused bridging job slots read as rid == -1
-		dfill(d_buf[P_JOBS], 0xff, cap[P_JOBS]);   // the same for gap jobs: slots of an allocation that overflowed the pool are never written
-		LaunchArgs L;
-		memset(&L, 0, sizeof(L));
-		L.c.g = M->g, L.c.ix = M->ix, L.c.opt = o;
-		L.c.b.n_reads = n_reads, L.c.b.seq = d_seq, L.c.b.seq_off = d_seq_off, L.c.b.seq_len = d_seq_len, L.c.b.name_hash = d_name_hash;
-		L.c.b.seg_off = d_seg_off, L.c.b.seg_len = d_seg_len, L.c.b.self_id = no_diag? d_self_id : 0;
-		L.c.b.pk = packed_mode? d_pk : 0, L.c.b.pk_off = packed_mode? d_pk_off : 0;
-		L.c.meta = d_meta;
-		L.c.pool_anchor = &d_pools[P_ANCHOR], L.c.anchor = (u128*)d_buf[P_ANCHOR];
-		L.c.pool_minipos = &d_pools[P_MINIPOS], L.c.minipos = (int32_t*)d_buf[P_MINIPOS];
-		L.c.pool_lchain = &d_pools[P_LCHAIN], L.c.lchain = (LChain*)d_buf[P_LCHAIN];
-		L.c.pool_out = &d_pools[P_OUT], L.c.out = (char*)d_buf[P_OUT];
-		L.c.pool_plan = &d_pools[P_PLAN], L.c.plan = (uint64_t*)d_buf[P_PLAN];
-		L.c.pool_jobs = &d_pools[P_JOBS], L.c.jobs = (WfaJob*)d_buf[P_JOBS];
-		L.c.pool_cig = &d_pools[P_CIG], L.c.cig = (uint32_t*)d_buf[P_CIG];
-		L.c.pool_gstate = &d_pools[P_GSTATE], L.c.gstate = (char*)d_buf[P_GSTATE];
-		L.c.pool_gjobs = &d_pools[P_GJOBS], L.c.gjobs = (GwfaJob*)d_buf[P_GJOBS];
-		L.c.pool_walk = &d_pools[P_WALK], L.c.walk = (int32_t*)d_buf[P_WALK];
-		L.c.next_read = d_next;
-		L.c.rescue_list = d_rescue, L.c.rescue_n = d_rescue_n;
-		memset(&L.c.lab, 0, sizeof(L.c.lab));
-		if (use_lab) {
-			L.c.lab.src_off = M->d_lab_off, L.c.lab.pool_hdr = M->d_lab_hdr, L.c.lab.pool = M->d_lab_pool, L.c.lab.new_src = d_lab_new, L.c.lab.n_new = d_lab_n;
-			L.c.lab.max_dist_g = M->lab_max_dist_g, L.c.lab.cap_new = M->g.n_seg * 2;
-			dzero(d_lab_n, 2 * sizeof(unsigned int));
-		}
-		L.c.prof = d_prof;
-		L.c.tier_hist = d_tier_hist, L.c.skip1_len = L_skip1;
-		L.c.jobq[0] = 0, L.c.jobq[1] = 0, L.c.jobq_n = d_jobq_n;
-		L.routs = d_routs;
-		int64_t jobs_done = 0, gjobs_done = 0;
-		const int64_t max_jobs = (int64_t)(cap[P_JOBS] / sizeof(WfaJob)) + 1, max_gjobs = (int64_t)(cap[P_GJOBS] / sizeof(GwfaJob)) + 1;
-		int32_t *jobq_buf = (int32_t*)sl.d_jobq.ensure(sizeof(int32_t) * 2 * (size_t)max_jobs);
-		int32_t *order_buf = (int32_t*)sl.d_order.ensure(sizeof(int32_t) * (size_t)std::max<int64_t>(std::max<int64_t>(max_jobs, max_gjobs), n_reads));
-		// one pass over a set of reads; job counts are read back between the planning and the job kernels
-		auto run_pass = [&](const int32_t *d_list, int32_t n_list, const Workers &W, bool timed) {
-			L.rid_list = d_list, L.n_work = n_list;
-#ifndef MGB_HOSTSIM
-			if (first_kernel) { CUDA_OK(cudaEventRecord(sl.ev_first, t_stream)); first_kernel = false; }
-#endif
-			if (timed) tm_seed.start();
-			{ if (timed) tm_k[S_SEED].start(); launch_stage<S_SEED>(L, W); if (timed) tm_k[S_SEED].stop(); }
-			if (timed) tm_seed.stop(), tm_chain.start();
-			{
-				if (timed) tm_k[S_CHAIN].start();
-				dzero(d_rescue_n, sizeof(unsigned int));
-				launch_stage<S_CHAIN>(L, W);
-				L.n_work_dev = d_rescue_n, L.rid_list = 0; // the reads k_chain put on the rescue list (count known on the device only)
-				launch_stage<S_CHAIN_RESCUE>(L, W);
-				L.n_work_dev = 0, L.rid_list = d_list;
-				if (timed) tm_k[S_CHAIN].stop();
-				S.n_launches += 1;
-			}
-			if (timed) tm_chain.stop(), tm_align.start();
-			if (use_lab) { // labels of the sources k_chain listed (count known on the device only)
-				L.n_work_dev = d_lab_n, L.rid_list = 0;
-				if (timed) tm_lab.start();
-				launch_stage<S_LABELS>(L, W);
-				L.n_work_dev = d_lab_n + 1;
-				launch_stage<S_LABELS_BIG>(L, W);
-				if (timed) tm_lab.stop();
-				L.n_work_dev = 0, L.rid_list = d_list;
-				S.n_launches += 2;
-			}
-			if (d_list == 0 && n_list >= 1024) { // whole batch: reads with many linear chains first (a few of them set the time of this kernel)
-				if (timed) tm_k[S_GCHAIN].start();
-				make_job_order(L, 2, 0, n_list, order_buf);
-				L.rid_list = order_buf;
-				launch_stage<S_GCHAIN>(L, W);
-				L.rid_list = d_list;
-				if (timed) tm_k[S_GCHAIN].stop();
-				S.n_launches += 1;
-			} else { if (timed) tm_k[S_GCHAIN].start(); launch_stage<S_GCHAIN>(L, W); if (timed) tm_k[S_GCHAIN].stop(); }
-			auto counts = [&]() {
-#ifndef MGB_HOSTSIM
-				k_job_counts<<<1, 1, 0, t_stream>>>(d_pools, (int)P_GJOBS, (int)P_JOBS, (unsigned int)gjobs_done, (unsigned int)jobs_done, d_cnt);
-				CUDA_OK(cudaGetLastError());
-#else
-				job_counts(d_pools, (int)P_GJOBS, (int)P_JOBS, (unsigned int)gjobs_done, (unsigned int)jobs_done, d_cnt);
-#endif
-			};
-			// From here on every kernel reads its number of units on the device: the whole pass is queued without a host round trip, so
-			// nothing another thread does in the driver (large copies, blocking waits) can open gaps between its kernels.
-			{ // bridging jobs planned by k_gchain, then materialisation
-				counts();
-				L.rid_list = 0, L.job_start = gjobs_done, L.n_work = 0, L.n_work_dev = d_cnt;
-				if (timed) tm_k[S_GWFA].start();
-				make_job_order(L, 0, 0, 0, order_buf, d_cnt);
-				L.rid_list = order_buf;
-				launch_stage<S_GWFA>(L, W);
-				if (timed) tm_k[S_GWFA].stop();
-				L.rid_list = d_list, L.n_work = n_list, L.n_work_dev = 0;
-				{ if (timed) tm_k[S_GCHAIN_GEN].start(); launch_stage<S_GCHAIN_GEN>(L, W); if (timed) tm_k[S_GCHAIN_GEN].stop(); }
-				S.n_launches += 4;
-			}
-			if (timed) tm_align.stop();
-			if (timed) tm_wfa.start();
-			{ // three tiers; a job that does not fit one tier is queued for the next
-				counts();
-				L.c.jobq[0] = jobq_buf, L.c.jobq[1] = jobq_buf + max_jobs;
-				dzero(d_jobq_n, 2 * sizeof(unsigned int));
-				L.rid_list = 0, L.job_start = jobs_done, L.n_work = 0, L.n_work_dev = d_cnt + 1;
-				{ if (timed) tm_k[S_WFA_SMALL].start(); launch_stage<S_WFA_SMALL>(L, W); if (timed) tm_k[S_WFA_SMALL].stop(); }
-				L.n_work_dev = d_jobq_n;
-				if (timed) tm_k[S_WFA_MID].start();
-				make_job_order(L, 1, L.c.jobq[0], 0, order_buf, d_jobq_n); // longest first: the long gaps, which run on one warp each, start early
-				L.rid_list = order_buf;
-				launch_stage<S_WFA_MID>(L, W);
-				if (timed) tm_k[S_WFA_MID].stop();
-				L.rid_list = 0, L.n_work_dev = d_jobq_n + 1;
-				if (timed) tm_k[S_WFA_BIG].start();
-				make_job_order(L, 1, L.c.jobq[1], 0, order_buf, d_jobq_n + 1);
-				L.rid_list = order_buf;
-				launch_stage<S_WFA_BIG>(L, W);
-				if (timed) tm_k[S_WFA_BIG].stop();
-				L.rid_list = 0, L.n_work_dev = 0;
-				S.n_launches += 6;
-			}
-			if (timed) tm_wfa.stop(), tm_fin.start();
-			L.rid_list = d_list, L.n_work = n_list;
-			{ if (timed) tm_k[S_FINISH].start(); launch_stage<S_FINISH>(L, W); if (timed) tm_k[S_FINISH].stop(); }
-			if (timed) tm_fin.stop();
-			S.n_launches += 4;
-#ifndef MGB_HOSTSIM
-			CUDA_OK(cudaEventRecord(sl.ev_last, t_stream));
-#endif
-			fetch_mail(msrc, mail); // (also the one wait of the pass)
-			gjobs_done = (int64_t)(std::min<uint64_t>(mail->pools[P_GJOBS].used, mail->pools[P_GJOBS].cap) / sizeof(GwfaJob));
-			jobs_done = (int64_t)(std::min<uint64_t>(mail->pools[P_JOBS].used, mail->pools[P_JOBS].cap) / sizeof(WfaJob));
-			if (timed) S.n_jobs_mid = mail->jobq_n[0], S.n_jobs_big = mail->jobq_n[1];
-		};
+	unsigned int *lab_n = use_lab? (unsigned int*)sl.d_lab_new.ensure(((size_t)M->g.n_seg * 2 + 4) * sizeof(int32_t)) : 0; // 2 counts, then the list
+	const char *hout = 0, *d_out = 0; // the host copy of the blobs; the output pool of the last attempt (the GAF path formats from it)
+	int rc = 0;
+	for (int attempt = 0;; ++attempt) {
+		Pass P(M, sl, o, b, D, cap, lab_n, L_skip1);
 		{
 			const double tq = now_ms();
 			if (attempt == 0) S.w_upload_ms = tq - t_host0;
 			std::lock_guard<std::mutex> gpu(M->gpu_mutex);
 			const double tw = now_ms();
 			S.w_gpu_wait_ms += tw - tq;
-			run_pass(0, n_reads, sl.W, true);
+			if (attempt == 0) ev_record(sl.ev_first);
+			P.run(0, n_reads, sl.W, &TM);
 			S.w_pass_ms += now_ms() - tw;
 		}
-		S.n_jobs = jobs_done;
-		d2h(routs, d_routs, sizeof(ReadOut) * (size_t)n_reads);
-		d2h(meta, d_meta, sizeof(ReadMeta) * (size_t)n_reads);
-
+		S.n_jobs = P.jobs_done, S.n_jobs_mid = mail->jobq_n[0], S.n_jobs_big = mail->jobq_n[1];
+		d2h(routs, P.L.routs, sizeof(ReadOut) * n);
+		d2h(meta, P.L.c.meta, sizeof(ReadMeta) * n);
 		// reads whose worker arena overflowed: run them again with large arenas and few workers (shared by the slots)
 		std::vector<int32_t> redo;
 		bool pool_full = false;
 		for (int i = 0; i < n_reads; ++i) {
-			int st = meta[i].status < 0? meta[i].status : routs[i].status;
+			const int st = read_status(meta[i], routs[i]);
 			if (st == MGB_E_ARENA) redo.push_back(i);
 			else if (st == MGB_E_POOL) pool_full = true;
 		}
@@ -1854,124 +1958,64 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 			uint64_t big = (uint64_t)p_arena_big_mb << 20;
 			int nw = (int)std::min<uint64_t>(16, std::max<uint64_t>(1, dev_free_mem() / 2 / big)); // a handful of reads per batch at most come here
 			if (M->Wbig.arena == 0 || M->Wbig.arena_bytes != big) ensure_workers(M->Wbig, std::max(1, nw), big);
-			h2d(d_list_buf, redo.data(), redo.size() * sizeof(int32_t));
-			{ std::lock_guard<std::mutex> gpu(M->gpu_mutex); const double tw = now_ms(); run_pass(d_list_buf, (int32_t)redo.size(), M->Wbig, false); S.w_redo_ms += now_ms() - tw; }
+			h2d(D.list, redo.data(), redo.size() * sizeof(int32_t));
+			{ std::lock_guard<std::mutex> gpu(M->gpu_mutex); const double tw = now_ms(); P.run(D.list, (int32_t)redo.size(), M->Wbig, 0); S.w_redo_ms += now_ms() - tw; }
 			S.n_retry += (int64_t)redo.size();
-			d2h(routs, d_routs, sizeof(ReadOut) * (size_t)n_reads);
-			d2h(meta, d_meta, sizeof(ReadMeta) * (size_t)n_reads);
-			for (int i = 0; i < n_reads; ++i) {
-				int st = meta[i].status < 0? meta[i].status : routs[i].status;
-				if (st == MGB_E_POOL) pool_full = true;
-			}
+			d2h(routs, P.L.routs, sizeof(ReadOut) * n);
+			d2h(meta, P.L.c.meta, sizeof(ReadMeta) * n);
+			for (int i = 0; i < n_reads; ++i) if (read_status(meta[i], routs[i]) == MGB_E_POOL) pool_full = true;
 		}
-		fetch_mail(msrc, mail);
-		memcpy(hp, mail->pools, sizeof(hp));
-		if (use_lab) { unsigned int nn[2] = {mail->lab_n[0], mail->lab_n[1]}; S.n_lab_new = (int64_t)nn[0], S.n_lab_big = (int64_t)nn[1]; lab_after_batch(M, nn[0]); }
-		bool done = !pool_full;
-		d_out_pool = (const char*)d_buf[P_OUT];
-		if (done && !gaf) { // blobs into read order, then to the host in pieces (the assembly below follows piece by piece)
-			tm_d2h.start();
-			const size_t pool_bytes = (size_t)std::min<uint64_t>(hp[P_OUT].used, cap[P_OUT]);
-			PackArgs P;
-			P.routs = d_routs, P.meta = d_meta, P.n = n_reads, P.pool = (const char*)d_buf[P_OUT];
-			P.packed = (char*)sl.d_packed.ensure(pool_bytes + 64), P.off = (uint64_t*)sl.d_packoff.ensure(sizeof(uint64_t) * ((size_t)n_reads + 1));
-			pack_results(P);
-			S.n_launches += 2;
-			d2h(routs, d_routs, sizeof(ReadOut) * (size_t)n_reads);
-			pack_off.resize((size_t)n_reads + 1);
-			d2h(pack_off.data(), P.off, sizeof(uint64_t) * ((size_t)n_reads + 1));
-			const size_t out_bytes = (size_t)pack_off[n_reads];
-			hout = (char*)sl.h_out.ensure(out_bytes + 64);
-			n_piece = n_reads >= 2048? 4 : 1;
-			for (int pc = 0; pc < n_piece; ++pc) {
-				const int64_t r0 = (int64_t)n_reads * pc / n_piece, r1 = (int64_t)n_reads * (pc + 1) / n_piece;
-				const uint64_t b0 = pack_off[r0], b1 = pack_off[r1];
-#ifndef MGB_HOSTSIM
-				if (b1 > b0) CUDA_OK(cudaMemcpyAsync(hout + b0, P.packed + b0, b1 - b0, cudaMemcpyDeviceToHost, t_stream));
-				CUDA_OK(cudaEventRecord(sl.ev_piece[pc], t_stream));
-#else
-				if (b1 > b0) memcpy(hout + b0, P.packed + b0, b1 - b0);
-#endif
-			}
-			tm_d2h.stop();
-			S.out_bytes = (int64_t)out_bytes;
+		fetch_mail(P.msrc, mail);
+		if (use_lab) { S.n_lab_new = (int64_t)mail->lab_n[0], S.n_lab_big = (int64_t)mail->lab_n[1]; lab_after_batch(M, mail->lab_n[0]); }
+		d_out = P.L.c.out;
+		if (!pool_full) { // blobs into read order, then to the host in pieces (the assembly below follows piece by piece)
+			if (!gaf) hout = download_blobs(sl, n_reads, routs, d_out, std::min<uint64_t>(mail->pools[P_OUT].used, cap[P_OUT]), TM.d2h, S);
+			break;
 		}
-		if (done) break;
 		// grow whatever overflowed (used counts keep growing past cap, so they tell how much was wanted)
-		for (int i = 0; i < N_POOLS; ++i) if (hp[i].used > cap[i]) cap[i] = (hp[i].used * 3 / 2 + 4095) & ~(uint64_t)4095;
-		if (attempt == 7) { set_error("output pools kept overflowing"); rc_final = -2; }
+		for (int i = 0; i < N_POOLS; ++i) if (mail->pools[i].used > cap[i]) cap[i] = (mail->pools[i].used * 3 / 2 + 4095) & ~(uint64_t)4095;
+		if (attempt == 7) { set_error("output pools kept overflowing"); rc = -2; break; }
 	}
-	S.t_h2d_ms = tm_h2d.ms(), S.t_seed_ms = tm_seed.ms(), S.t_chain_ms = tm_chain.ms(), S.t_align_ms = tm_align.ms();
-	S.t_wfa_ms = tm_wfa.ms(), S.t_finish_ms = tm_fin.ms();
-	for (int i = 0; i < 10; ++i) S.t_kernel_ms[i] = tm_k[i].ms();
-	S.t_lab_ms = tm_lab.ms();
+	TM.to_stats(S);
 	S.arena_peak = mail->arena_peak; // (the mailbox was last filled after the last pass of the batch)
 	for (int i = 0; i < 32; ++i) S.prof[i] = (uint64_t)mail->prof[i];
-	{ // tier-1 routing for the next batch: the first length bucket in which the sampled gaps mostly ended beyond tier 1
-		const unsigned int *h = mail->tier_hist;
-		int32_t t1 = INT32_MAX;
-		for (int b = 0; b < 32 && t1 == INT32_MAX; ++b) { unsigned int in = h[b * 4 + 1], out = h[b * 4 + 2] + h[b * 4 + 3]; if (in + out >= 8 && in < out) t1 = b * 16; }
-		unsigned int tot = 0;
-		for (int i = 0; i < 128; ++i) tot += h[i];
-		if (tot >= 64) { std::lock_guard<std::mutex> lock(M->big_mutex); M->skip1_len = t1; }
-		S.skip1_len = L_skip1, S.skip2_len = INT32_MAX; // every gap that fits tier 2's lengths is aligned there
-	}
-	if (rc_final < 0) return rc_final;
+	learn_tier_routing(M, mail->tier_hist);
+	S.skip1_len = L_skip1, S.skip2_len = INT32_MAX; // every gap that fits tier 2's lengths is aligned there
+	if (rc < 0) return rc;
 
 	// ---- results ----
-	double t_asm0 = now_ms();
+	const double t_asm0 = now_ms();
 	S.w_download_ms = t_asm0 - t_host0 - S.w_upload_ms - S.w_pass_ms - S.w_redo_ms - S.w_gpu_wait_ms;
-	int first_bad = -1;
 	for (int i = 0; i < n_reads; ++i) {
-		int st = meta[i].status < 0? meta[i].status : routs[i].status;
-		if (st < 0) { first_bad = i; break; }
+		const int st = read_status(meta[i], routs[i]);
+		if (st < 0) {
+			char buf[256];
+			snprintf(buf, sizeof(buf), "read '%s' (%d bp) failed on the device with code %d%s", names && names[i]? names[i] : "", qlens[i], st,
+					 st == MGB_E_ARENA? " (worker arena exhausted even in the retry pass; raise arena_big_mb)" : "");
+			set_error(buf);
+			return st;
+		}
 		S.n_seeds += meta[i].n_seed0, S.n_anchors_out += meta[i].n_a, S.n_chains_out += meta[i].n_u0, S.n_minimizers += meta[i].n_mz;
 	}
-	if (first_bad >= 0) {
-		int i = first_bad, st = meta[i].status < 0? meta[i].status : routs[i].status;
-		char buf[256];
-		snprintf(buf, sizeof(buf), "read '%s' (%d bp) failed on the device with code %d%s", names && names[i]? names[i] : "", qlens[i], st,
-				 st == MGB_E_ARENA? " (worker arena exhausted even in the retry pass; raise arena_big_mb)" : "");
-		set_error(buf);
-		return st;
-	}
 	if (gaf) {
-		const int rc = gaf_text(M, sl, *gaf, n_reads, qlens, names, routs, d_routs, d_out_pool, host_threads, S, tm_d2h);
-		S.t_d2h_ms = tm_d2h.ms(); // the GAF kernels + the pieces of the copy
+		rc = gaf_text(M, sl, *gaf, n_reads, qlens, names, routs, (const ReadOut*)sl.d_routs.p, d_out, host_threads, S, TM.d2h);
+		S.t_d2h_ms = TM.d2h.ms(); // the GAF kernels + the pieces of the copy
 		S.t_host_ms = now_ms() - t_host0;
 		return rc;
 	}
-	for (int pc = 0; pc < n_piece; ++pc) {
-		const int64_t r0 = (int64_t)n_reads * pc / n_piece, r1 = (int64_t)n_reads * (pc + 1) / n_piece;
-#ifndef MGB_HOSTSIM
-		CUDA_OK(cudaEventSynchronize(sl.ev_piece[pc]));
-#endif
-		pfor(r1 - r0, [&](int64_t k) {
-			const int64_t i = r0 + k;
-			int st = meta[i].status < 0? meta[i].status : routs[i].status;
-			if (st == 1) gcs[i] = 0; // empty or over-long read: reference returns before allocating (map-algo.c:359-360)
-			else gcs[i] = build_result(routs[i], hout);
+	const Pieces pcs(n_reads);
+	for (int pc = 0; pc < pcs.n; ++pc) {
+		const int64_t r0 = pcs.r0(pc);
+		ev_wait(sl.ev_piece[pc]);
+		pfor(sl.host_pool, host_threads, pcs.r0(pc + 1) - r0, [&](int64_t k) {
+			const int64_t i = r0 + k; // an empty or over-long read (status 1): the reference returns before allocating (map-algo.c:359-360)
+			gcs[i] = read_status(meta[i], routs[i]) == 1? 0 : build_result(routs[i], hout);
 		});
 	}
 	S.t_asm_ms = now_ms() - t_asm0;
-	S.t_d2h_ms = tm_d2h.ms(); // pack kernels + the pieces of the copy (they overlap the assembly above)
+	S.t_d2h_ms = TM.d2h.ms(); // pack kernels + the pieces of the copy (they overlap the assembly above)
 	S.t_host_ms = now_ms() - t_host0;
 	return 0;
-}
-
-static void slot_prepare(Model *M, Model::Slot &sl, int n_workers)
-{
-#ifndef MGB_HOSTSIM
-	if (!sl.ready) {
-		CUDA_OK(cudaStreamCreateWithFlags(&sl.stream, cudaStreamNonBlocking));
-		CUDA_OK(cudaEventCreate(&sl.ev_first));
-		CUDA_OK(cudaEventCreate(&sl.ev_last));
-		for (int i = 0; i < 4; ++i) CUDA_OK(cudaEventCreateWithFlags(&sl.ev_piece[i], cudaEventDisableTiming));
-	}
-#endif
-	sl.ready = true;
-	ensure_workers(sl.W, n_workers, (uint64_t)p_arena_mb << 20);
-	(void)M;
 }
 
 static thread_local mgb_stats_t t_last_stats; // of the last batch mapped by the calling thread
@@ -1999,15 +2043,9 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 	}
 	Model::Slot &sl = M->slots[k];
 	const double t_slot = now_ms();
-#ifndef MGB_HOSTSIM
-	cudaSetDevice(M->device);
-#endif
 	int rc = 0;
 	try {
 		slot_prepare(M, sl, p_slot_workers > 0? (int)p_slot_workers : default_workers());
-#ifndef MGB_HOSTSIM
-		t_stream = sl.stream;
-#endif
 		MapOptDev o;
 		fill_opt(o, opt, M->k);
 		{ // glibc logf table for mapq (reference: gcmisc.c:216-217); grown under the lock, old copies are kept until the model dies
@@ -2024,23 +2062,16 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		}
 		int nt = (int)p_host_threads;
 		if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
+		t_launches = 0;
 		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf);
-#ifndef MGB_HOSTSIM
-		t_stream = 0; // the slot's stream dies with the model; later calls on this thread (mg_index of another graph) use the default one
-#endif
 	} catch (const MgbError &e) {
 		rc = e.code;
-#ifndef MGB_HOSTSIM
-		t_stream = 0;
-#endif
 	}
+	dev_bind(M->device, 0); // the slot's stream dies with the model; later calls on this thread (mg_index of another graph) use the default one
 	mgb_stats_t S = sl.st;
+	S.n_launches = t_launches;
 	S.w_slot_wait_ms = t_slot - t0;
-#ifndef MGB_HOSTSIM
-	if (rc == 0 && sl.ready) { float a = 0; if (cudaEventElapsedTime(&a, sl.ev_first, sl.ev_last) == cudaSuccess) S.t_dev_span_ms = a; }
-#else
-	S.t_dev_span_ms = S.t_seed_ms + S.t_chain_ms + S.t_align_ms + S.t_wfa_ms + S.t_finish_ms;
-#endif
+	if (rc == 0) S.t_dev_span_ms = ev_ms(sl.ev_first, sl.ev_last);
 	S.n_slots = k;
 	S.t_host_ms = now_ms() - t0;
 	t_last_stats = S, t_has_stats = true;
@@ -2050,11 +2081,8 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		M->slot_busy[k] = false, --M->in_flight;
 	}
 	M->slot_cv.notify_all();
-	if (rc < 0) { // no partial results are left behind
-		for (int i = 0; i < n_reads; ++i) if (gcs[i]) { mg_gchain_free(gcs[i]); gcs[i] = 0; }
-		return rc;
-	}
-	return 0;
+	if (rc < 0) mgb_free_batch(n_reads, gcs); // no partial results are left behind
+	return rc;
 }
 
 // The batch on every device of the index: contiguous parts of about equal bases, one host thread per device, results in input order.
@@ -2106,10 +2134,8 @@ static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, con
 			gaf->len = tot;
 		}
 	}
-	if (rc < 0) for (int i = 0; i < n_reads; ++i) if (gcs[i]) { mg_gchain_free(gcs[i]); gcs[i] = 0; } // no partial results are left behind
-#ifndef MGB_HOSTSIM
-	cudaSetDevice(M->device);
-#endif
+	if (rc < 0) mgb_free_batch(n_reads, gcs); // no partial results are left behind
+	dev_bind(M->device, 0);
 	return rc;
 }
 
@@ -2221,15 +2247,10 @@ extern "C" void mg_map_frag(const mg_idx_t *gi, int n_segs, const int *qlens, co
 	for (int i = 0; i < n_segs; ++i) gcs[i] = 0;
 	if (n_segs <= 0) return;
 	if (n_segs != 1) { // reference: map-algo.c:356-360,366,457-464: one result for the concatenated fragment, no CIGAR
-		if (n_segs > 255) return; // MG_MAX_SEG
-		std::string cat;
-		std::vector<int32_t> seg_off(2), seg_len((size_t)n_segs);
-		for (int i = 0; i < n_segs; ++i) { seg_len[(size_t)i] = qlens[i] > 0? qlens[i] : 0; if (qlens[i] > 0) cat.append(seqs[i], (size_t)qlens[i]); }
-		seg_off[0] = 0, seg_off[1] = n_segs;
-		if (cat.empty()) return;
-		const int qlen_sum = (int)cat.size();
-		const char *sq = cat.data(), *nm1 = qname;
-		if (map_batch_impl(gi, 1, &qlen_sum, &sq, &nm1, gcs, opt, &seg_off, &seg_len) < 0) abort();
+		FragBatch fb(1, &n_segs, qlens, seqs);
+		if (fb.qsum[0] == 0) return; // (also more than MG_MAX_SEG segments)
+		const char *nm1 = qname;
+		if (map_batch_impl(gi, 1, fb.qsum.data(), fb.sq.data(), &nm1, gcs, opt, &fb.seg_off, &fb.seg_len) < 0) abort();
 		return;
 	}
 	const char *nm = qname;
@@ -2707,13 +2728,10 @@ static int test_sketch_impl(int k, int w, int n, const char *seq, const int64_t 
 	}
 	if (n == 0) return 0;
 	if (int e = test_no_device()) return e;
+	const BatchLayout lay(n, len); // the words as a batch lays them out
 	std::vector<int64_t> pk_off((size_t)n);
-	std::vector<uint64_t> hpk;
-	for (int i = 0; i < n; ++i) { // the words of the batch upload (map_range): one more than the bases need
-		pk_off[(size_t)i] = (int64_t)hpk.size();
-		hpk.resize(hpk.size() + (size_t)(len[i] + 31) / 32 + 1, 0);
-		if (!pack_read(seq + off[i], len[i], hpk.data() + pk_off[(size_t)i])) pk_off[(size_t)i] = -1;
-	}
+	std::vector<uint64_t> hpk(lay.n_words);
+	for (int i = 0; i < n; ++i) pk_off[(size_t)i] = pack_read(seq + off[i], len[i], hpk.data() + lay.pk_off[(size_t)i])? (int64_t)lay.pk_off[(size_t)i] : -1;
 	auto seq_d = upload(seq, test_seq_bytes(n, off, len));
 	auto off_d = upload(off, n), pk_off_d = upload(pk_off.data(), n), mz_off_d = upload(mz_off, (size_t)n + 1);
 	auto len_d = upload(len, n);
@@ -2737,9 +2755,9 @@ extern "C" int mgb_test_sketch(int k, int w, int n, const char *seq, const int64
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// test hook: stage_seed() itself on a batch packed as mg_map_batch packs it (the 2-bit words of every read that is all A/C/G/T;
-// fragments of several segments as ASCII only), with the graph and index of gi and the options flag, occ_max1 and max_qlen,
-// launched as k_seed is (test_launch).  The seeds and mini_pos of each read are read back from the pools.
+// test hook: stage_seed() itself on a batch uploaded as mg_map_batch uploads it (upload_batch), with the graph and index of gi and
+// the options flag, occ_max1 and max_qlen, launched as k_seed is (test_launch).  The seeds and mini_pos of each read are read back
+// from the pools.
 // ---------------------------------------------------------------------------------------------------------------
 struct TestSeed {
 	PipeCtx c;
@@ -2774,43 +2792,21 @@ static int test_seed_impl(const mg_idx_t *gi, int n, const int *qlens, const cha
 	if (n == 0) return 0;
 	const Model *M = model_of(gi);
 	if (int e = test_no_device(M->device)) return e;
-	// the batch as map_range lays it out: ASCII with slack, 2-bit words per read (pk_off ~0: the read has other letters)
-	std::vector<uint64_t> seq_off((size_t)n), pk_off((size_t)n), hpk;
-	std::vector<uint32_t> name_hash((size_t)n);
-	uint64_t tot = 0;
-	int64_t n_bases = 0;
-	for (int i = 0; i < n; ++i) {
-		seq_off[(size_t)i] = tot, tot = (tot + (uint64_t)qlens[i] + 8 + 15) & ~(uint64_t)15;
-		name_hash[(size_t)i] = names && names[i]? hash_str(names[i]) : 0;
-		pk_off[(size_t)i] = hpk.size();
-		hpk.resize(hpk.size() + (size_t)(qlens[i] + 31) / 32 + 1, 0);
-		if (qlens[i] > 0 && !pack_read(seqs[i], qlens[i], hpk.data() + pk_off[(size_t)i])) pk_off[(size_t)i] = ~0ULL;
-		n_bases += qlens[i];
-	}
-	std::vector<char> hseq((size_t)tot + 16, 0);
-	for (int i = 0; i < n; ++i) if (qlens[i] > 0) memcpy(hseq.data() + seq_off[(size_t)i], seqs[i], (size_t)qlens[i]);
-	auto seq_d = upload(hseq.data(), hseq.size());
-	auto seq_off_d = upload(seq_off.data(), n), pk_off_d = upload(pk_off.data(), n), pk_d = upload(hpk.data(), hpk.size());
-	auto len_d = upload((const int32_t*)qlens, n);
-	auto hash_d = upload(name_hash.data(), n);
-	const std::vector<int32_t> self = read_self_ids(M, n, names);
-	auto self_d = upload(self.data(), n);
-	const int n_seg_tot = seg_off? seg_off[n] : 0;
-	auto seg_off_d = upload(seg_off? seg_off : (const int32_t*)self.data(), seg_off? (size_t)n + 1 : 0);
-	auto seg_len_d = upload(seg_len? seg_len : (const int32_t*)self.data(), seg_off? (size_t)n_seg_tot : 0);
 	DevBuf<ReadMeta> meta_d((size_t)n);
 	DevBuf<Pool> pools_d(2);
 	TestSeed t;
 	memset(&t.c, 0, sizeof(t.c));
 	t.c.g = M->g, t.c.ix = M->ix;
 	t.c.opt.flag = flag, t.c.opt.occ_max1 = occ_max1, t.c.opt.max_qlen = max_qlen;
-	t.c.b.n_reads = n, t.c.b.seq = seq_d, t.c.b.seq_off = seq_off_d, t.c.b.seq_len = len_d, t.c.b.name_hash = hash_d;
-	t.c.b.self_id = (flag & F_NO_DIAG)? (const int32_t*)self_d : 0;
-	t.c.b.seg_off = seg_off? (const int32_t*)seg_off_d : 0, t.c.b.seg_len = seg_off? (const int32_t*)seg_len_d : 0;
-	t.c.b.pk = seg_off? 0 : (const uint64_t*)pk_d, t.c.b.pk_off = seg_off? 0 : (const uint64_t*)pk_off_d;
+	const BatchLayout lay(n, qlens);
+	Staging stg;
+	mgb::HostPool one;
+	mgb_stats_t st = {};
+	t.c.b = upload_batch(stg, lay, M, n, qlens, seqs, names, (flag & F_NO_DIAG) != 0, seg_off, seg_len, one, 1, 0, st);
 	t.c.meta = meta_d, t.c.pool_anchor = pools_d, t.c.pool_minipos = pools_d + 1;
-	// pools as map_range sizes them at first, doubled while a read runs out of them (the batch's retry)
-	uint64_t cap_a = std::max<uint64_t>((uint64_t)n_bases / 4 * sizeof(u128), (uint64_t)1 << 22), cap_mp = std::max<uint64_t>((uint64_t)n_bases * sizeof(int32_t) / 2, (uint64_t)1 << 20);
+	// the first pools of a batch, doubled while a read runs out of them (the batch's retry)
+	const std::array<uint64_t, N_POOLS> cap = pool_caps(n, lay.n_bases, 0);
+	uint64_t cap_a = cap[P_ANCHOR], cap_mp = cap[P_MINIPOS];
 	std::vector<ReadMeta> meta((size_t)n);
 	for (;;) {
 		DevBuf<u128> anchor_d(cap_a / sizeof(u128));

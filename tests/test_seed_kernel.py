@@ -575,6 +575,13 @@ def case_seeds(lib, seen, rng, paths, G, k, w, full):
             frags.append(("one segment", [chr1[900:2000]]))
             check_seeds(lib, gi, ix, frags, 0, 50, 0, seen, what + " fragments")
             check_seeds(lib, gi, ix, frags, MG_M_HEAP_SORT, 50, 0, seen, what + " fragments, heap merge")
+            with_n = []
+            for i in range(65):  # more than 64 reads with other letters: the whole batch goes up as ASCII
+                p = rng.randrange(len(chr1) - 1000)
+                s = bytearray(chr1[p:p + 1000])
+                s[rng.randrange(1000)] = ord("N")
+                with_n.append(("N %d" % i, [bytes(s)]))
+            check_seeds(lib, gi, ix, with_n, 0, 50, 0, seen, what + " a batch uploaded as ASCII")
     finally:
         lib.mg_idx_destroy(gi)
         lib.mgb_gfa_destroy(g)
