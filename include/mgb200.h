@@ -109,6 +109,14 @@ typedef struct { /* minigraph.h:93-98 */
 	struct mg_idx_bucket_s *B; /* hidden: here it points to the engine's model (host copy + device image) */
 } mg_idx_t;
 
+typedef struct { /* minigraph.h:100-106 */
+	int32_t off, cnt:31, inner_pre:1;
+	uint32_t v;
+	int32_t rs, re, qs, qe;
+	int32_t score, dist_pre;
+	uint32_t hash_pre;
+} mg_lchain_t;
+
 typedef struct { int32_t off, cnt; uint32_t v; int32_t score; int32_t ed; } mg_llchain_t; /* minigraph.h:108-113 */
 
 typedef struct { /* minigraph.h:115-118 */
@@ -319,6 +327,19 @@ int mgb_test_sketch(int k, int w, int n, const char *seq, const int64_t *off, co
  * MGB_E_POOL when they do not fit a_cap / mp_cap (out[] is filled), or a negative code (nothing run) for bad reads. */
 int mgb_test_seed(const mg_idx_t *gi, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off, const int32_t *seg_len,
 				  const char *const *names, uint64_t flag, int occ_max1, int max_qlen, int32_t *out, mg128_t *a, int64_t a_cap, int32_t *mini_pos, int64_t mp_cap);
+
+/* test hook: graph-chain materialisation, the primary/secondary filters and mapq (map-algo.c:464-474 up to the CIGAR) as the kernels
+ * k_gchain (its bridging plan), k_gwfa and k_gchain_gen run them, on n reads whose graph chaining is given, with the graph of gi
+ * and the options opt (MG_M_CIGAR is ignored).  Read i is seqs[i] (qlens[i] > 0 bases); seg_off == NULL: one segment each,
+ * otherwise as for mgb_test_seed.  hash[i] is its hash (map-algo.c:362-364), rep_len[i] and n_mz[i] its repeat length and
+ * minimizer count; its n_u[i] chains (score<<32 | linear chains), n_lc[i] linear chains in the order mg_gchain1_dp leaves them
+ * and n_a[i] anchors (minimizer index in x>>32, as after mg_update_anchors; lc[].off counts from the read's first anchor) follow
+ * those of read i-1 in u, lc and a.  out[4i..4i+3] = rc (0 or a negative code), bridging jobs planned, of which aligned, pairs
+ * of linear chains bridged again in place after a failed bridge; gcs[i] (NULL unless rc is 0) is freed by mg_gchain_free.
+ * Returns 0, or a negative code (nothing run) for malformed input. */
+int mgb_test_gchain_gen(const mg_idx_t *gi, const mg_mapopt_t *opt, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off,
+						const int32_t *seg_len, const uint32_t *hash, const int32_t *rep_len, const int32_t *n_mz, const int32_t *n_u, const uint64_t *u,
+						const int32_t *n_lc, const mg_lchain_t *lc, const int32_t *n_a, const mg128_t *a, int32_t *out, mg_gchains_t **gcs);
 
 const char *mgb_last_error(void);
 void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st);

@@ -38,6 +38,12 @@ class mg_idx_t(C.Structure):
                 ("flag", C.c_int32), ("n_seg", C.c_int32), ("B", C.c_void_p)]
 
 
+class mg_lchain_t(C.Structure):  # minigraph.h:100-106
+    _fields_ = [("off", C.c_int32), ("cnt", C.c_int32, 31), ("inner_pre", C.c_int32, 1), ("v", C.c_uint32), ("rs", C.c_int32),
+                ("re", C.c_int32), ("qs", C.c_int32), ("qe", C.c_int32), ("score", C.c_int32), ("dist_pre", C.c_int32),
+                ("hash_pre", C.c_uint32)]
+
+
 class mg_llchain_t(C.Structure):
     _fields_ = [("off", C.c_int32), ("cnt", C.c_int32), ("v", C.c_uint32), ("score", C.c_int32), ("ed", C.c_int32)]
 
@@ -204,6 +210,10 @@ def bind_engine_api(lib):
     lib.mgb_test_seed.restype = C.c_int
     lib.mgb_test_seed.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_char_p), i32p, i32p, C.POINTER(C.c_char_p),
                                   C.c_uint64, C.c_int, C.c_int, i32p, C.POINTER(mg128_t), C.c_int64, i32p, C.c_int64]
+    lib.mgb_test_gchain_gen.restype = C.c_int
+    lib.mgb_test_gchain_gen.argtypes = [C.POINTER(mg_idx_t), C.POINTER(mg_mapopt_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_char_p), i32p, i32p,
+                                        u32p, i32p, i32p, i32p, C.POINTER(C.c_uint64), i32p, C.POINTER(mg_lchain_t), i32p, C.POINTER(mg128_t), i32p,
+                                        C.POINTER(C.POINTER(mg_gchains_t))]
     lib.mg_map_batch_frag.restype = C.c_int
     lib.mg_map_batch_frag.argtypes = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_char_p), C.POINTER(C.c_char_p),
                                       C.POINTER(C.POINTER(mg_gchains_t)), C.POINTER(mg_mapopt_t)]

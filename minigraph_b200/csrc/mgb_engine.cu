@@ -2021,6 +2021,22 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 static thread_local mgb_stats_t t_last_stats; // of the last batch mapped by the calling thread
 static thread_local bool t_has_stats = false;
 
+// The glibc logf table of mapq (reference: gcmisc.c:216-217) for reads of up to max_qlen bases, into o.  Grown under the lock; old
+// copies are kept until the model dies.
+static void logf_prepare(Model *M, int32_t max_qlen, MapOptDev &o)
+{
+	std::lock_guard<std::mutex> lk(M->big_mutex);
+	int need = std::max(1 << 16, max_qlen + 4096);
+	if (M->n_logf < need) {
+		M->logf_tab.resize(need);
+		for (int i = 0; i < need; ++i) M->logf_tab[i] = logf((float)i);
+		if (M->d_logf) M->dev_ptrs.push_back(M->d_logf); // a call in flight may still read it
+		M->d_logf = upload(M->logf_tab.data(), M->logf_tab.size()).release();
+		M->n_logf = need;
+	}
+	o.logf_tab = M->d_logf, o.n_logf_tab = M->n_logf;
+}
+
 // One call = one slot: its own stream, staging buffers, pools and worker arenas.  Up to "slots" calls run at once on one index
 // (callers beyond that wait), so a host that maps mini-batch i+1 on a second thread overlaps its packing, copies and result
 // assembly with the kernels of mini-batch i -- what the reference's kt_pipeline does with its step threads (gmap.c:176).
@@ -2048,18 +2064,7 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		slot_prepare(M, sl, p_slot_workers > 0? (int)p_slot_workers : default_workers());
 		MapOptDev o;
 		fill_opt(o, opt, M->k);
-		{ // glibc logf table for mapq (reference: gcmisc.c:216-217); grown under the lock, old copies are kept until the model dies
-			std::lock_guard<std::mutex> lk(M->big_mutex);
-			int need = std::max(1 << 16, max_qlen + 4096);
-			if (M->n_logf < need) {
-				M->logf_tab.resize(need);
-				for (int i = 0; i < need; ++i) M->logf_tab[i] = logf((float)i);
-				if (M->d_logf) M->dev_ptrs.push_back(M->d_logf); // a call in flight may still read it
-				M->d_logf = upload(M->logf_tab.data(), M->logf_tab.size()).release();
-				M->n_logf = need;
-			}
-			o.logf_tab = M->d_logf, o.n_logf_tab = M->n_logf;
-		}
+		logf_prepare(M, max_qlen, o);
 		int nt = (int)p_host_threads;
 		if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
 		t_launches = 0;
@@ -2844,6 +2849,208 @@ extern "C" int mgb_test_seed(const mg_idx_t *gi, int n, const int *qlens, const 
 							 const char *const *names, uint64_t flag, int occ_max1, int max_qlen, int32_t *out, mg128_t *a, int64_t a_cap, int32_t *mini_pos, int64_t mp_cap)
 {
 	try { return test_seed_impl(gi, n, qlens, seqs, seg_off, seg_len, names, flag, occ_max1, max_qlen, out, (u128*)a, a_cap, mini_pos, mp_cap); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: K7b on reads whose graph chaining is given (u, lc, a), run in the order of a pass (Pass::run) with the graph of gi and
+// the options opt: the batch uploaded by upload_batch; the bridging plan of stage_gchain_plan on lane 0, as stage_gchain ends
+// (k_gchain); the bridging jobs in make_job_order's order through gwfa_job_run (k_gwfa); stage_gchain_gen (k_gchain_gen), each
+// launched as its kernel is (test_launch).  The results are built by build_result, as mg_map_batch builds them.
+// ---------------------------------------------------------------------------------------------------------------
+struct TestGcPlan {
+	PipeCtx c;
+	ReadOut *routs;
+	const uint64_t *u;    // read i's chains at u[u_off[i]..+n_u[i]); its linear chains are c.lchain[meta.lc_off..]
+	const int64_t *u_off;
+	const int32_t *n_u;
+	MG_HD int operator()(int i, int32_t *, Arena &A, int, int lane) const
+	{
+		ReadMeta &m = c.meta[i];
+		A.top = 0;
+		if (lane == 0) gchain_out_init(routs[i], m);
+		LChain *lc;
+		uint32_t *gc_hash;
+		MGB_ALLOC(A, lc, LChain, m.n_lc);
+		MGB_ALLOC(A, gc_hash, uint32_t, m.n_lc);
+		for (int32_t j = lane; j < m.n_lc; j += MGB_W) lc[j] = c.lchain[m.lc_off + j];
+		warp_sync();
+		const int rc = stage_gchain_tail(c, m, i, A, m.n_lc, lc, n_u[i], u + u_off[i], c.anchor + m.a_off, gc_hash, lane);
+		if (rc < 0 && lane == 0) m.status = rc, routs[i].status = rc; // as stage_fail records a failed read
+		warp_sync();
+		return 0;
+	}
+};
+
+struct TestGcBridge {
+	PipeCtx c;
+	ReadOut *routs;
+	const int32_t *order; // the jobs in the order k_gwfa takes them
+	MG_HD int operator()(int i, int32_t *smem, Arena &A, int, int lane) const
+	{
+		A.top = 0;
+		const int rc = gwfa_job_run(A, c, order[i], lane, smem);
+		if (rc < 0 && lane == 0) { const int rid = c.gjobs[order[i]].rid; c.meta[rid].status = rc, routs[rid].status = rc; }
+		warp_sync();
+		return 0;
+	}
+};
+
+struct TestGcGen {
+	PipeCtx c;
+	ReadOut *routs;
+	int32_t *out; // per read: rc, bridging jobs, of which aligned, pairs bridged again in place
+	MG_HD int operator()(int i, int32_t *, Arena &A, int, int lane) const
+	{
+		int32_t *o = out + 4 * (int64_t)i;
+		const ReadMeta &m = c.meta[i];
+		A.top = 0;
+		if (lane == 0 && m.status == 0) {
+			const GState *gsb = (const GState*)(c.gstate + m.gstate_off);
+			o[1] = gsb->n_jobs, o[2] = 0;
+			for (int32_t j = 0; j < gsb->n_jobs; ++j) o[2] += c.gjobs[gsb->job_first + j].s >= 0;
+		}
+		const int rc = stage_gchain_gen(c, routs, i, A, lane, &o[3]);
+		if (rc < 0 && lane == 0) c.meta[i].status = rc, routs[i].status = rc;
+		warp_sync();
+		return 0;
+	}
+};
+
+static int test_gchain_gen_impl(const mg_idx_t *gi, const mg_mapopt_t *opt, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off,
+								const int32_t *seg_len, const uint32_t *hash, const int32_t *rep_len, const int32_t *n_mz, const int32_t *n_u, const uint64_t *u,
+								const int32_t *n_lc, const mg_lchain_t *lc, const int32_t *n_a, const u128 *a, int32_t *out, mg_gchains_t **gcs)
+{
+	auto refuse = [](const std::string &why) { set_error("mgb_test_gchain_gen: " + why); return (int)MGB_E_UNSUPPORTED; };
+	if (gi == 0 || opt == 0 || n < 0) return refuse("an index, options and n at least 0");
+	const Model *M = model_of(gi);
+	std::vector<ReadMeta> meta((size_t)n);
+	std::vector<LChain> hlc;
+	std::vector<int64_t> u_off((size_t)n);
+	int64_t su = 0, sa = 0;
+	int32_t max_qlen = 0;
+	for (int i = 0; i < n; ++i) {
+		const std::string r = "read " + std::to_string(i);
+		if (qlens[i] < 1 || seqs[i] == 0) return refuse(r + " is empty");
+		if (seg_off) {
+			if (seg_off[i] < 0 || seg_off[i + 1] <= seg_off[i]) return refuse(r + " has no segment");
+			int64_t sum = 0;
+			for (int32_t j = seg_off[i]; j < seg_off[i + 1]; ++j) {
+				if (seg_len[j] < 1) return refuse(r + " has an empty segment");
+				sum += seg_len[j];
+			}
+			if (sum != qlens[i]) return refuse(r + ": its segments do not add up to its length");
+		}
+		if (n_u[i] < 0 || n_lc[i] < 0 || n_a[i] < 0 || n_mz[i] < 0 || rep_len[i] < 0) return refuse(r + " has a negative count");
+		int64_t sum = 0;
+		for (int32_t j = 0; j < n_u[i]; ++j) {
+			if ((uint32_t)u[su + j] == 0) return refuse(r + " has a chain of no linear chains");
+			sum += (uint32_t)u[su + j];
+		}
+		if (sum != n_lc[i]) return refuse(r + ": the linear chains counted by u do not add up to n_lc");
+		if (n_lc[i] > 0 && n_a[i] == 0) return refuse(r + " has linear chains but no anchors");
+		ReadMeta &m = meta[(size_t)i];
+		m.hash = hash[i], m.rep_len = rep_len[i], m.n_mz = n_mz[i], m.n_a = n_a[i], m.a_off = sa, m.n_lc = n_lc[i], m.lc_off = (int64_t)hlc.size();
+		for (int32_t j = 0; j < n_lc[i]; ++j) {
+			const mg_lchain_t &l = lc[m.lc_off + j];
+			if ((l.v >> 1) >= (uint32_t)M->g.n_seg) return refuse(r + " has a vertex outside the graph");
+			const int32_t vlen = M->seg_len[l.v >> 1];
+			if (l.off < 0 || l.cnt < 0 || (int64_t)l.off + l.cnt > n_a[i] || l.rs < 0 || l.rs > l.re || l.re > vlen || l.qs < 0 || l.qs > l.qe || l.qe > qlens[i])
+				return refuse(r + " has a linear chain outside its anchors, its vertex or the read");
+			for (int32_t t = l.off; t < l.off + l.cnt; ++t)
+				if ((int32_t)a[sa + t].x < 0 || (int32_t)a[sa + t].x >= vlen || (int32_t)a[sa + t].y < 0 || (int32_t)a[sa + t].y >= qlens[i])
+					return refuse(r + " has an anchor outside its vertex or the read");
+			LChain q;
+			q.off = l.off, q.cnt = l.cnt, q.v = l.v, q.rs = l.rs, q.re = l.re, q.qs = l.qs, q.qe = l.qe, q.score = l.score, q.dist_pre = l.dist_pre;
+			q.hash_pre = l.hash_pre, q.inner_pre = l.inner_pre;
+			hlc.push_back(q);
+		}
+		u_off[(size_t)i] = su;
+		su += n_u[i], sa += n_a[i];
+		max_qlen = std::max(max_qlen, qlens[i]);
+	}
+	if (n == 0) return 0;
+	if (int e = test_no_device(M->device)) return e;
+	PipeCtx c;
+	memset(&c, 0, sizeof(c));
+	c.g = M->g, c.ix = M->ix;
+	fill_opt(c.opt, opt, M->k);
+	c.opt.flag &= ~(uint64_t)F_CIGAR; // the alignment plan and what follows it are left out
+	logf_prepare((Model*)M, max_qlen, c.opt);
+	const BatchLayout lay(n, qlens);
+	Staging stg;
+	mgb::HostPool one;
+	mgb_stats_t st = {};
+	c.b = upload_batch(stg, lay, M, n, qlens, seqs, 0, false, seg_off, seg_len, one, 1, 0, st);
+	std::vector<u128> ha(a, a + sa);
+	std::vector<uint64_t> hu(u, u + su);
+	ha.resize((size_t)sa + 1), hu.resize((size_t)su + 1), hlc.resize(hlc.size() + 1); // no empty device buffers
+	auto a_d = upload(ha.data(), ha.size());
+	auto u_d = upload(hu.data(), hu.size());
+	auto lc_d = upload(hlc.data(), hlc.size());
+	auto u_off_d = upload(u_off.data(), (size_t)n);
+	auto n_u_d = upload(n_u, (size_t)n);
+	DevBuf<ReadMeta> meta_d((size_t)n);
+	DevBuf<ReadOut> routs_d((size_t)n);
+	DevBuf<int32_t> out_d(4 * (size_t)n);
+	DevBuf<Pool> pools_d(4);
+	c.meta = meta_d, c.anchor = a_d, c.lchain = lc_d;
+	c.pool_out = pools_d, c.pool_gstate = pools_d + 1, c.pool_gjobs = pools_d + 2, c.pool_walk = pools_d + 3;
+	const std::array<uint64_t, N_POOLS> cap0 = pool_caps(n, lay.n_bases, 0);
+	uint64_t cap[4] = {cap0[P_OUT], cap0[P_GSTATE], cap0[P_GJOBS], cap0[P_WALK]};
+	const uint64_t arena_bytes = (uint64_t)32 << 20; // (the pipeline's workers have 3 MB and retry a read that outgrows them with 1 GB)
+	std::vector<ReadOut> routs((size_t)n);
+	for (;;) {
+		DevBuf<char> out_pool(cap[0]), gstate(cap[1]);
+		DevBuf<GwfaJob> gjobs(cap[2] / sizeof(GwfaJob) + 1);
+		DevBuf<int32_t> walk(cap[3] / sizeof(int32_t) + 1);
+		Pool hp[4];
+		for (int p = 0; p < 4; ++p) hp[p].used = 0, hp[p].cap = cap[p];
+		h2d(pools_d, hp, sizeof(hp));
+		dfill(gjobs, 0xff, cap[2]); // reserved-but-unused bridging job slots read as rid == -1 (as in Pass)
+		h2d(meta_d, meta.data(), sizeof(ReadMeta) * (size_t)n);
+		dzero(routs_d, sizeof(ReadOut) * (size_t)n);
+		dzero(out_d, sizeof(int32_t) * 4 * (size_t)n);
+		c.out = out_pool, c.gstate = gstate, c.gjobs = gjobs, c.walk = walk;
+		const TestGcPlan tp{c, routs_d, u_d, u_off_d, n_u_d};
+		if (int e = test_launch<S_GCHAIN>(n, std::min(n, StageSpec<S_GCHAIN>::warps), arena_bytes, tp)) return e;
+		d2h(hp, pools_d, sizeof(hp));
+		const int n_jobs = (int)(std::min(hp[2].used, hp[2].cap) / sizeof(GwfaJob));
+		if (n_jobs > 0) {
+			LaunchArgs L;
+			memset(&L, 0, sizeof(L));
+			L.c = c;
+			DevBuf<int32_t> order((size_t)n_jobs);
+			make_job_order(L, 0, 0, n_jobs, order);
+			const TestGcBridge tb{c, routs_d, order};
+			if (int e = test_launch<S_GWFA>(n_jobs, std::min(n_jobs, 2 * StageSpec<S_GWFA>::warps), arena_bytes, tb)) return e;
+		}
+		const TestGcGen tg{c, routs_d, out_d};
+		if (int e = test_launch<S_GCHAIN_GEN>(n, std::min(n, StageSpec<S_GCHAIN_GEN>::warps), arena_bytes, tg)) return e;
+		std::vector<ReadMeta> m_out((size_t)n);
+		d2h(m_out.data(), meta_d, sizeof(ReadMeta) * (size_t)n);
+		d2h(routs.data(), routs_d, sizeof(ReadOut) * (size_t)n);
+		d2h(hp, pools_d, sizeof(hp));
+		bool pool_full = false;
+		for (int i = 0; i < n; ++i) pool_full |= read_status(m_out[(size_t)i], routs[(size_t)i]) == MGB_E_POOL;
+		if (pool_full) { for (int p = 0; p < 4; ++p) cap[p] *= 2; continue; }
+		std::vector<char> hout(std::min(hp[0].used, hp[0].cap) + 64);
+		d2h(hout.data(), out_pool, std::min(hp[0].used, hp[0].cap));
+		d2h(out, out_d, sizeof(int32_t) * 4 * (size_t)n);
+		for (int i = 0; i < n; ++i) {
+			out[4 * (int64_t)i] = read_status(m_out[(size_t)i], routs[(size_t)i]);
+			gcs[i] = out[4 * (int64_t)i] == 0? build_result(routs[(size_t)i], hout.data()) : 0;
+		}
+		return 0;
+	}
+}
+
+extern "C" int mgb_test_gchain_gen(const mg_idx_t *gi, const mg_mapopt_t *opt, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off,
+								   const int32_t *seg_len, const uint32_t *hash, const int32_t *rep_len, const int32_t *n_mz, const int32_t *n_u, const uint64_t *u,
+								   const int32_t *n_lc, const mg_lchain_t *lc, const int32_t *n_a, const mg128_t *a, int32_t *out, mg_gchains_t **gcs)
+{
+	for (int i = 0; i < n; ++i) gcs[i] = 0;
+	try { return test_gchain_gen_impl(gi, opt, n, qlens, seqs, seg_off, seg_len, hash, rep_len, n_mz, n_u, u, n_lc, lc, n_a, (const u128*)a, out, gcs); }
+	catch (const MgbError &e) { return e.code; }
 }
 
 extern "C" void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st) { *st = t_has_stats? t_last_stats : model_of(gi)->stats; } // the calling thread's last batch

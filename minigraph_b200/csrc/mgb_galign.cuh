@@ -547,6 +547,25 @@ MG_HD inline int stage_gchain_plan(const PipeCtx &c, ReadMeta &m, int rid, Arena
 	return 0;
 }
 
+// the result header of a read as K6 starts it (lane 0)
+MG_HD inline void gchain_out_init(ReadOut &ro, const ReadMeta &m)
+{
+	ro.status = 0, ro.n_gc = ro.n_lc = ro.n_a = 0, ro.rep_len = m.rep_len, ro.n_mz = m.n_mz, ro.blob_size = ro.blob2_size = 0, ro.blob_off = ro.blob2_off = 0;
+}
+
+// the end of K6 after the graph-chaining DP, entered by all lanes: the bridging plan on lane 0, its code on every lane
+MG_HD inline int stage_gchain_tail(const PipeCtx &c, ReadMeta &m, int rid, Arena &A, int32_t n_lc, LChain *lc, int32_t n_u, const uint64_t *u, const u128 *a,
+								   uint32_t *gc_hash, int lane)
+{
+	int rc = 0;
+	if (lane == 0) {
+		Arena B = A;
+		rc = stage_gchain_plan(c, m, rid, B, n_lc, lc, n_u, u, a, gc_hash);
+		if (B.peak > A.peak) A.peak = B.peak;
+	}
+	return warp_bcast_i32(rc, 0);
+}
+
 // K6 for one read, entered by all lanes of a warp: the graph-chaining DP is warp-wide (gchain_dp_w), the bridging plan and the
 // hand-over to K7 (a few dozen words per read) are written by lane 0.
 MG_HD inline int stage_gchain(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, int lane)
@@ -554,7 +573,7 @@ MG_HD inline int stage_gchain(const PipeCtx &c, ReadOut *routs, int rid, Arena &
 	ReadMeta &m = c.meta[rid];
 	ReadOut &ro = routs[rid];
 	const MapOptDev &o = c.opt;
-	if (lane == 0) ro.status = 0, ro.n_gc = ro.n_lc = ro.n_a = 0, ro.rep_len = m.rep_len, ro.n_mz = m.n_mz, ro.blob_size = ro.blob2_size = 0, ro.blob_off = ro.blob2_off = 0;
+	if (lane == 0) gchain_out_init(ro, m);
 	if (m.status != 0) { if (lane == 0) ro.status = m.status; return 0; } // status 1: read skipped (empty or too long) -> no result object
 	const uint64_t mark = A.top;
 	const int32_t qlen = c.b.seq_len[rid];
@@ -572,13 +591,7 @@ MG_HD inline int stage_gchain(const PipeCtx &c, ReadOut *routs, int rid, Arena &
 	gp.max_dist_g = gp.max_dist_q = gp.bw = o.bw_long, gp.ref_bonus = o.ref_bonus, gp.chn_pen_gap = o.chn_pen_gap, gp.mask_level = o.mask_level; // reference: map-algo.c:461-462
 	MGB_TRY(gchain_dp_w(A, c.g, c.lab, &n_lc, lc, qlen, gp, o.max_gc_skip, a, &u, &n_u, lane));
 	if (lane == 0) { unsigned long long dt = prof_clock() - pt0; prof_add(c, PROF_GC_DP_CYC, dt); prof_max(c, PROF_GC_DP_MAX_CYC, dt); }
-	int rc = 0;
-	if (lane == 0) {
-		Arena B = A;
-		rc = stage_gchain_plan(c, m, rid, B, n_lc, lc, n_u, u, a, gc_hash);
-		if (B.peak > A.peak) A.peak = B.peak;
-	}
-	rc = warp_bcast_i32(rc, 0);
+	const int rc = stage_gchain_tail(c, m, rid, A, n_lc, lc, n_u, u, a, gc_hash, lane);
 	A.top = mark;
 	return rc;
 }
@@ -722,7 +735,8 @@ MG_HD inline int gchain_cigar_plan_w(Arena &A, const PipeCtx &c, int rid, const 
 }
 
 // K7b for one read: materialise graph chains from the DP and the bridging results, post filters, alignment plan.
-MG_HD inline int stage_gchain_gen_head(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, GenHand *hand)
+// n_rebridged: as gchain_gen() has it.
+MG_HD inline int stage_gchain_gen_head(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, GenHand *hand, int32_t *n_rebridged = 0)
 {
 	ReadMeta &m = c.meta[rid];
 	ReadOut &ro = routs[rid];
@@ -746,7 +760,7 @@ MG_HD inline int stage_gchain_gen_head(const PipeCtx &c, ReadOut *routs, int rid
 	feed.job = c.gjobs + gsb->job_first, feed.walk_pool = c.walk, feed.next = 0, feed.n = gsb->n_jobs;
 	GcSet gs;
 	unsigned long long pt1 = prof_clock();
-	MGB_TRY(gchain_gen(A, c.g, n_u, u, lc, a, m.hash, o.min_gc_cnt, o.min_gc_score, o.gdp_max_ed, batch_n_seg(c.b, rid), qseq, gs, &feed, gc_hash));
+	MGB_TRY(gchain_gen(A, c.g, n_u, u, lc, a, m.hash, o.min_gc_cnt, o.min_gc_score, o.gdp_max_ed, batch_n_seg(c.b, rid), qseq, gs, &feed, gc_hash, n_rebridged));
 	gs.rep_len = m.rep_len;
 	unsigned long long pt2 = prof_clock();
 	prof_add(c, PROF_GC_GEN_CYC, pt2 - pt1);
@@ -774,7 +788,7 @@ MG_HD inline int stage_gchain_gen_head(const PipeCtx &c, ReadOut *routs, int rid
 
 // stage_gchain_gen() entered by all lanes of a warp (parameter "gen_v2"): lane 0 runs the sequential head, then the plan and
 // the copies of the first part of the result are shared by the lanes.
-MG_HD inline int stage_gchain_gen(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, int lane)
+MG_HD inline int stage_gchain_gen(const PipeCtx &c, ReadOut *routs, int rid, Arena &A, int lane, int32_t *n_rebridged = 0)
 {
 	GenHand h;
 	h.gs.n_gc = h.gs.n_lc = h.gs.n_a = h.gs.rep_len = 0, h.gs.gc = 0, h.gs.lc = 0, h.gs.a = 0;
@@ -782,7 +796,7 @@ MG_HD inline int stage_gchain_gen(const PipeCtx &c, ReadOut *routs, int rid, Are
 	h.boff = 0, h.off_lc = h.off_a = h.sz = 0, h.mark = A.top, h.pt3 = 0, h.want_plan = 0, h.skip = 1;
 	int rc = 0;
 	Arena B = A;
-	if (lane == 0) rc = stage_gchain_gen_head(c, routs, rid, B, &h);
+	if (lane == 0) rc = stage_gchain_gen_head(c, routs, rid, B, &h, n_rebridged);
 	rc = warp_bcast_i32(rc, 0);
 	A.top = warp_bcast_u64(B.top, 0), A.peak = warp_bcast_u64(B.peak, 0);
 	h.skip = warp_bcast_i32(h.skip, 0);

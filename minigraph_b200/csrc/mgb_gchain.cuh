@@ -649,10 +649,10 @@ MG_HD inline int gchain_prep(const GraphDev &g, int32_t n_u, const uint64_t *u, 
 }
 
 // With `feed`, gchain_prep() has already hashed the chains (gc_hash) and resolved overlaps, and the bridging
-// alignments come from the job kernel.
+// alignments come from the job kernel.  n_rebridged (NULL in the pipeline) counts the pairs bridged again in place.
 MG_HD inline int gchain_gen(Arena &A, const GraphDev &g, int32_t n_u, const uint64_t *u, LChain *lc, const u128 *a, uint32_t hash,
 							int32_t min_gc_cnt, int32_t min_gc_score, int32_t gdp_max_ed, int32_t n_seg, const char *qseq, GcSet &gs,
-							GwfaFeed *feed, const uint32_t *gc_hash)
+							GwfaFeed *feed, const uint32_t *gc_hash, int32_t *n_rebridged = 0)
 {
 	int32_t i, j, k, st, kmer_size;
 	gs.n_gc = gs.n_lc = gs.n_a = 0, gs.rep_len = 0, gs.gc = 0, gs.lc = 0, gs.a = 0, gs.cyc_gwfa = gs.cyc_shortk = gs.cyc_extra = 0;
@@ -704,6 +704,7 @@ MG_HD inline int gchain_gen(Arena &A, const GraphDev &g, int32_t n_u, const uint
 					if (failed) {
 						aux.feed = 0; // the rare re-bridging of consecutive pairs is not planned: align in place
 						for (int32_t t = j0; t < j; ++t) {
+							if (n_rebridged) ++*n_rebridged;
 							MGB_TRY(gc_bridge_lchains(A, aux, n_seg, kmer_size, gdp_max_ed, &lc[st + t], &lc[st + t + 1], a, &failed));
 							if (failed) return MGB_E_INTERNAL;
 						}
