@@ -232,6 +232,26 @@ void mgb_free_batch(int n_reads, mg_gchains_t **gcs);
 int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, const int *qlens, const char *const *seqs,
 					  const char *const *names, const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap);
 
+/* Map reads that already live in device memory: no base crosses PCIe, the batch is laid out on the device by k_ingest.
+ * Sequence i is d_seq[d_off[i] .. d_off[i+1]) (n_seq + 1 int64 offsets, themselves in device memory, non-decreasing, within
+ * [0, seq_bytes]), bytes in any case: they are upper-cased on the device by gmap.c:81 mg_toupper's rule (only 'a'..'z' change).
+ * n_seg == NULL: n_frag single-segment reads (n_seq == n_frag); otherwise as mg_map_batch_frag() (the caller has already
+ * reverse-complemented mates, as gmap.c:38-40 does).  names[] is per fragment, on the host, and may be NULL.  stream: the
+ * caller's cudaStream_t (NULL: the legacy default stream); the first read of d_seq / d_off is ordered after the work already
+ * queued on it, nothing is queued on it, and the call returns only once it no longer reads them.  Neither buffer is modified.
+ * The results are byte for byte those of mg_map_batch_frag() / mgb_map_batch_gaf() on the same reads after mg_toupper: gcs has
+ * n_seq entries filled as mg_map_batch_frag() fills them, and the text follows mgb_map_batch_gaf()'s buffer rules and refusals.
+ * Returns 0, or a negative code with the reason in mgb_last_error() and no partial results, also when d_seq or d_off is not device
+ * or managed memory on the index's device, the offsets decrease or fall outside [0, seq_bytes], or a read is longer than INT32_MAX.
+ * The host copies the offsets back (8 bytes per read) for the batch's layout.  MGB_DEVICES works as for mg_map_batch(): a part
+ * that maps on a peer device gets its span of d_seq copied device to device.  In the stats of such a call, h2d_bytes counts only
+ * the per-read tables, t_pack_ms is 0, and t_h2d_ms covers the copy of the offsets, the tables and the ingest kernel. */
+int mgb_map_batch_dev(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+					  const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, mg_gchains_t **gcs);
+int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+						  const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, char **out, size_t *out_len,
+						  size_t *out_cap);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Engine controls and instrumentation (not part of the reference API)
  * ---------------------------------------------------------------------------------------------------------- */
@@ -340,6 +360,13 @@ int mgb_test_seed(const mg_idx_t *gi, int n, const int *qlens, const char *const
 int mgb_test_gchain_gen(const mg_idx_t *gi, const mg_mapopt_t *opt, int n, const int *qlens, const char *const *seqs, const int32_t *seg_off,
 						const int32_t *seg_len, const uint32_t *hash, const int32_t *rep_len, const int32_t *n_mz, const int32_t *n_u, const uint64_t *u,
 						const int32_t *n_lc, const mg_lchain_t *lc, const int32_t *n_a, const mg128_t *a, int32_t *out, mg_gchains_t **gcs);
+
+/* test hook: the ingest step of reads in device memory as mgb_map_batch_dev() runs it (k_ingest on the device, its host loop in the
+ * simulators) on n sequences seq[off[i] .. off[i+1]) (host memory, copied to the device first).  Sequence i's upper-case copy goes
+ * to ascii_out[off[i] .. off[i+1]); unless segmented (a batch of fragments with segments, which has no 2-bit words), its
+ * (len + 31) / 32 words follow those of sequence i-1 in pk_out; raw_out[i] is 1 when it holds a byte other than A/C/G/T.
+ * Returns 0, or a negative code for bad offsets or when the batch's pk_off does not mark exactly the flagged reads. */
+int mgb_test_ingest(int n, const char *seq, const int64_t *off, int segmented, char *ascii_out, uint64_t *pk_out, int32_t *raw_out);
 
 const char *mgb_last_error(void);
 void mgb_get_stats(const mg_idx_t *gi, mgb_stats_t *st);

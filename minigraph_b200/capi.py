@@ -226,4 +226,13 @@ def bind_engine_api(lib):
     lib.mgb_write_gaf_batch.restype = None
     lib.mgb_write_gaf_batch.argtypes = [C.POINTER(gfa_t), C.c_int, C.POINTER(C.POINTER(mg_gchains_t)), C.POINTER(C.c_int),
                                         C.POINTER(C.c_char_p), C.c_uint64, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    # reads in device memory: d_seq, d_off and the stream are plain addresses (a CUDA tensor's data_ptr(), a cudaStream_t)
+    dev_args = [C.POINTER(mg_idx_t), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_char_p),
+                C.POINTER(mg_mapopt_t), C.c_void_p]
+    lib.mgb_map_batch_dev.restype = C.c_int
+    lib.mgb_map_batch_dev.argtypes = dev_args + [C.POINTER(C.POINTER(mg_gchains_t))]
+    lib.mgb_map_batch_dev_gaf.restype = C.c_int
+    lib.mgb_map_batch_dev_gaf.argtypes = dev_args + [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.mgb_test_ingest.restype = C.c_int
+    lib.mgb_test_ingest.argtypes = [C.c_int, C.c_char_p, i64p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64), i32p]
     return lib

@@ -25,6 +25,7 @@
 #include "../../include/mgb200.h"
 #include "mgb_galign.cuh"
 #include "mgb_gaf.cuh"
+#include "mgb_ingest.cuh"
 
 #ifndef MGB_HOSTSIM
 #include <cuda_runtime.h>
@@ -92,6 +93,7 @@ typedef double DevEvent; // the host clock when it was recorded
 static void dev_bind(int dev, DevStream s) { (void)dev, (void)s; }
 static void h2d_async(void *d, const void *h, size_t n) { if (n) memcpy(d, h, n); }
 static void d2h_async(void *h, const void *d, size_t n) { if (n) memcpy(h, d, n); }
+static void d2d_peer(void *d, int d_dev, const void *s, int s_dev, size_t n) { (void)d_dev, (void)s_dev; if (n) memcpy(d, s, n); }
 static void ev_record(DevEvent &e) { e = now_ms(); }
 static void ev_wait(DevEvent &e) { (void)e; }
 static double ev_ms(DevEvent &a, DevEvent &b) { return b - a; }
@@ -121,6 +123,8 @@ static void dev_bind(int dev, DevStream s) { cudaSetDevice(dev); t_stream = s; }
 // copies that do not wait: the host memory must be page-locked and stay untouched until the stream gets past them
 static void h2d_async(void *d, const void *h, size_t n) { if (n) CUDA_OK(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, t_stream)); }
 static void d2h_async(void *h, const void *d, size_t n) { if (n) CUDA_OK(cudaMemcpyAsync(h, d, n, cudaMemcpyDeviceToHost, t_stream)); }
+// from another device's memory (or the same device's)
+static void d2d_peer(void *d, int d_dev, const void *s, int s_dev, size_t n) { if (n) CUDA_OK(cudaMemcpyPeerAsync(d, d_dev, s, s_dev, n, t_stream)); }
 static void ev_record(DevEvent &e) { CUDA_OK(cudaEventRecord(e, t_stream)); }
 static void ev_wait(DevEvent &e) { CUDA_OK(cudaEventSynchronize(e)); }
 static double ev_ms(DevEvent &a, DevEvent &b) { float t = 0; return cudaEventElapsedTime(&t, a, b) == cudaSuccess? t : 0; }
@@ -606,6 +610,22 @@ static void unpack_reads(const UnpackArgs &U)
 	++t_launches;
 }
 
+// Reads already in device memory: their ASCII copy, words and flags (mgb_ingest.cuh)
+static void ingest_reads(const IngestArgs &I)
+{
+#ifndef MGB_HOSTSIM
+	k_ingest<<<dev_sm_count() * 8, 256, 0, t_stream>>>(I);
+	CUDA_OK(cudaGetLastError());
+#else
+	for (int r = 0; r < I.n_reads; ++r) {
+		uint32_t bad = 0;
+		for (int64_t wd = 0; wd * 32 < I.seq_len[r]; ++wd) bad |= ingest_word(I, r, wd);
+		ingest_flag(I, r, bad != 0);
+	}
+#endif
+	++t_launches;
+}
+
 // ---- the few words the host needs between two kernels (pool fill levels, queue lengths) ----
 // They do not travel by cudaMemcpy: a copy of 16 bytes queues behind whatever another call in flight has put on the copy engines
 // (a few hundred MB of results, tens of ms).  A one-warp kernel writes them into page-locked host memory the device can address.
@@ -880,6 +900,7 @@ struct BatchLayout {
 // The page-locked host copies and the device copies of a batch's reads and per-read tables (upload_batch)
 struct Staging {
 	GrowBuf h_tables{true}, h_seq{true}, h_pk{true}, d_tables, d_seq, d_pk, d_segs;
+	GrowBuf d_src; // reads in device memory that map on a peer device: their span of the caller's buffer (upload_batch_dev)
 };
 
 // The output pools of a batch (PipeCtx); an attempt at the batch that overflows one is run again with that pool grown
@@ -1639,6 +1660,50 @@ static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int
 	return 0;
 }
 
+// seq_off, seq_len and name_hash of a batch in one page-locked block (they go up in one copy, upload_tables)
+static uint64_t *batch_tables(Staging &B, const BatchLayout &lay, int n_reads, const int *qlens, const char *const *names)
+{
+	const size_t n = (size_t)n_reads;
+	uint64_t *seq_off = (uint64_t*)B.h_tables.ensure(n * 16 + 256);
+	int32_t *seq_len = (int32_t*)(seq_off + n);
+	uint32_t *name_hash = (uint32_t*)(seq_len + n);
+	memcpy(seq_off, lay.seq_off.data(), n * 8);
+	for (size_t i = 0; i < n; ++i) seq_len[i] = qlens[i], name_hash[i] = names && names[i]? hash_str(names[i]) : 0;
+	return seq_off;
+}
+
+// those tables to the device, into b (with room behind them for self_id)
+static void upload_tables(Staging &B, BatchDev &b, int n_reads, const uint64_t *h_tables, char *d_seq, mgb_stats_t &S)
+{
+	const size_t n = (size_t)n_reads;
+	uint64_t *d_seq_off = (uint64_t*)B.d_tables.ensure(n * 20 + 64); // seq_off, seq_len, name_hash, self_id
+	h2d(d_seq_off, h_tables, n * 16);
+	S.h2d_bytes += (int64_t)n * 16;
+	b.n_reads = n_reads, b.seq = d_seq, b.seq_off = d_seq_off, b.seq_len = (const int32_t*)(d_seq_off + n), b.name_hash = (const uint32_t*)(b.seq_len + n);
+}
+
+// what follows the reads of every batch: which segment name, if any, is each read's own (MG_M_NO_DIAG; exact string match on the
+// host), and the segments of the fragments (seg_off, seg_len: as BatchDev has them, or NULL)
+static void upload_read_extras(Staging &B, BatchDev &b, const Model *M, const char *const *names, bool no_diag, const int32_t *seg_off, const int32_t *seg_len)
+{
+	const size_t n = (size_t)b.n_reads;
+	if (no_diag) {
+		std::vector<int32_t> self(n, -1);
+		for (size_t i = 0; i < n; ++i)
+			if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[i] = it->second; }
+		int32_t *d_self_id = (int32_t*)(b.name_hash + n);
+		h2d(d_self_id, self.data(), sizeof(int32_t) * n);
+		b.self_id = d_self_id;
+	}
+	if (seg_off) {
+		const size_t n_len = (size_t)seg_off[n];
+		int32_t *d_segs = (int32_t*)B.d_segs.ensure(sizeof(int32_t) * (n + 1 + n_len));
+		h2d(d_segs, seg_off, sizeof(int32_t) * (n + 1));
+		h2d(d_segs + n + 1, seg_len, sizeof(int32_t) * n_len);
+		b.seg_off = d_segs, b.seg_len = d_segs + n + 1;
+	}
+}
+
 // Copies a batch laid out as lay says to the device and returns what the kernels read of it.  The reads go up 2 bits per base (a
 // quarter of the bytes) and k_unpack writes their ASCII copy on the device; a read with any byte other than A/C/G/T goes up as
 // ASCII, and so does the whole batch when such reads are many or the fragments have segments (seg_off, seg_len: as BatchDev has
@@ -1648,11 +1713,7 @@ static BatchDev upload_batch(Staging &B, const BatchLayout &lay, const Model *M,
 							 EvTimer *t, mgb_stats_t &S)
 {
 	const size_t n = (size_t)n_reads;
-	uint64_t *seq_off = (uint64_t*)B.h_tables.ensure(n * 16 + 256); // seq_off, seq_len and name_hash: one copy
-	int32_t *seq_len = (int32_t*)(seq_off + n);
-	uint32_t *name_hash = (uint32_t*)(seq_len + n);
-	memcpy(seq_off, lay.seq_off.data(), n * 8);
-	for (size_t i = 0; i < n; ++i) seq_len[i] = qlens[i], name_hash[i] = names && names[i]? hash_str(names[i]) : 0;
+	const uint64_t *seq_off = batch_tables(B, lay, n_reads, qlens, names);
 	char *hseq = (char*)B.h_seq.ensure(lay.seq_bytes), *d_seq = (char*)B.d_seq.ensure(lay.seq_bytes);
 	const Pieces pcs(n_reads);
 	BatchDev b;
@@ -1704,28 +1765,55 @@ static BatchDev upload_batch(Staging &B, const BatchLayout &lay, const Model *M,
 			dsync();
 			S.h2d_bytes = (int64_t)lay.seq_bytes;
 		}
-		uint64_t *d_seq_off = (uint64_t*)B.d_tables.ensure(n * 20 + 64); // seq_off, seq_len, name_hash, self_id
-		h2d(d_seq_off, seq_off, n * 16);
-		S.h2d_bytes += (int64_t)n * 16;
-		b.n_reads = n_reads, b.seq = d_seq, b.seq_off = d_seq_off, b.seq_len = (const int32_t*)(d_seq_off + n), b.name_hash = (const uint32_t*)(b.seq_len + n);
+		upload_tables(B, b, n_reads, seq_off, d_seq, S);
 		b.pk = packed? d_pk : 0, b.pk_off = packed? d_pk_off : 0;
-		if (packed) unpack_reads(UnpackArgs{d_pk, d_pk_off, d_seq_off, b.seq_len, d_seq, n_reads});
+		if (packed) unpack_reads(UnpackArgs{d_pk, d_pk_off, b.seq_off, b.seq_len, d_seq, n_reads});
 	}
-	if (no_diag) { // which segment name, if any, is each read's own (exact string match on the host)
-		std::vector<int32_t> self(n, -1);
-		for (size_t i = 0; i < n; ++i)
-			if (names && names[i]) { auto it = M->name_ids.find(names[i]); if (it != M->name_ids.end()) self[i] = it->second; }
-		int32_t *d_self_id = (int32_t*)(b.name_hash + n);
-		h2d(d_self_id, self.data(), sizeof(int32_t) * n);
-		b.self_id = d_self_id;
+	upload_read_extras(B, b, M, names, no_diag, seg_off, seg_len);
+	return b;
+}
+
+// Reads that are already in device memory (mgb_map_batch_dev*): read i of a batch is src[src_off[i] .. + its length) on device
+// src_dev.  copy: the batch maps on a peer (MGB_DEVICES), which takes its span of src into the slot's staging first.  t_off_ms: the
+// host time of the copy of the caller's offsets, counted in the batch's t_h2d_ms.
+struct DevReads { const char *src; const int64_t *src_off; int src_dev; bool copy; double t_off_ms; };
+
+// upload_batch() for reads in device memory: no base crosses PCIe.  The per-read tables and the reads' offsets go up, and k_ingest
+// writes the ASCII copy, the 2-bit words (none for fragments with segments) and, for a read that holds any other byte than
+// A/C/G/T, pk_off = ~0.  d_raw (or NULL) receives those flags.  t (or NULL) times the peer copy, the tables and k_ingest.
+static BatchDev upload_batch_dev(Staging &B, const BatchLayout &lay, const Model *M, int n_reads, const int *qlens, const DevReads &R,
+								 const char *const *names, bool no_diag, const int32_t *seg_off, const int32_t *seg_len, EvTimer *t, mgb_stats_t &S,
+								 int32_t *d_raw = 0)
+{
+	const size_t n = (size_t)n_reads, n8 = (n + 7) & ~(size_t)7;
+	const bool packed = seg_off == 0;
+	const uint64_t *h_tables = batch_tables(B, lay, n_reads, qlens, names);
+	char *d_seq = (char*)B.d_seq.ensure(lay.seq_bytes);
+	BatchDev b;
+	memset(&b, 0, sizeof(b));
+	{
+		Span span(t);
+		uint64_t *h = (uint64_t*)B.h_pk.ensure(n8 * 16 + 64); // pk_off, then the reads' offsets in src
+		memcpy(h, lay.pk_off.data(), n * 8);
+		int64_t *src_off = (int64_t*)(h + n8);
+		const char *src = R.src;
+		if (R.copy) {
+			int64_t lo = INT64_MAX, hi = 0;
+			for (size_t i = 0; i < n; ++i) if (qlens[i] > 0) lo = std::min(lo, R.src_off[i]), hi = std::max(hi, R.src_off[i] + qlens[i]);
+			if (lo > hi) lo = hi = 0;
+			char *d_src = (char*)B.d_src.ensure((size_t)(hi - lo) + 16);
+			d2d_peer(d_src, M->device, R.src + lo, R.src_dev, (size_t)(hi - lo));
+			src = d_src;
+			for (size_t i = 0; i < n; ++i) src_off[i] = R.src_off[i] - lo;
+		} else memcpy(src_off, R.src_off, n * 8);
+		uint64_t *d_pk_off = (uint64_t*)B.d_pk.ensure((2 * n8 + (packed? lay.n_words : 0) + 8) * 8);
+		h2d(d_pk_off, h, n8 * 16);
+		S.h2d_bytes = (int64_t)n * 16;
+		upload_tables(B, b, n_reads, h_tables, d_seq, S);
+		b.pk = packed? d_pk_off + 2 * n8 : 0, b.pk_off = packed? d_pk_off : 0;
+		ingest_reads(IngestArgs{src, (const int64_t*)(d_pk_off + n8), b.seq_off, b.seq_len, d_seq, (uint64_t*)b.pk, d_pk_off, d_raw, n_reads});
 	}
-	if (seg_off) {
-		const size_t n_len = (size_t)seg_off[n];
-		int32_t *d_segs = (int32_t*)B.d_segs.ensure(sizeof(int32_t) * (n + 1 + n_len));
-		h2d(d_segs, seg_off, sizeof(int32_t) * (n + 1));
-		h2d(d_segs + n + 1, seg_len, sizeof(int32_t) * n_len);
-		b.seg_off = d_segs, b.seg_len = d_segs + n + 1;
-	}
+	upload_read_extras(B, b, M, names, no_diag, seg_off, seg_len);
 	return b;
 }
 
@@ -1897,9 +1985,10 @@ static void learn_tier_routing(Model *M, const unsigned int *h)
 }
 
 // Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).  With gaf, the result is the batch's GAF text
-// (gaf_text) instead of mg_gchains_t objects.
+// (gaf_text) instead of mg_gchains_t objects.  With dev, the reads are in device memory (seqs is NULL).
 static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
-					 mg_gchains_t **gcs, int host_threads, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0, GafJob *gaf = 0)
+					 mg_gchains_t **gcs, int host_threads, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0, GafJob *gaf = 0,
+					 const DevReads *dev = 0)
 {
 	mgb_stats_t &S = sl.st;
 	memset(&S, 0, sizeof(S));
@@ -1912,8 +2001,10 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	TM.reset();
 	const BatchLayout lay(n_reads, qlens);
 	S.n_reads = n_reads, S.n_bases = lay.n_bases;
-	const BatchDev b = upload_batch(sl.stage, lay, M, n_reads, qlens, seqs, names, (o.flag & F_NO_DIAG) != 0, seg_off? seg_off->data() : 0,
-									seg_len? seg_len->data() : 0, sl.host_pool, host_threads, &TM.h2d, S);
+	const bool no_diag = (o.flag & F_NO_DIAG) != 0;
+	const int32_t *so = seg_off? seg_off->data() : 0, *sg = seg_len? seg_len->data() : 0;
+	const BatchDev b = dev? upload_batch_dev(sl.stage, lay, M, n_reads, qlens, *dev, names, no_diag, so, sg, &TM.h2d, S)
+						  : upload_batch(sl.stage, lay, M, n_reads, qlens, seqs, names, no_diag, so, sg, sl.host_pool, host_threads, &TM.h2d, S);
 	// ---- device buffers (all persistent: cudaMalloc/cudaFree would serialise the slots) ----
 	const PassScratch D(sl.d_scratch, n_reads);
 	void *d_meta = sl.d_meta.ensure(sizeof(ReadMeta) * n), *d_routs = sl.d_routs.ensure(sizeof(ReadOut) * n);
@@ -1977,6 +2068,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		if (attempt == 7) { set_error("output pools kept overflowing"); rc = -2; break; }
 	}
 	TM.to_stats(S);
+	if (dev) S.t_h2d_ms += dev->t_off_ms;
 	S.arena_peak = mail->arena_peak; // (the mailbox was last filled after the last pass of the batch)
 	for (int i = 0; i < 32; ++i) S.prof[i] = (uint64_t)mail->prof[i];
 	learn_tier_routing(M, mail->tier_hist);
@@ -2042,7 +2134,7 @@ static void logf_prepare(Model *M, int32_t max_qlen, MapOptDev &o)
 // assembly with the kernels of mini-batch i -- what the reference's kt_pipeline does with its step threads (gmap.c:176).
 static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 						mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
-						GafJob *gaf = 0)
+						GafJob *gaf = 0, const DevReads *dev = 0)
 {
 	for (int i = 0; i < n_reads; ++i) gcs[i] = 0;
 	if (n_reads <= 0) return 0;
@@ -2068,7 +2160,7 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		int nt = (int)p_host_threads;
 		if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
 		t_launches = 0;
-		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf);
+		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf, dev);
 	} catch (const MgbError &e) {
 		rc = e.code;
 	}
@@ -2091,13 +2183,14 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 }
 
 // The batch on every device of the index: contiguous parts of about equal bases, one host thread per device, results in input order.
+// Reads in device memory (dev) that map on a peer are copied there device to device.
 static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 						  mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
-						  GafJob *gaf = 0)
+						  GafJob *gaf = 0, const DevReads *dev = 0)
 {
 	Model *M = (Model*)gi->B;
 	const int n_dev = 1 + (int)M->peers.size();
-	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len, gaf);
+	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len, gaf, dev);
 	for (Model *P : M->peers) if (P == 0) { set_error("the index is missing on one of the MGB_DEVICES"); return MGB_E_INTERNAL; }
 	int64_t tot = 0;
 	for (int i = 0; i < n_reads; ++i) tot += qlens[i] > 0? qlens[i] : 0;
@@ -2117,12 +2210,14 @@ static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, con
 		parts[d] = *gaf, parts[d].len = 0;
 		parts[d].dest = [&texts, d](size_t n) { texts[d].resize(n + 1); return texts[d].data(); };
 	}
+	std::vector<DevReads> dparts(dev? (size_t)n_dev : 0);
+	for (size_t d = 0; d < dparts.size(); ++d) dparts[d] = *dev, dparts[d].src_off += bound[d], dparts[d].copy = d > 0;
 	std::vector<std::thread> th;
 	for (int d = 0; d < n_dev; ++d)
 		th.emplace_back([&, d]() {
 			const int b = bound[(size_t)d], e = bound[(size_t)d + 1];
-			if (e > b) rcs[(size_t)d] = map_batch_on(d == 0? M : M->peers[(size_t)d - 1], e - b, qlens + b, seqs + b, names? names + b : 0, gcs + b, opt,
-													  0, 0, gaf? &parts[(size_t)d] : 0);
+			if (e > b) rcs[(size_t)d] = map_batch_on(d == 0? M : M->peers[(size_t)d - 1], e - b, qlens + b, seqs? seqs + b : 0, names? names + b : 0, gcs + b, opt,
+													  0, 0, gaf? &parts[(size_t)d] : 0, dev? &dparts[(size_t)d] : 0);
 		});
 	for (auto &t : th) t.join();
 	int rc = 0;
@@ -2150,8 +2245,9 @@ extern "C" int mg_map_batch(const mg_idx_t *gi, int n_reads, const int *qlens, c
 	return map_batch_impl(gi, n_reads, qlens, seqs, names, gcs, opt);
 }
 
-// Fragments of several segments as the kernels take them: each fragment's segments concatenated (qsum/sq), their lengths in seg_len
-// from seg_off[f], and first[f] = n_seg[0] + ... + n_seg[f-1], the fragment's first entry in the caller's arrays.
+// Fragments of several segments as the kernels take them: each fragment's segments concatenated (qsum/sq; seqs == NULL: the lengths
+// only), their lengths in seg_len from seg_off[f], and first[f] = n_seg[0] + ... + n_seg[f-1], the fragment's first entry in the
+// caller's arrays.
 struct FragBatch {
 	std::vector<std::string> cat;
 	std::vector<int> qsum;
@@ -2166,12 +2262,14 @@ struct FragBatch {
 			seg_off[(size_t)f] = (int32_t)seg_len.size();
 			first[(size_t)f] = off;
 			const int ns = n_seg[f] > 0 && n_seg[f] <= 255? n_seg[f] : 0; // more than MG_MAX_SEG segments: no result (map-algo.c:359)
+			int sum = 0;
 			for (int j = 0; j < ns; ++j) {
 				const int l = qlens[off + j] > 0? qlens[off + j] : 0;
 				seg_len.push_back(l);
-				if (l > 0) cat[(size_t)f].append(seqs[off + j], (size_t)l);
+				if (l > 0 && seqs) cat[(size_t)f].append(seqs[off + j], (size_t)l);
+				sum += l;
 			}
-			qsum[(size_t)f] = (int)cat[(size_t)f].size(), sq[(size_t)f] = cat[(size_t)f].data();
+			qsum[(size_t)f] = sum, sq[(size_t)f] = cat[(size_t)f].data();
 			off += n_seg[f] > 0? n_seg[f] : 0;
 		}
 		seg_off[(size_t)n_frag] = (int32_t)seg_len.size();
@@ -2198,9 +2296,18 @@ extern "C" int mg_map_batch_frag(const mg_idx_t *gi, int n_frag, const int *n_se
 	return 0;
 }
 
-// Map a batch and return its GAF text, formatted on the device (mgb_gaf.cuh, gaf_text).
-extern "C" int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, const int *qlens, const char *const *seqs, const char *const *names,
-								 const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap)
+// No text: *out_len = 0, and an empty caller's buffer or no block
+static int gaf_no_text(int rc, char **out, size_t *out_len, size_t *out_cap)
+{
+	if (out_cap) { if (*out && *out_cap) (*out)[0] = 0; }
+	else *out = 0;
+	*out_len = 0;
+	return rc;
+}
+
+// The GAF text of a batch of n_frag fragments, formatted on the device (mgb_gaf.cuh, gaf_text), into (out, out_len, out_cap):
+// map(J) maps the batch with J, whose qlens are those of its sequences, as its GafJob.
+static int gaf_call(int n_frag, const int *qlens, const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap, const std::function<int(GafJob &)> &map)
 {
 	const uint64_t F_CAL_COV = 0x4000, F_INDEPEND_SEG = 0x20000; // minigraph.h:19,22
 	char *fresh = 0;
@@ -2214,36 +2321,145 @@ extern "C" int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_se
 		}
 		return *out;
 	};
-	auto fail = [&](int rc) { // no partial text
-		if (out_cap) { if (*out && *out_cap) (*out)[0] = 0; }
-		else { free(fresh); *out = 0; }
-		*out_len = 0;
-		return rc;
-	};
+	auto fail = [&](int rc) { free(fresh); return gaf_no_text(rc, out, out_len, out_cap); }; // no partial text
 	*out_len = 0;
 	if (opt->flag & (F_CAL_COV | F_INDEPEND_SEG)) { set_error("mgb_map_batch_gaf: --cov and independent segments print no per-fragment GAF record"); return fail(MGB_E_UNSUPPORTED); }
 	GafJob J;
 	J.flag = opt->flag, J.n_seg = 0, J.seg_first = 0, J.qlens = qlens, J.dest = dest, J.len = 0;
-	int rc = 0;
 	if (n_frag <= 0) {
 		char *o = dest(0);
 		if (o == 0) { set_error("mgb_map_batch_gaf: out of host memory"); return fail(MGB_E_INTERNAL); }
 		o[0] = 0;
-	} else {
-		bool single = true;
-		for (int f = 0; f < n_frag && n_seg; ++f) if (n_seg[f] != 1) single = false;
-		std::vector<mg_gchains_t*> gcs((size_t)n_frag, (mg_gchains_t*)0); // stays empty: the results go out as text
-		if (single) rc = map_batch_impl(gi, n_frag, qlens, seqs, names, gcs.data(), opt, 0, 0, &J);
-		else {
-			FragBatch fb(n_frag, n_seg, qlens, seqs);
-			J.n_seg = n_seg, J.seg_first = fb.first.data();
-			rc = map_batch_impl(gi, n_frag, fb.qsum.data(), fb.sq.data(), names, gcs.data(), opt, &fb.seg_off, &fb.seg_len, &J);
-		}
+	} else if (int rc = map(J)) {
 		if (rc < 0) return fail(rc);
 	}
 	if (out_cap == 0) *out = fresh;
 	*out_len = J.len;
 	return 0;
+}
+
+// Map a batch and return its GAF text, formatted on the device.
+extern "C" int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, const int *qlens, const char *const *seqs, const char *const *names,
+								 const mg_mapopt_t *opt, char **out, size_t *out_len, size_t *out_cap)
+{
+	return gaf_call(n_frag, qlens, opt, out, out_len, out_cap, [&](GafJob &J) {
+		bool single = true;
+		for (int f = 0; f < n_frag && n_seg; ++f) if (n_seg[f] != 1) single = false;
+		std::vector<mg_gchains_t*> gcs((size_t)n_frag, (mg_gchains_t*)0); // stays empty: the results go out as text
+		if (single) return map_batch_impl(gi, n_frag, qlens, seqs, names, gcs.data(), opt, 0, 0, &J);
+		FragBatch fb(n_frag, n_seg, qlens, seqs);
+		J.n_seg = n_seg, J.seg_first = fb.first.data();
+		return map_batch_impl(gi, n_frag, fb.qsum.data(), fb.sq.data(), names, gcs.data(), opt, &fb.seg_off, &fb.seg_len, &J);
+	});
+}
+
+// ---- reads in device memory (mgb_map_batch_dev, mgb_map_batch_dev_gaf) ----
+// A batch whose n_seq + 1 offsets d_off (sequence i is d_seq[d_off[i] .. d_off[i+1])) are in device memory: checks the buffers, copies
+// the offsets back once the caller's stream has got past the work queued on it, checks them, and gives the sequences' lengths.
+// Returns 0, or a negative code with the reason set.
+struct DevBatch {
+	std::vector<int64_t> off;
+	std::vector<int> qlen;
+	DevReads R;
+};
+static int dev_batch_prepare(const mg_idx_t *gi, const char *who, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+							 const int64_t *d_off, const mg_mapopt_t *opt, void *stream, DevBatch &D)
+{
+	auto refuse = [&](const std::string &why) { set_error(std::string(who) + ": " + why); return (int)MGB_E_UNSUPPORTED; };
+	if (gi == 0 || opt == 0 || n_frag < 0 || n_seq < 0 || seq_bytes < 0 || d_off == 0 || (seq_bytes > 0 && d_seq == 0))
+		return refuse("an index, options, the offsets, and counts and seq_bytes at least 0");
+	if (n_seg == 0 && n_seq != n_frag) return refuse("n_seq must be n_frag when n_seg is NULL");
+	if (n_seg) {
+		int64_t tot = 0;
+		for (int f = 0; f < n_frag; ++f) tot += n_seg[f] > 0? n_seg[f] : 0;
+		if (tot != n_seq) return refuse("the fragments' segments add up to " + std::to_string(tot) + ", not n_seq = " + std::to_string(n_seq));
+	}
+	const Model *M = model_of(gi);
+	D.off.assign((size_t)n_seq + 1, 0);
+	D.R.src = d_seq, D.R.src_off = 0, D.R.src_dev = M->device, D.R.copy = false, D.R.t_off_ms = 0;
+#ifdef MGB_HOSTSIM
+	(void)stream;
+	memcpy(D.off.data(), d_off, sizeof(int64_t) * ((size_t)n_seq + 1));
+#else
+	CUDA_OK(cudaSetDevice(M->device));
+	const void *bufs[2] = {d_off, seq_bytes > 0? (const void*)d_seq : 0};
+	for (int k = 0; k < 2; ++k) {
+		if (bufs[k] == 0) continue;
+		cudaPointerAttributes a;
+		const bool ok = cudaPointerGetAttributes(&a, bufs[k]) == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == M->device;
+		cudaGetLastError();
+		if (!ok) return refuse(std::string(k? "d_seq" : "d_off") + " is not device or managed memory on the index's device " + std::to_string(M->device));
+	}
+	CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+	const double t0 = now_ms();
+	CUDA_OK(cudaMemcpy(D.off.data(), d_off, sizeof(int64_t) * ((size_t)n_seq + 1), cudaMemcpyDeviceToHost));
+	D.R.t_off_ms = now_ms() - t0;
+#endif
+	D.qlen.resize((size_t)std::max(n_seq, 1));
+	for (int i = 0; i <= n_seq; ++i)
+		if (D.off[(size_t)i] < 0 || D.off[(size_t)i] > seq_bytes) return refuse("offset " + std::to_string(i) + " lies outside [0, seq_bytes]");
+	for (int i = 0; i < n_seq; ++i) {
+		const int64_t l = D.off[(size_t)i + 1] - D.off[(size_t)i];
+		if (l < 0) return refuse("the offsets decrease at sequence " + std::to_string(i));
+		if (l > INT32_MAX) return refuse("sequence " + std::to_string(i) + " is longer than INT32_MAX");
+		D.qlen[(size_t)i] = (int)l;
+	}
+	if (n_seg) { // a fragment's segments follow each other in d_seq: it is mapped from there as one read
+		for (int f = 0, i = 0; f < n_frag; ++f) {
+			const int ns = n_seg[f] > 0? n_seg[f] : 0;
+			if (D.off[(size_t)(i + ns)] - D.off[(size_t)i] > INT32_MAX) return refuse("fragment " + std::to_string(f) + " is longer than INT32_MAX");
+			i += ns;
+		}
+	}
+	return 0;
+}
+
+// The batch D.  gcs (n_seq entries, or NULL when gaf takes the results as text) as mg_map_batch_frag() fills it.
+static int dev_batch_map(const mg_idx_t *gi, int n_frag, const int *n_seg, DevBatch &D, const char *const *names, const mg_mapopt_t *opt,
+						 mg_gchains_t **gcs, GafJob *gaf)
+{
+	bool single = true;
+	for (int f = 0; f < n_frag && n_seg; ++f) if (n_seg[f] != 1) single = false;
+	std::vector<int> ones(n_seg? 0 : (size_t)n_frag, 1);
+	const int *ns = n_seg? n_seg : ones.data();
+	FragBatch fb(n_frag, ns, D.qlen.data(), 0);
+	std::vector<int64_t> src((size_t)std::max(n_frag, 1));
+	for (int f = 0; f < n_frag; ++f) src[(size_t)f] = D.off[(size_t)fb.first[(size_t)f]];
+	D.R.src_off = src.data();
+	std::vector<mg_gchains_t*> res((size_t)std::max(n_frag, 1), (mg_gchains_t*)0);
+	int rc;
+	if (single) rc = map_batch_impl(gi, n_frag, D.qlen.data(), 0, names, res.data(), opt, 0, 0, gaf, &D.R);
+	else {
+		if (gaf) gaf->n_seg = n_seg, gaf->seg_first = fb.first.data();
+		rc = map_batch_impl(gi, n_frag, fb.qsum.data(), 0, names, res.data(), opt, &fb.seg_off, &fb.seg_len, gaf, &D.R);
+	}
+	if (rc < 0 || gcs == 0) return rc;
+	for (int f = 0; f < n_frag; ++f) if (ns[f] > 0) gcs[fb.first[(size_t)f]] = res[(size_t)f];
+	return 0;
+}
+
+extern "C" int mgb_map_batch_dev(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+								 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, mg_gchains_t **gcs)
+{
+	for (int i = 0; i < n_seq && gcs; ++i) gcs[i] = 0;
+	try {
+		DevBatch D;
+		if (int rc = dev_batch_prepare(gi, "mgb_map_batch_dev", n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, opt, stream, D)) return rc;
+		if (n_frag == 0) return 0;
+		return dev_batch_map(gi, n_frag, n_seg, D, names, opt, gcs, 0);
+	} catch (const MgbError &e) { return e.code; }
+}
+
+extern "C" int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+									 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, char **out, size_t *out_len,
+									 size_t *out_cap)
+{
+	try {
+		DevBatch D;
+		if (int rc = dev_batch_prepare(gi, "mgb_map_batch_dev_gaf", n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, opt, stream, D))
+			return gaf_no_text(rc, out, out_len, out_cap);
+		return gaf_call(n_frag, D.qlen.data(), opt, out, out_len, out_cap, [&](GafJob &J) { return dev_batch_map(gi, n_frag, n_seg, D, names, opt, 0, &J); });
+	} catch (const MgbError &e) { return gaf_no_text(e.code, out, out_len, out_cap); }
 }
 
 extern "C" void mg_map_frag(const mg_idx_t *gi, int n_segs, const int *qlens, const char **seqs, mg_gchains_t **gcs, mg_tbuf_t *b, const mg_mapopt_t *opt, const char *qname)
@@ -2757,6 +2973,60 @@ static int test_sketch_impl(int k, int w, int n, const char *seq, const int64_t 
 extern "C" int mgb_test_sketch(int k, int w, int n, const char *seq, const int64_t *off, const int32_t *len, int mode, int32_t *out, mg128_t *mz, const int64_t *mz_off)
 {
 	try { return test_sketch_impl(k, w, n, seq, off, len, mode, out, (u128*)mz, mz_off); } catch (const MgbError &e) { return e.code; }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// test hook: the ingest step of reads in device memory as mgb_map_batch_dev uploads them (upload_batch_dev, k_ingest): sequence i is
+// seq[off[i] .. off[i+1]), copied to the device first.  Its ASCII copy goes to ascii_out[off[i]..], its 2-bit words (unless segmented)
+// follow those of sequence i-1 in pk_out, its flag to raw_out[i].  pk_off must be ~0 exactly for the flagged reads.
+// ---------------------------------------------------------------------------------------------------------------
+static int test_ingest_impl(int n, const char *seq, const int64_t *off, int segmented, char *ascii_out, uint64_t *pk_out, int32_t *raw_out)
+{
+	if (n < 0 || (n > 0 && (off == 0 || off[0] < 0))) { set_error("mgb_test_ingest: n at least 0 and offsets from 0"); return MGB_E_UNSUPPORTED; }
+	std::vector<int> qlen((size_t)std::max(n, 1));
+	for (int i = 0; i < n; ++i) {
+		if (off[i + 1] < off[i] || off[i + 1] - off[i] > INT32_MAX) { set_error("mgb_test_ingest: sequence " + std::to_string(i) + " has a bad length"); return MGB_E_UNSUPPORTED; }
+		qlen[(size_t)i] = (int)(off[i + 1] - off[i]);
+	}
+	if (n == 0) return 0;
+	if (int e = test_no_device()) return e;
+	auto seq_d = upload(seq, (size_t)off[n]);
+	const BatchLayout lay(n, qlen.data());
+	std::vector<int32_t> seg_off((size_t)n + 1), seg_len(qlen.begin(), qlen.begin() + n); // segmented: one segment per read
+	for (int i = 0; i <= n; ++i) seg_off[(size_t)i] = i;
+	DevReads R;
+	R.src = seq_d, R.src_off = off, R.src_dev = (int)p_device, R.copy = false, R.t_off_ms = 0;
+	DevBuf<int32_t> raw_d((size_t)n);
+	Staging stg;
+	mgb_stats_t st = {};
+	const BatchDev b = upload_batch_dev(stg, lay, 0, n, qlen.data(), R, 0, false, segmented? seg_off.data() : 0, segmented? seg_len.data() : 0, 0, st, raw_d);
+	std::vector<char> hseq(lay.seq_bytes);
+	d2h(hseq.data(), b.seq, lay.seq_bytes);
+	d2h(raw_out, raw_d, sizeof(int32_t) * (size_t)n);
+	for (int i = 0; i < n; ++i) memcpy(ascii_out + off[i], hseq.data() + lay.seq_off[(size_t)i], (size_t)qlen[(size_t)i]);
+	if (segmented) {
+		if (b.pk || b.pk_off) { set_error("mgb_test_ingest: words of fragments with segments"); return MGB_E_INTERNAL; }
+		return 0;
+	}
+	std::vector<uint64_t> pk(lay.n_words + 1), pk_off((size_t)n);
+	d2h(pk.data(), b.pk, sizeof(uint64_t) * lay.n_words);
+	d2h(pk_off.data(), b.pk_off, sizeof(uint64_t) * (size_t)n);
+	int64_t at = 0;
+	for (int i = 0; i < n; ++i) {
+		const int nw = (qlen[(size_t)i] + 31) / 32;
+		memcpy(pk_out + at, pk.data() + lay.pk_off[(size_t)i], sizeof(uint64_t) * (size_t)nw);
+		at += nw;
+		if (pk_off[(size_t)i] != (raw_out[i]? ~0ULL : lay.pk_off[(size_t)i])) {
+			set_error("mgb_test_ingest: read " + std::to_string(i) + ": pk_off does not follow its flag");
+			return MGB_E_INTERNAL;
+		}
+	}
+	return 0;
+}
+
+extern "C" int mgb_test_ingest(int n, const char *seq, const int64_t *off, int segmented, char *ascii_out, uint64_t *pk_out, int32_t *raw_out)
+{
+	try { return test_ingest_impl(n, seq, off, segmented, ascii_out, pk_out, raw_out); } catch (const MgbError &e) { return e.code; }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
