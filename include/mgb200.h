@@ -252,6 +252,43 @@ int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, int 
 						  const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, char **out, size_t *out_len,
 						  size_t *out_cap);
 
+/* Map reads that already live in device memory straight to result tables in device memory: the content of the mg_gchains_t that
+ * mgb_map_batch_dev() would give, as dense row-major tables in one block, written on the device from the result blobs (no blob
+ * crosses PCIe).  The arguments, their checks and refusals are those of mgb_map_batch_dev().  alloc(alloc_ctx, bytes) is called
+ * exactly once, from the calling thread, by every call that passes those checks, and only once mapping succeeded; it returns a
+ * block of at least `bytes` bytes of device memory on the index's device, which the caller owns (a NULL return fails the call).
+ * The call returns once the tables are written: they may be used on any stream right away.  *out receives the rows of every table,
+ * the block and the byte offset of each table in it (256-byte aligned):
+ *   MGB_REC_SEQ_CSR   int64 [n_seq + 1][3]  sequence i's first record, first linear chain and first anchor; row n_seq: the totals
+ *   MGB_REC_SEQ_INFO  int32 [n_seq][2]      has_result (1 where mgb_map_batch_dev() leaves gcs[i] non-NULL: not for an empty or
+ *                                           over-long read, nor for the non-first segments of a fragment), rep_len
+ *   MGB_REC_GC        int32 [n_rec][MGB_GC_NCOL]  the fields of mg_gchain_t in struct order but div (hash as its bits, off
+ *                                           relative to the read's linear chains), then has_cigar, n_cigar and the mg_cigar_t header
+ *   MGB_REC_GC_DIV    float [n_rec]         mg_gchain_t.div
+ *   MGB_REC_CIGAR_CSR int64 [n_rec + 1]     record k's first CIGAR operation; row n_rec: their number
+ *   MGB_REC_LC        int32 [n_lc][5]       mg_llchain_t (off relative to the read's anchors, cnt, v, score, ed)
+ *   MGB_REC_A         int64 [n_a][2]        mg128_t (x, y as their bits)
+ *   MGB_REC_CIGAR     int64 [n_cigar]       mg_cigar_t.cigar (len<<4 | op)
+ * The ds:Z strings are not in the tables: mgb_map_batch_dev() and mgb_map_batch_dev_gaf() give them.  MGB_DEVICES works as for
+ * mg_map_batch(): every part is mapped and tabled on its device and the tables are joined in input order in the one block.  In the
+ * stats of such a call, out_bytes counts the bytes copied back (what the div values need, 16 per record), t_d2h_ms covers the
+ * table kernels, those copies and the host work between them, and t_asm_ms is 0: nothing is assembled after the kernels. */
+typedef void *(*mgb_dev_alloc_fn)(void *ctx, size_t bytes);
+enum { MGB_REC_SEQ_CSR, MGB_REC_SEQ_INFO, MGB_REC_GC, MGB_REC_GC_DIV, MGB_REC_CIGAR_CSR, MGB_REC_LC, MGB_REC_A, MGB_REC_CIGAR, MGB_REC_NTAB };
+enum { /* the columns of MGB_REC_GC */
+	MGB_GC_ID, MGB_GC_PARENT, MGB_GC_OFF, MGB_GC_CNT, MGB_GC_N_ANCHOR, MGB_GC_SCORE, MGB_GC_QS, MGB_GC_QE, MGB_GC_PLEN, MGB_GC_PS,
+	MGB_GC_PE, MGB_GC_BLEN, MGB_GC_MLEN, MGB_GC_HASH, MGB_GC_SUBSC, MGB_GC_N_SUB, MGB_GC_MAPQ, MGB_GC_FLT,
+	MGB_GC_HAS_CIGAR, MGB_GC_N_CIGAR, MGB_GC_C_MLEN, MGB_GC_C_BLEN, MGB_GC_C_APLEN, MGB_GC_C_SS, MGB_GC_C_EE, MGB_GC_NCOL
+};
+typedef struct {
+	int64_t n_seq, n_rec, n_lc, n_a, n_cigar; /* rows of the tables above */
+	void *block; int64_t bytes;               /* the one block alloc() returned, and its size */
+	int64_t off[MGB_REC_NTAB];                /* byte offset of each table in the block, 256-byte aligned */
+} mgb_records_t;
+int mgb_map_batch_dev_rec(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+						  const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
+						  mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Engine controls and instrumentation (not part of the reference API)
  * ---------------------------------------------------------------------------------------------------------- */

@@ -101,6 +101,21 @@ class mgb_stats_t(C.Structure):
                 ("w_gpu_wait_ms", C.c_double), ("w_slot_wait_ms", C.c_double), ("w_upload_ms", C.c_double), ("w_pass_ms", C.c_double), ("w_redo_ms", C.c_double), ("w_download_ms", C.c_double)]
 
 
+# mgb_map_batch_dev_rec(): the tables of mgb_records_t (mgb200.h MGB_REC_*) and the columns of its GC table (MGB_GC_*)
+REC_TABLES = ("seq_csr", "seq_info", "gc", "gc_div", "cigar_csr", "lc", "a", "cigar")
+GC_COLUMNS = ("id", "parent", "off", "cnt", "n_anchor", "score", "qs", "qe", "plen", "ps", "pe", "blen", "mlen", "hash", "subsc", "n_sub",
+              "mapq", "flt", "has_cigar", "n_cigar", "c_mlen", "c_blen", "c_aplen", "c_ss", "c_ee")
+
+
+class mgb_records_t(C.Structure):
+    _fields_ = [("n_seq", C.c_int64), ("n_rec", C.c_int64), ("n_lc", C.c_int64), ("n_a", C.c_int64), ("n_cigar", C.c_int64),
+                ("block", C.c_void_p), ("bytes", C.c_int64), ("off", C.c_int64 * len(REC_TABLES))]
+
+
+# void *alloc(void *ctx, size_t bytes)
+mgb_dev_alloc_fn = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
+
+
 class mgb_reads_t(C.Structure):
     _fields_ = [("n_reads", C.c_int64), ("n_bases", C.c_int64), ("name", C.POINTER(C.c_char_p)), ("seq", C.POINTER(C.c_char_p)),
                 ("len", C.POINTER(C.c_int)), ("block", C.c_void_p)]
@@ -233,6 +248,8 @@ def bind_engine_api(lib):
     lib.mgb_map_batch_dev.argtypes = dev_args + [C.POINTER(C.POINTER(mg_gchains_t))]
     lib.mgb_map_batch_dev_gaf.restype = C.c_int
     lib.mgb_map_batch_dev_gaf.argtypes = dev_args + [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.mgb_map_batch_dev_rec.restype = C.c_int
+    lib.mgb_map_batch_dev_rec.argtypes = dev_args + [mgb_dev_alloc_fn, C.c_void_p, C.POINTER(mgb_records_t)]
     lib.mgb_test_ingest.restype = C.c_int
     lib.mgb_test_ingest.argtypes = [C.c_int, C.c_char_p, i64p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64), i32p]
     return lib

@@ -26,6 +26,7 @@
 #include "mgb_galign.cuh"
 #include "mgb_gaf.cuh"
 #include "mgb_ingest.cuh"
+#include "mgb_records.cuh"
 
 #ifndef MGB_HOSTSIM
 #include <cuda_runtime.h>
@@ -794,12 +795,6 @@ __global__ void __launch_bounds__(256) k_gaf_req(GafArgs G)
 	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
 	for (int r = warp; r < G.n; r += n_warp) gaf_requests(G, r, lane);
 }
-__device__ inline int gaf_next_read(unsigned int *next, int lane)
-{
-	unsigned int r = 0;
-	if (lane == 0) r = atomicAdd(next, 1u);
-	return (int)__shfl_sync(0xffffffffu, r, 0);
-}
 __global__ void __launch_bounds__(256) k_gaf_count(GafArgs G)
 {
 	const int lane = threadIdx.x & 31;
@@ -808,19 +803,20 @@ __global__ void __launch_bounds__(256) k_gaf_count(GafArgs G)
 		if (lane == 0) G.off[r] = n;
 	}
 }
-__global__ void __launch_bounds__(1024) k_gaf_scan(GafArgs G)
+// v[0 .. n) replaced by its exclusive prefix sum, v[n] = the total (the GAF texts' offsets, the records' first CIGAR operations)
+__global__ void __launch_bounds__(1024) k_scan_u64(uint64_t *v, int n)
 {
 	__shared__ uint64_t part[1024];
-	const int tid = threadIdx.x, per = (G.n + 1023) / 1024;
-	const int r0 = tid * per < G.n? tid * per : G.n, r1 = r0 + per < G.n? r0 + per : G.n;
+	const int tid = threadIdx.x, per = (n + 1023) / 1024;
+	const int r0 = tid * per < n? tid * per : n, r1 = r0 + per < n? r0 + per : n;
 	uint64_t sum = 0;
-	for (int r = r0; r < r1; ++r) sum += G.off[r];
+	for (int r = r0; r < r1; ++r) sum += v[r];
 	part[tid] = sum;
 	__syncthreads();
-	if (tid == 0) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[i]; part[i] = acc; acc += c; } G.off[G.n] = acc; }
+	if (tid == 0) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[i]; part[i] = acc; acc += c; } v[n] = acc; }
 	__syncthreads();
 	uint64_t acc = part[tid];
-	for (int r = r0; r < r1; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
+	for (int r = r0; r < r1; ++r) { const uint64_t c = v[r]; v[r] = acc; acc += c; }
 }
 __global__ void __launch_bounds__(256) k_gaf_write(GafArgs G)
 {
@@ -848,20 +844,29 @@ static void gaf_list_requests(const GafArgs &G)
 #endif
 	++t_launches;
 }
+static void scan_u64(uint64_t *v, int n)
+{
+#ifndef MGB_HOSTSIM
+	k_scan_u64<<<1, 1024, 0, t_stream>>>(v, n);
+	CUDA_OK(cudaGetLastError());
+#else
+	uint64_t acc = 0;
+	for (int r = 0; r < n; ++r) { const uint64_t c = v[r]; v[r] = acc; acc += c; }
+	v[n] = acc;
+#endif
+	++t_launches;
+}
 // the length of every read's text and where it starts, in read order (G.off; G.off[n]: the whole text); G.next[0] zeroed
 static void gaf_offsets(const GafArgs &G)
 {
 #ifndef MGB_HOSTSIM
 	k_gaf_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
-	k_gaf_scan<<<1, 1024, 0, t_stream>>>(G);
 	CUDA_OK(cudaGetLastError());
 #else
 	sim_each_read(G.n, [&](int r, int lane) { const uint64_t b = gaf_read(G, r, 0, lane); if (lane == 0) G.off[r] = b; return (int)b; });
-	uint64_t acc = 0;
-	for (int r = 0; r < G.n; ++r) { const uint64_t c = G.off[r]; G.off[r] = acc; acc += c; }
-	G.off[G.n] = acc;
 #endif
-	t_launches += 2;
+	++t_launches;
+	scan_u64(G.off, G.n);
 }
 // the text (G.text); G.next[1] zeroed
 static void gaf_write(const GafArgs &G)
@@ -991,6 +996,7 @@ struct Model {
 		Staging stage;
 		GrowBuf h_out{true}, h_mail{true}, h_routs{true}, d_meta, d_routs, d_scratch, d_jobq, d_order, d_packed, d_packoff, d_lab_new, d_pool[N_POOLS];
 		GrowBuf h_gaf{true}, d_gaf, d_gaf_text; // mgb_map_batch_gaf(): the reads' names and segments, requests and cells; the text
+		GrowBuf h_rec{true}, d_rec; // mgb_map_batch_dev_rec(): SEQ_CSR, SEQ_INFO and the reads' rows; CIGAR counts, div requests and values
 		mgb::HostPool host_pool; // packing and result assembly of the batch on this slot
 		Workers W;
 		mgb_stats_t st;
@@ -1445,7 +1451,6 @@ static float gc_div(int32_t n_mini, int32_t n_anchor, int32_t q_span)
 
 static mg_gchains_t *build_result(const ReadOut &ro, const char *pool)
 {
-	const char *blob = pool + ro.blob_off;
 	mg_gchains_t *gs = (mg_gchains_t*)calloc(1, sizeof(mg_gchains_t));
 	gs->rep_len = ro.rep_len;
 	if (ro.n_gc == 0) return gs; // reference: gchain1.c:460 returns the bare struct
@@ -1453,11 +1458,10 @@ static mg_gchains_t *build_result(const ReadOut &ro, const char *pool)
 	gs->gc = (mg_gchain_t*)calloc((size_t)ro.n_gc, sizeof(mg_gchain_t));
 	gs->lc = (mg_llchain_t*)malloc((size_t)(ro.n_lc > 0? ro.n_lc : 1) * sizeof(mg_llchain_t));
 	gs->a = (mg128_t*)malloc((size_t)(ro.n_a > 0? ro.n_a : 1) * sizeof(mg128_t));
-	const GChain *d = (const GChain*)blob;
-	uint64_t off_lc = align8((uint64_t)ro.n_gc * sizeof(GChain));
-	uint64_t off_a = off_lc + align8((uint64_t)ro.n_lc * sizeof(LLChain));
-	memcpy(gs->lc, blob + off_lc, (size_t)ro.n_lc * sizeof(mg_llchain_t));
-	memcpy(gs->a, blob + off_a, (size_t)ro.n_a * sizeof(mg128_t));
+	const ReadBlob B = read_blob(pool, ro);
+	const GChain *d = B.gc;
+	memcpy(gs->lc, B.lc, (size_t)ro.n_lc * sizeof(mg_llchain_t));
+	memcpy(gs->a, B.a, (size_t)ro.n_a * sizeof(mg128_t));
 	for (int32_t i = 0; i < ro.n_gc; ++i) {
 		mg_gchain_t *p = &gs->gc[i];
 		const GChain *s = &d[i];
@@ -1657,6 +1661,117 @@ static int gaf_text(Model *M, Model::Slot &sl, GafJob &J, int n_reads, const int
 	J.len = (size_t)total;
 	S.out_bytes = (int64_t)total;
 	S.t_asm_ms = now_ms() - t_asm0;
+	return 0;
+}
+
+// mgb_map_batch_dev_rec(): the segments of every read of the part, and where its tables go
+struct RecJob {
+	const int *n_seg;  // segments per read, NULL: one
+	std::function<void(mgb_records_t &)> dest; // given the rows (and offsets, bytes) of the tables, sets .block: device memory on the part's device, or NULL
+	void *stream;      // the caller's stream (reads of the block are ordered after the work queued on it)
+	mgb_records_t rec; // the part's tables as written
+};
+
+// Every table's offset in the block (256-byte aligned) and the block's size, from the rows r.n_*
+static void rec_layout(mgb_records_t &r)
+{
+	const int64_t bytes[MGB_REC_NTAB] = {24 * (r.n_seq + 1), 8 * r.n_seq, 4 * MGB_GC_NCOL * r.n_rec, 4 * r.n_rec, 8 * (r.n_rec + 1), 20 * r.n_lc, 16 * r.n_a, 8 * r.n_cigar};
+	int64_t at = 0;
+	for (int t = 0; t < MGB_REC_NTAB; ++t) r.off[t] = at, at += (bytes[t] + 255) & ~(int64_t)255;
+	r.bytes = at;
+}
+
+// the block of J.dest, ordered after the caller's stream; false when there is none
+static bool rec_block(RecJob &J, mgb_records_t &r)
+{
+	rec_layout(r);
+	r.block = 0;
+	J.dest(r);
+	if (r.block == 0) { set_error("mgb_map_batch_dev_rec: the allocator returned no block of " + std::to_string(r.bytes) + " bytes"); return false; }
+#ifndef MGB_HOSTSIM
+	CUDA_OK(cudaStreamSynchronize((cudaStream_t)J.stream)); // a block the caller's allocator reuses may still be read by work queued there
+#endif
+	return true;
+}
+
+// The tables of a mapped sub-batch, written on the device from the blobs in the output pool (mgb_records.cuh): SEQ_CSR and the
+// reads' rows from the host, the CIGAR operations counted and scanned, the div requests to the host and the values back up, then
+// the block from J.dest and the write pass.  Returns 0 or a negative code.
+static int rec_tables(Model::Slot &sl, RecJob &J, int n_reads, const ReadMeta *meta, const ReadOut *routs, const ReadOut *d_routs,
+					  const char *d_pool, int host_threads, mgb_stats_t &S, EvTimer &tm_d2h)
+{
+	const size_t n = (size_t)n_reads;
+	auto has_result = [&](size_t f) { return (J.n_seg == 0 || J.n_seg[f] > 0) && read_status(meta[f], routs[f]) != 1; }; // mgb_map_batch_dev() leaves one
+	mgb_records_t &R = J.rec;
+	memset(&R, 0, sizeof(R));
+	for (size_t f = 0; f < n; ++f) {
+		R.n_seq += J.n_seg? std::max(J.n_seg[f], 0) : 1;
+		if (has_result(f)) R.n_rec += std::max(routs[f].n_gc, 0);
+	}
+	if (R.n_rec >= INT32_MAX) { set_error("mgb_map_batch_dev_rec: more than INT32_MAX records in one batch"); return MGB_E_UNSUPPORTED; }
+	const size_t n_seq = (size_t)R.n_seq, n_rec = (size_t)R.n_rec;
+	auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
+	// host and device: seq_csr | seq_info | row_of (uploaded), then on the device cig_off | req | next, on the host req | div
+	const size_t o_info = al(24 * (n_seq + 1)), o_row = o_info + al(8 * n_seq), o_up = o_row + al(4 * n);
+	const size_t o_cig = o_up, o_req = o_cig + al(8 * (n_rec + 1)), o_next = o_req + al(sizeof(GafReq) * n_rec);
+	const size_t o_hdiv = o_up + al(sizeof(GafReq) * n_rec);
+	char *h = (char*)sl.h_rec.ensure(o_hdiv + 4 * n_rec + 16), *d = (char*)sl.d_rec.ensure(o_next + 16);
+	int64_t *csr = (int64_t*)h;
+	int32_t *info = (int32_t*)(h + o_info), *row_of = (int32_t*)(h + o_row);
+	GafReq *hreq = (GafReq*)(h + o_up);
+	float *hdiv = (float*)(h + o_hdiv);
+	int64_t rec = 0, lc = 0, a = 0;
+	for (size_t f = 0, s = 0; f < n; ++f) {
+		const int ns = J.n_seg? std::max(J.n_seg[f], 0) : 1;
+		const bool has = has_result(f);
+		const ReadOut &o = routs[f];
+		row_of[f] = has? (int32_t)s : -1;
+		for (int j = 0; j < ns; ++j, ++s) {
+			csr[3 * s] = rec, csr[3 * s + 1] = lc, csr[3 * s + 2] = a;
+			info[2 * s] = has && j == 0, info[2 * s + 1] = has && j == 0? o.rep_len : 0;
+			if (has && j == 0 && o.n_gc > 0) rec += o.n_gc, lc += o.n_lc, a += o.n_a;
+		}
+	}
+	csr[3 * n_seq] = rec, csr[3 * n_seq + 1] = R.n_lc = lc, csr[3 * n_seq + 2] = R.n_a = a;
+	RecArgs A;
+	A.routs = d_routs, A.pool = d_pool, A.n = n_reads;
+	A.row_of = (const int32_t*)(d + o_row), A.seq_csr = (const int64_t*)d;
+	A.cig_off = (uint64_t*)(d + o_cig), A.req = (GafReq*)(d + o_req), A.next = (unsigned int*)(d + o_next);
+	{
+		Span span(&tm_d2h);
+		h2d(d, h, o_up);
+		S.h2d_bytes += (int64_t)o_up;
+#ifndef MGB_HOSTSIM
+		k_rec_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
+		CUDA_OK(cudaGetLastError());
+#else
+		sim_each_read(n_reads, [&](int r, int lane) { rec_read(A, r, lane, false); return 0; });
+#endif
+		++t_launches;
+		scan_u64(A.cig_off, (int)n_rec);
+		d2h_async(hreq, A.req, sizeof(GafReq) * n_rec);
+		d2h(&R.n_cigar, A.cig_off + n_rec, 8);
+		S.out_bytes = (int64_t)(sizeof(GafReq) * n_rec + 8);
+		pfor(sl.host_pool, host_threads, (int64_t)n_rec, [&](int64_t k) { hdiv[k] = gc_div(hreq[k].a, hreq[k].b, hreq[k].q_span); });
+		if (!rec_block(J, R)) return MGB_E_INTERNAL;
+		char *b = (char*)R.block;
+		d2d(b + R.off[MGB_REC_SEQ_CSR], d, 24 * (n_seq + 1));
+		d2d(b + R.off[MGB_REC_SEQ_INFO], d + o_info, 8 * n_seq);
+		d2d(b + R.off[MGB_REC_CIGAR_CSR], A.cig_off, 8 * (n_rec + 1));
+		h2d_async(b + R.off[MGB_REC_GC_DIV], hdiv, 4 * n_rec);
+		S.h2d_bytes += (int64_t)(4 * n_rec);
+		A.gc = (int32_t*)(b + R.off[MGB_REC_GC]), A.lc = (uint32_t*)(b + R.off[MGB_REC_LC]);
+		A.a = (uint64_t*)(b + R.off[MGB_REC_A]), A.cigar = (uint64_t*)(b + R.off[MGB_REC_CIGAR]);
+		dzero(A.next, sizeof(unsigned int));
+#ifndef MGB_HOSTSIM
+		k_rec_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
+		CUDA_OK(cudaGetLastError());
+#else
+		sim_each_read(n_reads, [&](int r, int lane) { rec_read(A, r, lane, true); return 0; });
+#endif
+		++t_launches;
+	}
+	dsync();
 	return 0;
 }
 
@@ -1985,10 +2100,11 @@ static void learn_tier_routing(Model *M, const unsigned int *h)
 }
 
 // Map reads [0, n_reads) of one sub-batch on the calling thread's stream (slot `sl`).  With gaf, the result is the batch's GAF text
-// (gaf_text) instead of mg_gchains_t objects.  With dev, the reads are in device memory (seqs is NULL).
+// (gaf_text) instead of mg_gchains_t objects; with rec, its tables in device memory (rec_tables).  With dev, the reads are in device
+// memory (seqs is NULL).
 static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 					 mg_gchains_t **gcs, int host_threads, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0, GafJob *gaf = 0,
-					 const DevReads *dev = 0)
+					 const DevReads *dev = 0, RecJob *rec = 0)
 {
 	mgb_stats_t &S = sl.st;
 	memset(&S, 0, sizeof(S));
@@ -2060,7 +2176,7 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 		if (use_lab) { S.n_lab_new = (int64_t)mail->lab_n[0], S.n_lab_big = (int64_t)mail->lab_n[1]; lab_after_batch(M, mail->lab_n[0]); }
 		d_out = P.L.c.out;
 		if (!pool_full) { // blobs into read order, then to the host in pieces (the assembly below follows piece by piece)
-			if (!gaf) hout = download_blobs(sl, n_reads, routs, d_out, std::min<uint64_t>(mail->pools[P_OUT].used, cap[P_OUT]), TM.d2h, S);
+			if (!gaf && !rec) hout = download_blobs(sl, n_reads, routs, d_out, std::min<uint64_t>(mail->pools[P_OUT].used, cap[P_OUT]), TM.d2h, S);
 			break;
 		}
 		// grow whatever overflowed (used counts keep growing past cap, so they tell how much was wanted)
@@ -2092,6 +2208,13 @@ static int map_range(Model *M, Model::Slot &sl, const MapOptDev &o, int n_reads,
 	if (gaf) {
 		rc = gaf_text(M, sl, *gaf, n_reads, qlens, names, routs, (const ReadOut*)sl.d_routs.p, d_out, host_threads, S, TM.d2h);
 		S.t_d2h_ms = TM.d2h.ms(); // the GAF kernels + the pieces of the copy
+		S.t_host_ms = now_ms() - t_host0;
+		return rc;
+	}
+	if (rec) {
+		rc = rec_tables(sl, *rec, n_reads, meta, routs, (const ReadOut*)sl.d_routs.p, d_out, host_threads, S, TM.d2h);
+		S.t_d2h_ms = TM.d2h.ms(); // the table kernels + their copies and the host work between them; t_asm_ms stays 0: the tables are final
+		                          // when the write pass ends
 		S.t_host_ms = now_ms() - t_host0;
 		return rc;
 	}
@@ -2134,7 +2257,7 @@ static void logf_prepare(Model *M, int32_t max_qlen, MapOptDev &o)
 // assembly with the kernels of mini-batch i -- what the reference's kt_pipeline does with its step threads (gmap.c:176).
 static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 						mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
-						GafJob *gaf = 0, const DevReads *dev = 0)
+						GafJob *gaf = 0, const DevReads *dev = 0, RecJob *rec = 0)
 {
 	for (int i = 0; i < n_reads; ++i) gcs[i] = 0;
 	if (n_reads <= 0) return 0;
@@ -2160,7 +2283,7 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 		int nt = (int)p_host_threads;
 		if (nt <= 0) { nt = (int)std::thread::hardware_concurrency(); if (nt > 16) nt = 16; if (nt < 1) nt = 1; }
 		t_launches = 0;
-		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf, dev);
+		rc = map_range(M, sl, o, n_reads, qlens, seqs, names, gcs, nt, seg_off, seg_len, gaf, dev, rec);
 	} catch (const MgbError &e) {
 		rc = e.code;
 	}
@@ -2182,15 +2305,65 @@ static int map_batch_on(Model *M, int n_reads, const int *qlens, const char *con
 	return rc;
 }
 
+// The rows of totals of R's block (SEQ_CSR row n_seq, CIGAR_CSR row n_rec), on the calling thread's stream, which is synchronised
+static void rec_totals(const mgb_records_t &R)
+{
+	const int64_t tot[4] = {R.n_rec, R.n_lc, R.n_a, R.n_cigar};
+	char *b = (char*)R.block;
+	h2d_async(b + R.off[MGB_REC_SEQ_CSR] + 24 * R.n_seq, tot, 24);
+	h2d_async(b + R.off[MGB_REC_CIGAR_CSR] + 8 * R.n_rec, tot + 3, 8);
+	dsync();
+}
+
+// The tables of the parts of a batch (parts[d].rec, each in its own block on device dev[d]) joined in input order into the block of
+// J on M's device: every table copied behind those of the parts before, the CSR rows raised by the rows before, the totals written
+// last.  On the caller's stream.  Returns 0 or a negative code.
+static int rec_join(Model *M, RecJob &J, const std::vector<RecJob> &parts, const std::vector<int> &dev)
+{
+	mgb_records_t &R = J.rec;
+	memset(&R, 0, sizeof(R));
+	for (const RecJob &p : parts) R.n_seq += p.rec.n_seq, R.n_rec += p.rec.n_rec, R.n_lc += p.rec.n_lc, R.n_a += p.rec.n_a, R.n_cigar += p.rec.n_cigar;
+#ifndef MGB_HOSTSIM
+	dev_bind(M->device, (cudaStream_t)J.stream);
+#endif
+	if (!rec_block(J, R)) return MGB_E_INTERNAL;
+	enum { SEQ, REC, LC, A, CIG };
+	static const int kind[MGB_REC_NTAB] = {SEQ, SEQ, REC, REC, REC, LC, A, CIG};
+	static const int64_t row_bytes[MGB_REC_NTAB] = {24, 8, 4 * MGB_GC_NCOL, 4, 8, 20, 16, 8};
+	char *b = (char*)R.block;
+	int64_t at[5] = {0, 0, 0, 0, 0}; // rows of the parts before
+	for (size_t d = 0; d < parts.size(); ++d) {
+		const mgb_records_t &p = parts[d].rec;
+		const int64_t rows[5] = {p.n_seq, p.n_rec, p.n_lc, p.n_a, p.n_cigar};
+		if (p.block)
+			for (int t = 0; t < MGB_REC_NTAB; ++t)
+				d2d_peer(b + R.off[t] + at[kind[t]] * row_bytes[t], M->device, (const char*)p.block + p.off[t], dev[d], (size_t)(rows[kind[t]] * row_bytes[t]));
+		const RecRebase rb[2] = {{(int64_t*)(b + R.off[MGB_REC_SEQ_CSR]) + 3 * at[SEQ], p.n_seq, 3, {at[REC], at[LC], at[A]}},
+								 {(int64_t*)(b + R.off[MGB_REC_CIGAR_CSR]) + at[REC], p.n_rec, 1, {at[CIG], 0, 0}}};
+		for (const RecRebase &B : rb) {
+			if (B.n == 0 || (B.base[0] == 0 && B.base[1] == 0 && B.base[2] == 0)) continue;
+#ifndef MGB_HOSTSIM
+			k_rec_rebase<<<(int)std::min<int64_t>((B.n + 255) / 256, dev_sm_count() * 8), 256, 0, t_stream>>>(B);
+			CUDA_OK(cudaGetLastError());
+#else
+			for (int64_t i = 0; i < B.n; ++i) rec_rebase_row(B, i);
+#endif
+		}
+		for (int k = 0; k < 5; ++k) at[k] += rows[k];
+	}
+	rec_totals(R);
+	return 0;
+}
+
 // The batch on every device of the index: contiguous parts of about equal bases, one host thread per device, results in input order.
 // Reads in device memory (dev) that map on a peer are copied there device to device.
 static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 						  mg_gchains_t **gcs, const mg_mapopt_t *opt, const std::vector<int32_t> *seg_off = 0, const std::vector<int32_t> *seg_len = 0,
-						  GafJob *gaf = 0, const DevReads *dev = 0)
+						  GafJob *gaf = 0, const DevReads *dev = 0, RecJob *rec = 0)
 {
 	Model *M = (Model*)gi->B;
 	const int n_dev = 1 + (int)M->peers.size();
-	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len, gaf, dev);
+	if (n_dev == 1 || seg_off || n_reads < 2 * n_dev) return map_batch_on(M, n_reads, qlens, seqs, names, gcs, opt, seg_off, seg_len, gaf, dev, rec);
 	for (Model *P : M->peers) if (P == 0) { set_error("the index is missing on one of the MGB_DEVICES"); return MGB_E_INTERNAL; }
 	int64_t tot = 0;
 	for (int i = 0; i < n_reads; ++i) tot += qlens[i] > 0? qlens[i] : 0;
@@ -2212,16 +2385,32 @@ static int map_batch_impl(const mg_idx_t *gi, int n_reads, const int *qlens, con
 	}
 	std::vector<DevReads> dparts(dev? (size_t)n_dev : 0);
 	for (size_t d = 0; d < dparts.size(); ++d) dparts[d] = *dev, dparts[d].src_off += bound[d], dparts[d].copy = d > 0;
+	// the tables of each part in a block of its own on its device, joined into the caller's block below
+	struct PartBlocks {
+		std::vector<int> dev; std::vector<void*> p;
+		~PartBlocks() { for (size_t d = 0; d < p.size(); ++d) if (p[d]) dev_ok(dev[d]), dfree(p[d]); if (!p.empty()) dev_ok(dev[0]); }
+	} rb;
+	std::vector<RecJob> rparts(rec? (size_t)n_dev : 0);
+	rb.p.assign(rparts.size(), (void*)0);
+	for (size_t d = 0; d < rparts.size(); ++d) {
+		rparts[d] = *rec;
+		memset(&rparts[d].rec, 0, sizeof(mgb_records_t));
+		rb.dev.push_back(d == 0? M->device : M->peers[d - 1]->device);
+		rparts[d].dest = [&rb, d](mgb_records_t &r) { r.block = rb.p[d] = dmalloc((size_t)r.bytes); };
+	}
 	std::vector<std::thread> th;
 	for (int d = 0; d < n_dev; ++d)
 		th.emplace_back([&, d]() {
 			const int b = bound[(size_t)d], e = bound[(size_t)d + 1];
 			if (e > b) rcs[(size_t)d] = map_batch_on(d == 0? M : M->peers[(size_t)d - 1], e - b, qlens + b, seqs? seqs + b : 0, names? names + b : 0, gcs + b, opt,
-													  0, 0, gaf? &parts[(size_t)d] : 0, dev? &dparts[(size_t)d] : 0);
+													  0, 0, gaf? &parts[(size_t)d] : 0, dev? &dparts[(size_t)d] : 0, rec? &rparts[(size_t)d] : 0);
 		});
 	for (auto &t : th) t.join();
 	int rc = 0;
 	for (int d = 0; d < n_dev; ++d) if (rcs[(size_t)d] < 0 && rc == 0) rc = rcs[(size_t)d];
+	if (rc == 0 && rec) {
+		try { rc = rec_join(M, *rec, rparts, rb.dev); } catch (const MgbError &e) { rc = e.code; }
+	}
 	if (rc == 0 && gaf) {
 		size_t tot = 0;
 		for (const GafJob &p : parts) tot += p.len;
@@ -2414,9 +2603,9 @@ static int dev_batch_prepare(const mg_idx_t *gi, const char *who, int n_frag, co
 	return 0;
 }
 
-// The batch D.  gcs (n_seq entries, or NULL when gaf takes the results as text) as mg_map_batch_frag() fills it.
+// The batch D.  gcs (n_seq entries, or NULL when gaf takes the results as text or rec as tables) as mg_map_batch_frag() fills it.
 static int dev_batch_map(const mg_idx_t *gi, int n_frag, const int *n_seg, DevBatch &D, const char *const *names, const mg_mapopt_t *opt,
-						 mg_gchains_t **gcs, GafJob *gaf)
+						 mg_gchains_t **gcs, GafJob *gaf, RecJob *rec = 0)
 {
 	bool single = true;
 	for (int f = 0; f < n_frag && n_seg; ++f) if (n_seg[f] != 1) single = false;
@@ -2428,10 +2617,11 @@ static int dev_batch_map(const mg_idx_t *gi, int n_frag, const int *n_seg, DevBa
 	D.R.src_off = src.data();
 	std::vector<mg_gchains_t*> res((size_t)std::max(n_frag, 1), (mg_gchains_t*)0);
 	int rc;
-	if (single) rc = map_batch_impl(gi, n_frag, D.qlen.data(), 0, names, res.data(), opt, 0, 0, gaf, &D.R);
+	if (single) rc = map_batch_impl(gi, n_frag, D.qlen.data(), 0, names, res.data(), opt, 0, 0, gaf, &D.R, rec);
 	else {
 		if (gaf) gaf->n_seg = n_seg, gaf->seg_first = fb.first.data();
-		rc = map_batch_impl(gi, n_frag, fb.qsum.data(), 0, names, res.data(), opt, &fb.seg_off, &fb.seg_len, gaf, &D.R);
+		if (rec) rec->n_seg = n_seg;
+		rc = map_batch_impl(gi, n_frag, fb.qsum.data(), 0, names, res.data(), opt, &fb.seg_off, &fb.seg_len, gaf, &D.R, rec);
 	}
 	if (rc < 0 || gcs == 0) return rc;
 	for (int f = 0; f < n_frag; ++f) if (ns[f] > 0) gcs[fb.first[(size_t)f]] = res[(size_t)f];
@@ -2460,6 +2650,34 @@ extern "C" int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *
 			return gaf_no_text(rc, out, out_len, out_cap);
 		return gaf_call(n_frag, D.qlen.data(), opt, out, out_len, out_cap, [&](GafJob &J) { return dev_batch_map(gi, n_frag, n_seg, D, names, opt, 0, &J); });
 	} catch (const MgbError &e) { return gaf_no_text(e.code, out, out_len, out_cap); }
+}
+
+extern "C" int mgb_map_batch_dev_rec(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+									 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
+									 mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out)
+{
+	if (out) memset(out, 0, sizeof(*out));
+	try {
+		if (alloc == 0 || out == 0) { set_error("mgb_map_batch_dev_rec: an allocator and an mgb_records_t for the tables"); return MGB_E_UNSUPPORTED; }
+		DevBatch D;
+		if (int rc = dev_batch_prepare(gi, "mgb_map_batch_dev_rec", n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, opt, stream, D)) return rc;
+		RecJob J;
+		J.n_seg = 0, J.stream = stream;
+		J.dest = [&](mgb_records_t &r) { r.block = alloc(alloc_ctx, (size_t)r.bytes); };
+		memset(&J.rec, 0, sizeof(J.rec));
+		int rc = 0;
+		if (n_frag == 0) { // no read: the two rows of totals alone, all 0
+			const Model *M = model_of(gi);
+			struct Unbind { int dev; ~Unbind() { dev_bind(dev, 0); } } unbind{M->device}; // (also when a CUDA call throws)
+#ifndef MGB_HOSTSIM
+			dev_bind(M->device, (cudaStream_t)stream);
+#endif
+			if (!rec_block(J, J.rec)) rc = MGB_E_INTERNAL;
+			else rec_totals(J.rec);
+		} else rc = dev_batch_map(gi, n_frag, n_seg, D, names, opt, 0, 0, &J);
+		if (rc == 0) *out = J.rec;
+		return rc;
+	} catch (const MgbError &e) { return e.code; }
 }
 
 extern "C" void mg_map_frag(const mg_idx_t *gi, int n_segs, const int *qlens, const char **seqs, mg_gchains_t **gcs, mg_tbuf_t *b, const mg_mapopt_t *opt, const char *qname)

@@ -114,24 +114,12 @@ MG_HD inline void gaf_list(GafOut &o, int32_t n, const F &item)
 	}
 }
 
-// the blobs of read r
-struct GafBlob { const GChain *gc; const LLChain *lc; const u128 *a; };
-MG_HD inline GafBlob gaf_blob(const GafArgs &G, const ReadOut &ro)
-{
-	GafBlob b;
-	const char *blob = G.pool + ro.blob_off;
-	b.gc = (const GChain*)blob;
-	b.lc = (const LLChain*)(blob + align8((uint64_t)ro.n_gc * sizeof(GChain)));
-	b.a = (const u128*)((const char*)b.lc + align8((uint64_t)ro.n_lc * sizeof(LLChain)));
-	return b;
-}
-
 // the requests of read r (warp-uniform)
 MG_HD inline void gaf_requests(const GafArgs &G, int r, int lane)
 {
 	const ReadOut &ro = G.routs[r];
 	if (ro.n_gc == 0) return;
-	const GafBlob B = gaf_blob(G, ro);
+	const ReadBlob B = read_blob(G.pool, ro);
 	GafReq *q = G.req + G.req_off[r];
 	for (int32_t i = lane; i < ro.n_gc; i += MGB_W) {
 		GafReq t; t.a = B.gc[i].n_mini, t.b = B.gc[i].n_anchor, t.q_span = B.gc[i].q_span, t.kind = 0;
@@ -174,7 +162,7 @@ MG_HD inline uint64_t gaf_read(const GafArgs &G, int r, char *dst, int lane)
 		if (flag & F_SHOW_UNMAP) { put_qname(); o.c('\t'); o.d(qlen); o.lit("\t0\t0\t*\t*\t0\t0\t0\t0\t0\t0\n"); }
 		return o.n;
 	}
-	const GafBlob B = gaf_blob(G, ro);
+	const ReadBlob B = read_blob(G.pool, ro);
 	const char *cells = G.cells + (uint64_t)GAF_CELL * (uint64_t)G.req_off[r];
 	int rev_sign = 0; // sticky across the records of the read (format.c:123,193)
 	for (int32_t i = 0; i < ro.n_gc; ++i) {
@@ -293,5 +281,15 @@ MG_HD inline uint64_t gaf_read(const GafArgs &G, int r, char *dst, int lane)
 	}
 	return o.n;
 }
+
+#ifndef MGB_HOSTSIM
+// the next read of a pass that pulls its reads from a counter: lane 0 takes it, the warp gets it
+__device__ inline int gaf_next_read(unsigned int *next, int lane)
+{
+	unsigned int r = 0;
+	if (lane == 0) r = atomicAdd(next, 1u);
+	return (int)__shfl_sync(0xffffffffu, r, 0);
+}
+#endif
 
 } // namespace mgb

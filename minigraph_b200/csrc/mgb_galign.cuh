@@ -503,6 +503,18 @@ struct ReadOut {
 
 MG_HD inline uint64_t align8(uint64_t x) { return (x + 7) & ~(uint64_t)7; }
 
+// the three parts of a read's first blob in the output pool (ReadOut::blob_off), each 8-byte aligned
+struct ReadBlob { const GChain *gc; const LLChain *lc; const u128 *a; };
+MG_HD inline ReadBlob read_blob(const char *pool, const ReadOut &ro)
+{
+	ReadBlob b;
+	const char *blob = pool + ro.blob_off;
+	b.gc = (const GChain*)blob;
+	b.lc = (const LLChain*)(blob + align8((uint64_t)ro.n_gc * sizeof(GChain)));
+	b.a = (const u128*)((const char*)b.lc + align8((uint64_t)ro.n_lc * sizeof(LLChain)));
+	return b;
+}
+
 // state handed from the graph-chaining DP pass to the materialisation pass
 struct GState {
 	int32_t n_lc, n_u, n_gc, n_jobs;

@@ -17,27 +17,32 @@ def pack_reads(reads, device):
     return torch.from_numpy(seq.copy()).to(device), torch.from_numpy(off).to(device)
 
 
+def _batch_args(who, gi, seq, off, names, opt, n_seg):
+    """the arguments that mgb_map_batch_dev*() share, after the checks of a (seq, off) pair"""
+    import torch
+    if opt is None:
+        raise TypeError("%s: opt is the mg_mapopt_t that mg_index() updated" % who)
+    if seq.dtype != torch.uint8 or off.dtype != torch.int64:
+        raise TypeError("%s: seq must be torch.uint8 and off torch.int64, not %s and %s" % (who, seq.dtype, off.dtype))
+    if not (seq.is_cuda and off.is_cuda and seq.device == off.device):
+        raise ValueError("%s: seq and off must be CUDA tensors on one device (%s, %s)" % (who, seq.device, off.device))
+    if not (seq.is_contiguous() and off.is_contiguous()) or seq.dim() != 1 or off.dim() != 1 or off.numel() < 1:
+        raise ValueError("%s: seq and off must be contiguous 1-D tensors, off with n + 1 entries" % who)
+    n_seq = off.numel() - 1
+    n_frag = len(n_seg) if n_seg is not None else n_seq
+    cnseg = (C.c_int * max(1, n_frag))(*n_seg) if n_seg is not None else None
+    cnames = (C.c_char_p * max(1, n_frag))(*names) if names is not None else None
+    stream = torch.cuda.current_stream(seq.device).cuda_stream
+    return n_seq, (gi, n_frag, cnseg, n_seq, seq.data_ptr(), seq.numel(), off.data_ptr(), cnames, C.byref(opt), stream)
+
+
 def map_cuda_reads(lib, gi, seq, off, names=None, opt=None, n_seg=None, gaf=True):
     """Map the reads of (seq, off) with the index gi and the options opt (the mg_mapopt_t that mg_index() updated), ordered after
     the work queued on the current stream.  n_seg: segments per fragment (read pairs), or None for single-segment reads; names:
     one bytes object per fragment, or None.  Returns the GAF text (bytes) or, with gaf=False, a ctypes array of one
     mg_gchains_t pointer per sequence, owned by the caller (mgb_free_batch).  Raises RuntimeError with the library's reason when
     it refuses the batch (for instance tensors on another device than the index's)."""
-    import torch
-    if opt is None:
-        raise TypeError("map_cuda_reads: opt is the mg_mapopt_t that mg_index() updated")
-    if seq.dtype != torch.uint8 or off.dtype != torch.int64:
-        raise TypeError("map_cuda_reads: seq must be torch.uint8 and off torch.int64, not %s and %s" % (seq.dtype, off.dtype))
-    if not (seq.is_cuda and off.is_cuda and seq.device == off.device):
-        raise ValueError("map_cuda_reads: seq and off must be CUDA tensors on one device (%s, %s)" % (seq.device, off.device))
-    if not (seq.is_contiguous() and off.is_contiguous()) or seq.dim() != 1 or off.dim() != 1 or off.numel() < 1:
-        raise ValueError("map_cuda_reads: seq and off must be contiguous 1-D tensors, off with n + 1 entries")
-    n_seq = off.numel() - 1
-    n_frag = len(n_seg) if n_seg is not None else n_seq
-    cnseg = (C.c_int * max(1, n_frag))(*n_seg) if n_seg is not None else None
-    cnames = (C.c_char_p * max(1, n_frag))(*names) if names is not None else None
-    stream = torch.cuda.current_stream(seq.device).cuda_stream
-    args = (gi, n_frag, cnseg, n_seq, seq.data_ptr(), seq.numel(), off.data_ptr(), cnames, C.byref(opt), stream)
+    n_seq, args = _batch_args("map_cuda_reads", gi, seq, off, names, opt, n_seg)
     if gaf:
         out, ln = C.c_void_p(0), C.c_size_t(0)
         rc = lib.mgb_map_batch_dev_gaf(*args, C.byref(out), C.byref(ln), None)
@@ -51,3 +56,62 @@ def map_cuda_reads(lib, gi, seq, off, names=None, opt=None, n_seg=None, gaf=True
     if rc < 0:
         raise RuntimeError("mgb_map_batch_dev: %s" % lib.mgb_last_error().decode())
     return gcs
+
+
+# the mg_gchain_t fields (and the mg_cigar_t header) of the columns of MappedTables.gc, in order (mgb200.h MGB_GC_*)
+GC_COLUMNS = capi.GC_COLUMNS
+
+
+class MappedTables:
+    """The results of a batch as tensors on the index's device, all views of one uint8 tensor (`block`), row-major:
+
+      seq_csr   int64 [n_seq + 1, 3]  sequence i's first record (row of gc), first linear chain (row of lc), first anchor (row of a);
+                                      the last row holds the totals
+      seq_info  int32 [n_seq, 2]      has_result (1 where map_cuda_reads(gaf=False) gives a non-NULL result), rep_len
+      gc        int32 [n_rec, len(GC_COLUMNS)]  one row per graph chain (hash as its bits; off counts from the read's first lc row)
+      gc_div    float32 [n_rec]       mg_gchain_t.div
+      cigar_csr int64 [n_rec + 1]     record k's CIGAR operations are cigar[cigar_csr[k]:cigar_csr[k+1]]
+      lc        int32 [n_lc, 5]       mg_llchain_t: off (from the read's first anchor row), cnt, v, score, ed
+      a         int64 [n_a, 2]        mg128_t x, y (as their bits)
+      cigar     int64 [n_cigar]       len<<4 | op
+
+    The ds:Z strings are not here (map_cuda_reads gives them)."""
+
+    def __init__(self, block, rec):
+        import torch
+        shapes = {"seq_csr": (torch.int64, (rec.n_seq + 1, 3)), "seq_info": (torch.int32, (rec.n_seq, 2)),
+                  "gc": (torch.int32, (rec.n_rec, len(GC_COLUMNS))), "gc_div": (torch.float32, (rec.n_rec,)),
+                  "cigar_csr": (torch.int64, (rec.n_rec + 1,)), "lc": (torch.int32, (rec.n_lc, 5)), "a": (torch.int64, (rec.n_a, 2)),
+                  "cigar": (torch.int64, (rec.n_cigar,))}
+        self.block = block
+        for t, name in enumerate(capi.REC_TABLES):
+            dtype, shape = shapes[name]
+            n = 1
+            for x in shape:
+                n *= x
+            o = rec.off[t]
+            size = n * torch.empty((), dtype=dtype).element_size()
+            setattr(self, name, block[o:o + size].view(dtype).view(shape))
+
+
+def map_cuda_reads_to_tensors(lib, gi, seq, off, names=None, opt=None, n_seg=None):
+    """map_cuda_reads() with the results as tables written on the device into one block that torch allocates on seq's device
+    (mgb_map_batch_dev_rec): returns a MappedTables.  The same arguments, checks and refusals as map_cuda_reads()."""
+    import torch
+    n_seq, args = _batch_args("map_cuda_reads_to_tensors", gi, seq, off, names, opt, n_seg)
+    got, failed = [], []
+
+    def alloc(ctx, nbytes):
+        try:
+            got.append(torch.empty(nbytes, dtype=torch.uint8, device=seq.device))
+            return got[-1].data_ptr()
+        except BaseException as e:  # a NULL block fails the call with a reason; the exception is raised from it below
+            failed.append(e)
+            return None
+
+    cb = capi.mgb_dev_alloc_fn(alloc)  # referenced until the call returns
+    rec = capi.mgb_records_t()
+    rc = lib.mgb_map_batch_dev_rec(*args, cb, None, C.byref(rec))
+    if rc < 0:
+        raise RuntimeError("mgb_map_batch_dev_rec: %s" % lib.mgb_last_error().decode()) from (failed[0] if failed else None)
+    return MappedTables(got[0], rec)
