@@ -87,3 +87,21 @@ def host_dev_gaf(lib, ix, names, seqs, n_seg=None):
     if out.value:
         C.CDLL(None).free(out)
     return rc, text
+
+
+def host_dev_results(lib, ix, names, seqs, n_seg=None):
+    """mgb_map_batch_dev in a simulator: (rc, one result per sequence as mgtest.gchains_to_py() gives it, None where gcs[i] is NULL)"""
+    import mgtest as T
+    from minigraph_b200 import capi
+    blob, off = flat(seqs)
+    buf = C.create_string_buffer(blob, max(1, len(blob)))
+    coff = (C.c_int64 * len(off))(*off.tolist())
+    n = len(seqs)
+    n_frag = len(n_seg) if n_seg is not None else n
+    cnseg = (C.c_int * max(1, n_frag))(*n_seg) if n_seg is not None else None
+    cnames = (C.c_char_p * max(1, n_frag))(*names) if names is not None else None
+    gcs = (C.POINTER(capi.mg_gchains_t) * max(1, n))()
+    rc = lib.mgb_map_batch_dev(ix.gi, n_frag, cnseg, n, C.addressof(buf), len(blob), C.addressof(coff), cnames, C.byref(ix.mo), None, gcs)
+    out = [T.gchains_to_py(gcs[i]) for i in range(n)]
+    lib.mgb_free_batch(n, gcs)
+    return rc, out

@@ -1,6 +1,7 @@
 """mgb_map_batch_gaf() in both simulators of the device code (one lane, and 32 lanes as fibres, which run the warp scans and the
 lane-parallel CIGAR / ds:Z / delta writes the GPU runs): GAF text byte for byte against the reference's golden files, and against
-the host writer over mg_map_batch() results under every GAF output option."""
+the host writer over mg_map_batch() results under every GAF output option; a batch split over several devices (MGB_DEVICES) gives
+the text of one."""
 import pytest
 
 import gafcases as GC
@@ -30,6 +31,10 @@ def test_goldens_reach_the_traps():
 
 def test_empty_batch_null_names_buffer_reuse_refusals(lib, workdir):
     GC.case_api(lib, workdir)
+
+
+def test_several_devices(lib, workdir):
+    GC.case_multi_device(lib, workdir)
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not built")

@@ -1,6 +1,8 @@
 """Reads in device memory, in both simulators of the device code: the ingest step (mgb_test_ingest, k_ingest's per-word code run by
-its host loop) against a restatement of mg_toupper + pack_read_scalar, and mgb_map_batch_dev_gaf() on the GAF test sets, lower case
-included, against mgb_map_batch_gaf() on the upper-cased reads."""
+its host loop) against a restatement of mg_toupper + pack_read_scalar, mgb_map_batch_dev_gaf() on the GAF test sets, lower case
+included, against mgb_map_batch_gaf() on the upper-cased reads, mgb_map_batch_dev() against mg_map_batch_frag() field by field, and
+both split over several devices (MGB_DEVICES) against one."""
+import os
 import random
 
 import pytest
@@ -8,6 +10,7 @@ import pytest
 import devreads as DR
 import gafcases as GC
 import mgtest as T
+import reccases as RC
 
 
 @pytest.fixture(scope="module", params=["hostsim", "hostsim32"])
@@ -132,3 +135,67 @@ def test_gaf_refusals_leave_no_text(lib, workdir):
         assert rc < 0 and text is None and b"independent" in lib.mgb_last_error()
     finally:
         ix.close()
+
+
+def dev_results_vs_host(lib, gfa, names, seqs, preset="lr", cigar=True, flag=0, n_seg=None):
+    """mgb_map_batch_dev() on mixed-case reads against mg_map_batch_frag() on the upper-cased ones, field by field; the latter's results"""
+    ix = GC.Index(lib, gfa, preset, cigar, flag)
+    try:
+        want = RC.host_results(lib, ix, names, seqs, n_seg)
+        rc, got = DR.host_dev_results(lib, ix, names, DR.mixed_case(seqs, 7), n_seg)
+        assert rc == 0, lib.mgb_last_error()
+    finally:
+        ix.close()
+    assert len(got) == len(want)
+    for i, (a, b) in enumerate(zip(want, got)):
+        d = T.diff_results(a, b)
+        assert d is None, "sequence %d: %s" % (i, d)
+    return want
+
+
+def test_dev_results(lib, workdir):
+    for kind, flag in (("c2", 0), ("sv_edge", GC.X)):
+        gfa, names, seqs = GC.inputs(kind, workdir)
+        want = dev_results_vs_host(lib, gfa, names, seqs, "lr", True, flag)
+        assert sum(r is not None and r["n_gc"] > 0 for r in want) > len(seqs) // 2
+
+
+def test_dev_results_read_pairs(lib, workdir):
+    gfa, names, n_seg, flat = GC.pair_inputs(workdir)
+    want = dev_results_vs_host(lib, gfa, names, flat, "sr", False, GC.SHOW_UNMAP, n_seg)
+    assert all(want[i] is None for i in range(1, len(flat), 2))
+    assert sum(r is not None for r in want) == len(names)
+
+
+def test_dev_results_empty_batch(lib, workdir):
+    gfa, _, _ = GC.inputs("c2", workdir)
+    assert dev_results_vs_host(lib, gfa, None, []) == []
+
+
+def test_dev_several_devices(lib, workdir):
+    """MGB_DEVICES: the batch cut into one part per device, each part's span of the reads copied to its device; the results and the
+    text of the parts, joined in input order, equal those of one device"""
+    gfa, names, seqs = GC.inputs("sv_edge", workdir)
+    seqs = DR.mixed_case(seqs, 2)
+    out = []
+    for devices in (None, "0,0,0"):
+        if devices:
+            os.environ["MGB_DEVICES"] = devices
+        try:
+            ix = GC.Index(lib, gfa, "lr", True, GC.X)
+        finally:
+            os.environ.pop("MGB_DEVICES", None)
+        try:
+            rc, res = DR.host_dev_results(lib, ix, names, seqs)
+            assert rc == 0, lib.mgb_last_error()
+            rc, text = DR.host_dev_gaf(lib, ix, names, seqs)
+            assert rc == 0, lib.mgb_last_error()
+            out.append((res, text))
+        finally:
+            ix.close()
+    (one, one_text), (many, many_text) = out
+    assert len(many) == len(one) >= 6
+    for i, (a, b) in enumerate(zip(one, many)):
+        d = T.diff_results(a, b)
+        assert d is None, "sequence %d: %s" % (i, d)
+    GC.check(many_text, one_text)
