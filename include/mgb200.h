@@ -269,7 +269,7 @@ int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *n_seg, int 
  *   MGB_REC_LC        int32 [n_lc][5]       mg_llchain_t (off relative to the read's anchors, cnt, v, score, ed)
  *   MGB_REC_A         int64 [n_a][2]        mg128_t (x, y as their bits)
  *   MGB_REC_CIGAR     int64 [n_cigar]       mg_cigar_t.cigar (len<<4 | op)
- * The ds:Z strings are not in the tables: mgb_map_batch_dev() and mgb_map_batch_dev_gaf() give them.  MGB_DEVICES works as for
+ * The ds:Z strings are not in these tables: mgb_map_batch_dev_rec_ds() below adds them.  MGB_DEVICES works as for
  * mg_map_batch(): every part is mapped and tabled on its device and the tables are joined in input order in the one block.  In the
  * stats of such a call, out_bytes counts the bytes copied back (what the div values need, 16 per record), t_d2h_ms covers the
  * table kernels, those copies and the host work between them, and t_asm_ms is 0: nothing is assembled after the kernels. */
@@ -288,6 +288,25 @@ typedef struct {
 int mgb_map_batch_dev_rec(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
 						  const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
 						  mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out);
+
+/* mgb_map_batch_dev_rec() with the ds:Z strings too: the same arguments, checks, refusals, allocator contract, stream rules and
+ * MGB_DEVICES behaviour, and in *out the same eight tables with the same rows and offsets.  The one block also holds three more
+ * tables, placed after those eight; *ds_out receives their rows and byte offsets in the block (256-byte aligned), and out->bytes
+ * counts them too:
+ *   MGB_REC_DS_CSR  int64 [n_rec + 1][2]  record k's first byte in MGB_REC_DS and first entry in MGB_REC_DS_OFF; row n_rec: the totals
+ *   MGB_REC_DS      uint8 [n_ds]          each record's mg_ds_t.ds (ds.len bytes, no terminating 0), records one after another
+ *   MGB_REC_DS_OFF  int32 [n_ds_off]      each record's mg_ds_t.off[0 .. ds.n_off)
+ * A record without a CIGAR (has_cigar 0: without MG_M_CIGAR, fragments with several segments, no alignment) has an empty ds.  The
+ * strings are copied on the device from the result blobs; only the two totals come back.  In the stats, out_bytes is that of
+ * mgb_map_batch_dev_rec() plus 16 bytes per part (the totals), t_d2h_ms also covers the ds copy, and t_asm_ms is 0. */
+enum { MGB_REC_DS_CSR, MGB_REC_DS, MGB_REC_DS_OFF, MGB_REC_DS_NTAB };
+typedef struct {
+	int64_t n_ds, n_ds_off;        /* rows of MGB_REC_DS and MGB_REC_DS_OFF */
+	int64_t off[MGB_REC_DS_NTAB];  /* byte offset of each table in out->block, 256-byte aligned */
+} mgb_records_ds_t;
+int mgb_map_batch_dev_rec_ds(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+							 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
+							 mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out, mgb_records_ds_t *ds_out);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Engine controls and instrumentation (not part of the reference API)

@@ -112,6 +112,14 @@ class mgb_records_t(C.Structure):
                 ("block", C.c_void_p), ("bytes", C.c_int64), ("off", C.c_int64 * len(REC_TABLES))]
 
 
+# mgb_map_batch_dev_rec_ds(): the ds tables of mgb_records_ds_t (mgb200.h MGB_REC_DS_*), in the same block after REC_TABLES
+REC_DS_TABLES = ("ds_csr", "ds", "ds_off")
+
+
+class mgb_records_ds_t(C.Structure):
+    _fields_ = [("n_ds", C.c_int64), ("n_ds_off", C.c_int64), ("off", C.c_int64 * len(REC_DS_TABLES))]
+
+
 # void *alloc(void *ctx, size_t bytes)
 mgb_dev_alloc_fn = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 
@@ -250,6 +258,8 @@ def bind_engine_api(lib):
     lib.mgb_map_batch_dev_gaf.argtypes = dev_args + [C.POINTER(C.c_void_p), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.mgb_map_batch_dev_rec.restype = C.c_int
     lib.mgb_map_batch_dev_rec.argtypes = dev_args + [mgb_dev_alloc_fn, C.c_void_p, C.POINTER(mgb_records_t)]
+    lib.mgb_map_batch_dev_rec_ds.restype = C.c_int
+    lib.mgb_map_batch_dev_rec_ds.argtypes = dev_args + [mgb_dev_alloc_fn, C.c_void_p, C.POINTER(mgb_records_t), C.POINTER(mgb_records_ds_t)]
     lib.mgb_test_ingest.restype = C.c_int
     lib.mgb_test_ingest.argtypes = [C.c_int, C.c_char_p, i64p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64), i32p]
     return lib

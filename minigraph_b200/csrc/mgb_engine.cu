@@ -804,20 +804,26 @@ __global__ void __launch_bounds__(256) k_gaf_count(GafArgs G)
 		if (lane == 0) G.off[r] = n;
 	}
 }
-// v[0 .. n) replaced by its exclusive prefix sum, v[n] = the total (the GAF texts' offsets, the records' first CIGAR operations)
+// Rows [0 .. n) of W columns (v[W r + j]) replaced by their exclusive prefix sums, column by column, row n = the totals (the GAF
+// texts' offsets, the records' first CIGAR operations; W = 2: their first ds byte and offset)
+template<int W>
 __global__ void __launch_bounds__(1024) k_scan_u64(uint64_t *v, int n)
 {
-	__shared__ uint64_t part[1024];
+	__shared__ uint64_t part[W][1024];
 	const int tid = threadIdx.x, per = (n + 1023) / 1024;
 	const int r0 = tid * per < n? tid * per : n, r1 = r0 + per < n? r0 + per : n;
-	uint64_t sum = 0;
-	for (int r = r0; r < r1; ++r) sum += v[r];
-	part[tid] = sum;
+	for (int j = 0; j < W; ++j) {
+		uint64_t sum = 0;
+		for (int r = r0; r < r1; ++r) sum += v[W * r + j];
+		part[j][tid] = sum;
+	}
 	__syncthreads();
-	if (tid == 0) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[i]; part[i] = acc; acc += c; } v[n] = acc; }
+	if (tid < W) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[tid][i]; part[tid][i] = acc; acc += c; } v[W * n + tid] = acc; }
 	__syncthreads();
-	uint64_t acc = part[tid];
-	for (int r = r0; r < r1; ++r) { const uint64_t c = v[r]; v[r] = acc; acc += c; }
+	for (int j = 0; j < W; ++j) {
+		uint64_t acc = part[j][tid];
+		for (int r = r0; r < r1; ++r) { const uint64_t c = v[W * r + j]; v[W * r + j] = acc; acc += c; }
+	}
 }
 __global__ void __launch_bounds__(256) k_gaf_write(GafArgs G)
 {
@@ -845,15 +851,18 @@ static void gaf_list_requests(const GafArgs &G)
 #endif
 	++t_launches;
 }
+template<int W = 1>
 static void scan_u64(uint64_t *v, int n)
 {
 #ifndef MGB_HOSTSIM
-	k_scan_u64<<<1, 1024, 0, t_stream>>>(v, n);
+	k_scan_u64<W><<<1, 1024, 0, t_stream>>>(v, n);
 	CUDA_OK(cudaGetLastError());
 #else
-	uint64_t acc = 0;
-	for (int r = 0; r < n; ++r) { const uint64_t c = v[r]; v[r] = acc; acc += c; }
-	v[n] = acc;
+	for (int j = 0; j < W; ++j) {
+		uint64_t acc = 0;
+		for (int r = 0; r < n; ++r) { const uint64_t c = v[W * r + j]; v[W * r + j] = acc; acc += c; }
+		v[W * n + j] = acc;
+	}
 #endif
 	++t_launches;
 }
@@ -1807,25 +1816,33 @@ int GafSink::results(Model *M, Model::Slot &sl, const Batch &B, const Last &L, i
 	return 0;
 }
 
-// Every table's offset in the block (256-byte aligned) and the block's size, from the rows r.n_*
-static void rec_layout(mgb_records_t &r)
+// Every table's offset in the block (256-byte aligned) and the block's size, from the rows r.n_* (and x.n_*: the ds tables after
+// the others; x NULL: none)
+static void rec_layout(mgb_records_t &r, mgb_records_ds_t *x)
 {
 	const int64_t bytes[MGB_REC_NTAB] = {24 * (r.n_seq + 1), 8 * r.n_seq, 4 * MGB_GC_NCOL * r.n_rec, 4 * r.n_rec, 8 * (r.n_rec + 1), 20 * r.n_lc, 16 * r.n_a, 8 * r.n_cigar};
 	int64_t at = 0;
 	for (int t = 0; t < MGB_REC_NTAB; ++t) r.off[t] = at, at += (bytes[t] + 255) & ~(int64_t)255;
+	if (x) {
+		const int64_t ds_bytes[MGB_REC_DS_NTAB] = {16 * (r.n_rec + 1), x->n_ds, 4 * x->n_ds_off};
+		for (int t = 0; t < MGB_REC_DS_NTAB; ++t) x->off[t] = at, at += (ds_bytes[t] + 255) & ~(int64_t)255;
+	}
 	r.bytes = at;
 }
 
-// Tables in device memory (mgb_map_batch_dev_rec), R, in one block from the caller's allocator on the index's device, ordered after
-// the work queued on the caller's stream.  A part (alloc NULL) writes its tables into a block of its own on its device, freed with
-// it, and the join copies them into the caller's block.
+// Tables in device memory (mgb_map_batch_dev_rec, with_ds: mgb_map_batch_dev_rec_ds), R and X, in one block from the caller's
+// allocator on the index's device, ordered after the work queued on the caller's stream.  A part (alloc NULL) writes its tables into
+// a block of its own on its device, freed with it, and the join copies them into the caller's block.
 struct RecSink : Sink {
 	mgb_dev_alloc_fn alloc;
 	void *alloc_ctx, *stream;
 	int device;       // where the block is
+	bool with_ds;
 	mgb_records_t R;  // the tables as written
+	mgb_records_ds_t X;
 	std::vector<std::unique_ptr<RecSink>> parts;
-	RecSink(mgb_dev_alloc_fn alloc_, void *alloc_ctx_, void *stream_, int device_) : alloc(alloc_), alloc_ctx(alloc_ctx_), stream(stream_), device(device_) { memset(&R, 0, sizeof(R)); }
+	RecSink(mgb_dev_alloc_fn alloc_, void *alloc_ctx_, void *stream_, int device_, bool with_ds_)
+		: alloc(alloc_), alloc_ctx(alloc_ctx_), stream(stream_), device(device_), with_ds(with_ds_) { memset(&R, 0, sizeof(R)), memset(&X, 0, sizeof(X)); }
 	~RecSink() // (the calling thread is left on the device of the first part, the index's)
 	{
 		if (alloc == 0 && R.block) dev_ok(device), dfree(R.block);
@@ -1834,7 +1851,7 @@ struct RecSink : Sink {
 	// R's block, ordered after the caller's stream; false when there is none
 	bool block()
 	{
-		rec_layout(R);
+		rec_layout(R, with_ds? &X : 0);
 		R.block = alloc? alloc(alloc_ctx, (size_t)R.bytes) : dmalloc((size_t)R.bytes);
 		if (R.block == 0) { set_error("mgb_map_batch_dev_rec: the allocator returned no block of " + std::to_string(R.bytes) + " bytes"); return false; }
 #ifndef MGB_HOSTSIM
@@ -1843,7 +1860,7 @@ struct RecSink : Sink {
 		return true;
 	}
 	int results(Model *M, Model::Slot &sl, const Batch &B, const Last &L, int host_threads) override;
-	Sink &part(int, int, int device_) override { parts.emplace_back(new RecSink(0, 0, stream, device_)); return *parts.back(); }
+	Sink &part(int, int, int device_) override { parts.emplace_back(new RecSink(0, 0, stream, device_, with_ds)); return *parts.back(); }
 	int join(Model *M) override;
 	int empty(Model *M) override // the two rows of totals alone, all 0: the join of no part
 	{
@@ -1852,12 +1869,16 @@ struct RecSink : Sink {
 		dev_bind(M->device, 0);
 		return rc;
 	}
-	int end(mgb_records_t *out, int rc) { if (rc == 0) *out = R; return rc; } // no block handed back on failure
+	int end(mgb_records_t *out, mgb_records_ds_t *ds_out, int rc) // no block handed back on failure
+	{
+		if (rc == 0) { *out = R; if (ds_out) *ds_out = X; }
+		return rc;
+	}
 };
 
 // The tables of a mapped sub-batch, written on the device from the blobs in the output pool (mgb_records.cuh): SEQ_CSR and the
-// reads' rows from the host, the CIGAR operations counted and scanned, the div requests to the host and the values back up, then
-// the block and the write pass.  t_d2h_ms: the table kernels, their copies and the host work between them; t_asm_ms stays 0: the
+// reads' rows from the host, the CIGAR operations (with_ds: and the ds bytes and offsets, of which only the totals come back) counted
+// and scanned, the div requests to the host and the values back up, then the block and the write pass.  t_d2h_ms: the table kernels, their copies and the host work between them; t_asm_ms stays 0: the
 // tables are final when the write pass ends.
 int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, int host_threads)
 {
@@ -1866,7 +1887,7 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 	mgb_stats_t &S = sl.st;
 	const size_t n = (size_t)n_reads;
 	auto has_result = [&](size_t f) { return (B.n_seg == 0 || B.n_seg[f] > 0) && read_status(L.meta[f], routs[f]) != 1; }; // mgb_map_batch_dev() leaves one
-	memset(&R, 0, sizeof(R));
+	memset(&R, 0, sizeof(R)), memset(&X, 0, sizeof(X));
 	for (size_t f = 0; f < n; ++f) {
 		R.n_seq += B.n_seg? std::max(B.n_seg[f], 0) : 1;
 		if (has_result(f)) R.n_rec += std::max(routs[f].n_gc, 0);
@@ -1874,11 +1895,13 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 	if (R.n_rec >= INT32_MAX) { set_error("mgb_map_batch_dev_rec: more than INT32_MAX records in one batch"); return MGB_E_UNSUPPORTED; }
 	const size_t n_seq = (size_t)R.n_seq, n_rec = (size_t)R.n_rec;
 	auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-	// host and device: seq_csr | seq_info | row_of (uploaded), then on the device cig_off | req | next, on the host req | div
+	// host and device: seq_csr | seq_info | row_of (uploaded), then on the device cig_off | req | next [| ds_n], on the host
+	// req | div [| the two ds totals]
 	const size_t o_info = al(24 * (n_seq + 1)), o_row = o_info + al(8 * n_seq), o_up = o_row + al(4 * n);
-	const size_t o_cig = o_up, o_req = o_cig + al(8 * (n_rec + 1)), o_next = o_req + al(sizeof(GafReq) * n_rec);
-	const size_t o_hdiv = o_up + al(sizeof(GafReq) * n_rec);
-	char *h = (char*)sl.h_rec.ensure(o_hdiv + 4 * n_rec + 16), *d = (char*)sl.d_rec.ensure(o_next + 16);
+	const size_t o_cig = o_up, o_req = o_cig + al(8 * (n_rec + 1)), o_next = o_req + al(sizeof(GafReq) * n_rec), o_ds = o_next + al(16);
+	const size_t o_hdiv = o_up + al(sizeof(GafReq) * n_rec), o_htot = o_hdiv + al(4 * n_rec);
+	char *h = (char*)sl.h_rec.ensure(with_ds? o_htot + 16 : o_hdiv + 4 * n_rec + 16);
+	char *d = (char*)sl.d_rec.ensure(with_ds? o_ds + 16 * (n_rec + 1) : o_next + 16);
 	int64_t *csr = (int64_t*)h;
 	int32_t *info = (int32_t*)(h + o_info), *row_of = (int32_t*)(h + o_row);
 	GafReq *hreq = (GafReq*)(h + o_up);
@@ -1900,37 +1923,45 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 	A.routs = (const ReadOut*)sl.d_routs.p, A.pool = L.d_out, A.n = n_reads;
 	A.row_of = (const int32_t*)(d + o_row), A.seq_csr = (const int64_t*)d;
 	A.cig_off = (uint64_t*)(d + o_cig), A.req = (GafReq*)(d + o_req), A.next = (unsigned int*)(d + o_next);
+	A.ds_n = with_ds? (uint64_t*)(d + o_ds) : 0, A.ds = 0, A.ds_off = 0;
 	{
 		Span span(&sl.timers->d2h);
 		h2d(d, h, o_up);
 		S.h2d_bytes += (int64_t)o_up;
 #ifndef MGB_HOSTSIM
-		k_rec_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
+		(with_ds? k_rec_count<true> : k_rec_count<false>)<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
 		CUDA_OK(cudaGetLastError());
 #else
-		sim_each_read(n_reads, [&](int r, int lane) { rec_read(A, r, lane, false); return 0; });
+		sim_each_read(n_reads, [&](int r, int lane) { with_ds? rec_read<true>(A, r, lane, false) : rec_read<false>(A, r, lane, false); return 0; });
 #endif
 		++t_launches;
 		scan_u64(A.cig_off, (int)n_rec);
+		int64_t *htot = (int64_t*)(h + o_htot);
+		if (with_ds) scan_u64<2>(A.ds_n, (int)n_rec), d2h_async(htot, A.ds_n + 2 * n_rec, 16);
 		d2h_async(hreq, A.req, sizeof(GafReq) * n_rec);
 		d2h(&R.n_cigar, A.cig_off + n_rec, 8);
 		S.out_bytes = (int64_t)(sizeof(GafReq) * n_rec + 8);
+		if (with_ds) X.n_ds = htot[0], X.n_ds_off = htot[1], S.out_bytes += 16;
 		pfor(sl.host_pool, host_threads, (int64_t)n_rec, [&](int64_t k) { hdiv[k] = gc_div(hreq[k].a, hreq[k].b, hreq[k].q_span); });
 		if (!block()) return MGB_E_INTERNAL;
 		char *b = (char*)R.block;
 		d2d(b + R.off[MGB_REC_SEQ_CSR], d, 24 * (n_seq + 1));
 		d2d(b + R.off[MGB_REC_SEQ_INFO], d + o_info, 8 * n_seq);
 		d2d(b + R.off[MGB_REC_CIGAR_CSR], A.cig_off, 8 * (n_rec + 1));
+		if (with_ds) {
+			d2d(b + X.off[MGB_REC_DS_CSR], A.ds_n, 16 * (n_rec + 1));
+			A.ds = b + X.off[MGB_REC_DS], A.ds_off = (int32_t*)(b + X.off[MGB_REC_DS_OFF]);
+		}
 		h2d_async(b + R.off[MGB_REC_GC_DIV], hdiv, 4 * n_rec);
 		S.h2d_bytes += (int64_t)(4 * n_rec);
 		A.gc = (int32_t*)(b + R.off[MGB_REC_GC]), A.lc = (uint32_t*)(b + R.off[MGB_REC_LC]);
 		A.a = (uint64_t*)(b + R.off[MGB_REC_A]), A.cigar = (uint64_t*)(b + R.off[MGB_REC_CIGAR]);
 		dzero(A.next, sizeof(unsigned int));
 #ifndef MGB_HOSTSIM
-		k_rec_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
+		(with_ds? k_rec_write<true> : k_rec_write<false>)<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
 		CUDA_OK(cudaGetLastError());
 #else
-		sim_each_read(n_reads, [&](int r, int lane) { rec_read(A, r, lane, true); return 0; });
+		sim_each_read(n_reads, [&](int r, int lane) { with_ds? rec_read<true>(A, r, lane, true) : rec_read<false>(A, r, lane, true); return 0; });
 #endif
 		++t_launches;
 	}
@@ -1938,13 +1969,15 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 	return 0;
 }
 
-// The rows of totals of R's block (SEQ_CSR row n_seq, CIGAR_CSR row n_rec), on the calling thread's stream, which is synchronised
-static void rec_totals(const mgb_records_t &R)
+// The rows of totals of R's block (SEQ_CSR row n_seq, CIGAR_CSR row n_rec; x: DS_CSR row n_rec), on the calling thread's stream,
+// which is synchronised
+static void rec_totals(const mgb_records_t &R, const mgb_records_ds_t *x)
 {
-	const int64_t tot[4] = {R.n_rec, R.n_lc, R.n_a, R.n_cigar};
+	const int64_t tot[6] = {R.n_rec, R.n_lc, R.n_a, R.n_cigar, x? x->n_ds : 0, x? x->n_ds_off : 0};
 	char *b = (char*)R.block;
 	h2d_async(b + R.off[MGB_REC_SEQ_CSR] + 24 * R.n_seq, tot, 24);
 	h2d_async(b + R.off[MGB_REC_CIGAR_CSR] + 8 * R.n_rec, tot + 3, 8);
+	if (x) h2d_async(b + x->off[MGB_REC_DS_CSR] + 16 * R.n_rec, tot + 4, 16);
 	dsync();
 }
 
@@ -1952,25 +1985,33 @@ static void rec_totals(const mgb_records_t &R)
 // copied behind those of the parts before, the CSR rows raised by the rows before, the totals written last.  On the caller's stream.
 int RecSink::join(Model *M)
 {
-	memset(&R, 0, sizeof(R));
-	for (const auto &p : parts) R.n_seq += p->R.n_seq, R.n_rec += p->R.n_rec, R.n_lc += p->R.n_lc, R.n_a += p->R.n_a, R.n_cigar += p->R.n_cigar;
+	memset(&R, 0, sizeof(R)), memset(&X, 0, sizeof(X));
+	for (const auto &p : parts) {
+		R.n_seq += p->R.n_seq, R.n_rec += p->R.n_rec, R.n_lc += p->R.n_lc, R.n_a += p->R.n_a, R.n_cigar += p->R.n_cigar;
+		X.n_ds += p->X.n_ds, X.n_ds_off += p->X.n_ds_off;
+	}
 #ifndef MGB_HOSTSIM
 	dev_bind(M->device, (cudaStream_t)stream);
 #endif
 	if (!block()) return MGB_E_INTERNAL;
-	enum { SEQ, REC, LC, A, CIG };
-	static const int kind[MGB_REC_NTAB] = {SEQ, SEQ, REC, REC, REC, LC, A, CIG};
-	static const int64_t row_bytes[MGB_REC_NTAB] = {24, 8, 4 * MGB_GC_NCOL, 4, 8, 20, 16, 8};
+	// the tables of R, then those of X
+	enum { SEQ, REC, LC, A, CIG, DS, DSO, N_KIND };
+	const int n_tab = MGB_REC_NTAB + (with_ds? MGB_REC_DS_NTAB : 0);
+	static const int kind[MGB_REC_NTAB + MGB_REC_DS_NTAB] = {SEQ, SEQ, REC, REC, REC, LC, A, CIG, REC, DS, DSO};
+	static const int64_t row_bytes[MGB_REC_NTAB + MGB_REC_DS_NTAB] = {24, 8, 4 * MGB_GC_NCOL, 4, 8, 20, 16, 8, 16, 1, 4};
+	auto off = [](const mgb_records_t &r, const mgb_records_ds_t &x, int t) { return t < MGB_REC_NTAB? r.off[t] : x.off[t - MGB_REC_NTAB]; };
 	char *b = (char*)R.block;
-	int64_t at[5] = {0, 0, 0, 0, 0}; // rows of the parts before
+	int64_t at[N_KIND] = {0, 0, 0, 0, 0, 0, 0}; // rows of the parts before
 	for (size_t d = 0; d < parts.size(); ++d) {
 		const mgb_records_t &p = parts[d]->R;
-		const int64_t rows[5] = {p.n_seq, p.n_rec, p.n_lc, p.n_a, p.n_cigar};
+		const mgb_records_ds_t &px = parts[d]->X;
+		const int64_t rows[N_KIND] = {p.n_seq, p.n_rec, p.n_lc, p.n_a, p.n_cigar, px.n_ds, px.n_ds_off};
 		if (p.block)
-			for (int t = 0; t < MGB_REC_NTAB; ++t)
-				d2d_peer(b + R.off[t] + at[kind[t]] * row_bytes[t], M->device, (const char*)p.block + p.off[t], parts[d]->device, (size_t)(rows[kind[t]] * row_bytes[t]));
-		const RecRebase rb[2] = {{(int64_t*)(b + R.off[MGB_REC_SEQ_CSR]) + 3 * at[SEQ], p.n_seq, 3, {at[REC], at[LC], at[A]}},
-								 {(int64_t*)(b + R.off[MGB_REC_CIGAR_CSR]) + at[REC], p.n_rec, 1, {at[CIG], 0, 0}}};
+			for (int t = 0; t < n_tab; ++t)
+				d2d_peer(b + off(R, X, t) + at[kind[t]] * row_bytes[t], M->device, (const char*)p.block + off(p, px, t), parts[d]->device, (size_t)(rows[kind[t]] * row_bytes[t]));
+		const RecRebase rb[3] = {{(int64_t*)(b + R.off[MGB_REC_SEQ_CSR]) + 3 * at[SEQ], p.n_seq, 3, {at[REC], at[LC], at[A]}},
+								 {(int64_t*)(b + R.off[MGB_REC_CIGAR_CSR]) + at[REC], p.n_rec, 1, {at[CIG], 0, 0}},
+								 {(int64_t*)(b + X.off[MGB_REC_DS_CSR]) + 2 * at[REC], with_ds? p.n_rec : 0, 2, {at[DS], at[DSO], 0}}};
 		for (const RecRebase &B : rb) {
 			if (B.n == 0 || (B.base[0] == 0 && B.base[1] == 0 && B.base[2] == 0)) continue;
 #ifndef MGB_HOSTSIM
@@ -1980,9 +2021,9 @@ int RecSink::join(Model *M)
 			for (int64_t i = 0; i < B.n; ++i) rec_rebase_row(B, i);
 #endif
 		}
-		for (int k = 0; k < 5; ++k) at[k] += rows[k];
+		for (int k = 0; k < N_KIND; ++k) at[k] += rows[k];
 	}
-	rec_totals(R);
+	rec_totals(R, with_ds? &X : 0);
 	return 0;
 }
 
@@ -2553,7 +2594,7 @@ static int map_batch_impl(Model *M, const Batch &B, Sink &K, const mg_mapopt_t *
 	return rc;
 }
 
-// The seven entry points below check their input, describe the reads (make_batch) and where the results go (a sink), and map.
+// The eight entry points below check their input, describe the reads (make_batch) and where the results go (a sink), and map.
 
 extern "C" int mg_map_batch(const mg_idx_t *gi, int n_reads, const int *qlens, const char *const *seqs, const char *const *names,
 							mg_gchains_t **gcs, const mg_mapopt_t *opt)
@@ -2583,7 +2624,7 @@ extern "C" int mgb_map_batch_gaf(const mg_idx_t *gi, int n_frag, const int *n_se
 	return K.end(map_batch_impl((Model*)gi->B, make_batch(n_frag, n_seg, qlens, seqs, names, 0), K, opt));
 }
 
-// ---- reads in device memory (mgb_map_batch_dev, mgb_map_batch_dev_gaf, mgb_map_batch_dev_rec) ----
+// ---- reads in device memory (mgb_map_batch_dev, mgb_map_batch_dev_gaf, mgb_map_batch_dev_rec, mgb_map_batch_dev_rec_ds) ----
 // A batch whose n_seq + 1 offsets d_off (sequence i is d_seq[d_off[i] .. d_off[i+1])) are in device memory: checks the buffers, copies
 // the offsets back once the caller's stream has got past the work queued on it, checks them, and gives the sequences' lengths and
 // their DevReads.  Returns 0, or a negative code with the reason set.
@@ -2668,18 +2709,37 @@ extern "C" int mgb_map_batch_dev_gaf(const mg_idx_t *gi, int n_frag, const int *
 	} catch (const MgbError &e) { return K.end(e.code); }
 }
 
+// mgb_map_batch_dev_rec(), and with ds_out mgb_map_batch_dev_rec_ds()
+static int dev_rec(const char *who, const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+				   const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream, mgb_dev_alloc_fn alloc, void *alloc_ctx,
+				   mgb_records_t *out, mgb_records_ds_t *ds_out, bool with_ds)
+{
+	if (out) memset(out, 0, sizeof(*out));
+	if (ds_out) memset(ds_out, 0, sizeof(*ds_out));
+	try {
+		if (alloc == 0 || out == 0 || (with_ds && ds_out == 0)) {
+			set_error(std::string(who) + (with_ds? ": an allocator, an mgb_records_t and an mgb_records_ds_t for the tables" : ": an allocator and an mgb_records_t for the tables"));
+			return MGB_E_UNSUPPORTED;
+		}
+		DevBatch D;
+		if (int rc = dev_batch_prepare(gi, who, n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, opt, stream, D)) return rc;
+		RecSink K(alloc, alloc_ctx, stream, model_of(gi)->device, with_ds);
+		return K.end(out, ds_out, map_batch_impl((Model*)gi->B, make_batch(n_frag, n_seg, D.qlen.data(), 0, names, &D.R), K, opt));
+	} catch (const MgbError &e) { return e.code; }
+}
+
 extern "C" int mgb_map_batch_dev_rec(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
 									 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
 									 mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out)
 {
-	if (out) memset(out, 0, sizeof(*out));
-	try {
-		if (alloc == 0 || out == 0) { set_error("mgb_map_batch_dev_rec: an allocator and an mgb_records_t for the tables"); return MGB_E_UNSUPPORTED; }
-		DevBatch D;
-		if (int rc = dev_batch_prepare(gi, "mgb_map_batch_dev_rec", n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, opt, stream, D)) return rc;
-		RecSink K(alloc, alloc_ctx, stream, model_of(gi)->device);
-		return K.end(out, map_batch_impl((Model*)gi->B, make_batch(n_frag, n_seg, D.qlen.data(), 0, names, &D.R), K, opt));
-	} catch (const MgbError &e) { return e.code; }
+	return dev_rec("mgb_map_batch_dev_rec", gi, n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, names, opt, stream, alloc, alloc_ctx, out, 0, false);
+}
+
+extern "C" int mgb_map_batch_dev_rec_ds(const mg_idx_t *gi, int n_frag, const int *n_seg, int n_seq, const char *d_seq, int64_t seq_bytes,
+										const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
+										mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out, mgb_records_ds_t *ds_out)
+{
+	return dev_rec("mgb_map_batch_dev_rec_ds", gi, n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, names, opt, stream, alloc, alloc_ctx, out, ds_out, true);
 }
 
 extern "C" void mg_map_frag(const mg_idx_t *gi, int n_segs, const int *qlens, const char **seqs, mg_gchains_t **gcs, mg_tbuf_t *b, const mg_mapopt_t *opt, const char *qname)

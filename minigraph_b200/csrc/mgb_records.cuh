@@ -6,9 +6,13 @@
 //     it for dv:f; the host computes div with its libm, SURVEY H3);
 //   * write pass: the read's GChains transposed into its GC rows, one 32-bit cell per lane; its LLChains and anchors copied word by
 //     word; each record's CIGAR operations copied to where CIGAR_CSR puts them.
+// With the ds tables (mgb_map_batch_dev_rec_ds) the count pass also stores each record's ds bytes and offsets (scanned into DS_CSR),
+// and the write pass copies them: the text 16 bytes per lane, the offsets one per lane.  Both passes are instantiated with and
+// without them (DS), so that the tables without ds run the code they ran before.
 #pragma once
 #include "../../include/mgb200.h"
 #include "mgb_gaf.cuh"
+#include "mgb_ingest.cuh"
 
 namespace mgb {
 
@@ -29,9 +33,74 @@ struct RecArgs {
 	uint32_t *lc;
 	uint64_t *a, *cigar;
 	unsigned int *next;      // work counter of the write pass
+	// the ds tables (rec_read<true>)
+	uint64_t *ds_n;          // [n_rec + 1][2]: ds bytes and offsets of record k (count pass), then its first of each (scan): DS_CSR
+	char *ds;                // the tables (write pass)
+	int32_t *ds_off;
 };
 
-// read r, warp-uniform; write == false: the count pass, otherwise the write pass
+// Bytes src[0 .. len) to dst, by all lanes: lane l writes the 16-byte-aligned chunks l, l + 32, ... of the destination, each from
+// the (at most two) aligned 16-byte chunks of the source that hold its bytes, whole where the chunk is all the string's and byte by
+// byte at the ends.  A source chunk that holds none of the string's bytes is not loaded.  (Records' strings follow each other in
+// DS at any byte; the blob's string starts 8-aligned.)
+MG_HD inline void rec_copy_bytes(char *dst, const char *src, int64_t len, int lane)
+{
+	const int h = (int)((uintptr_t)dst & 15);
+	char *d0 = dst - h;
+	const int64_t n_chunk = (h + len + 15) >> 4;
+	for (int64_t c = lane; c < n_chunk; c += MGB_W) {
+		const int64_t o = 16 * c - h; // the string's byte at the chunk's start (negative in the first chunk)
+		const char *base = (const char*)((uintptr_t)(src + o) & ~(uintptr_t)15);
+		const int sh = (int)((uintptr_t)(src + o) & 15);
+		uint32_t v[8];
+		for (int k = 0; k < 2; ++k) {
+			uint32_t *w = v + 4 * k;
+			const char *p = base + 16 * k;
+			if (p < src + len && p + 16 > src) {
+#if MGB_ON_DEVICE
+				const uint4 x = *(const uint4*)p;
+				w[0] = x.x, w[1] = x.y, w[2] = x.z, w[3] = x.w;
+#else
+				memcpy(w, p, 16);
+#endif
+			} else w[0] = w[1] = w[2] = w[3] = 0;
+		}
+		const int ws = sh >> 2, bs = 8 * (sh & 3);
+		uint32_t q[4];
+		for (int j = 0; j < 4; ++j) { // (no indexing by a variable: registers)
+			const uint32_t lo = ws == 0? v[j] : ws == 1? v[j + 1] : ws == 2? v[j + 2] : v[j + 3];
+			const uint32_t hi = ws == 0? v[j + 1] : ws == 1? v[j + 2] : ws == 2? v[j + 3] : v[j + 4];
+			q[j] = ingest_fshr(lo, hi, bs);
+		}
+		char *d = d0 + 16 * c;
+		const int b0 = o < 0? (int)-o : 0, b1 = len - o < 16? (int)(len - o) : 16; // the chunk's bytes that are the string's
+		if (b0 == 0 && b1 == 16) {
+#if MGB_ON_DEVICE
+			*(uint4*)d = make_uint4(q[0], q[1], q[2], q[3]);
+#else
+			memcpy(d, q, 16);
+#endif
+		} else {
+			const uint64_t lo = (uint64_t)q[1] << 32 | q[0], hi = (uint64_t)q[3] << 32 | q[2]; // (no indexing by a variable)
+			for (int b = b0; b < b1; ++b) d[b] = (char)((b < 8? lo : hi) >> 8 * (b & 7));
+		}
+	}
+}
+
+// the ds of the n_gc records of a read from k0 on (write pass)
+MG_HD inline void rec_ds(const RecArgs &R, const GChain *gc, int64_t k0, int64_t n_gc, int lane)
+{
+	for (int64_t i = 0; i < n_gc; ++i) {
+		const uint64_t *c = R.ds_n + 2 * (k0 + i);
+		const int64_t nb = (int64_t)(c[2] - c[0]), no = (int64_t)(c[3] - c[1]);
+		if (nb) rec_copy_bytes(R.ds + c[0], R.pool + gc[i].ds_off, nb, lane);
+		const int32_t *so = no? (const int32_t*)(R.pool + gc[i].dsoff_off) : 0;
+		for (int64_t j = lane; j < no; j += MGB_W) R.ds_off[c[1] + j] = so[j];
+	}
+}
+
+// read r, warp-uniform; write == false: the count pass, otherwise the write pass; DS: with the ds tables
+template<bool DS>
 MG_HD inline void rec_read(const RecArgs &R, int r, int lane, bool write)
 {
 	const int32_t s = R.row_of[r];
@@ -47,6 +116,7 @@ MG_HD inline void rec_read(const RecArgs &R, int r, int lane, bool write)
 			R.cig_off[k0 + i] = p.has_cigar? (uint64_t)p.n_cigar : 0;
 			GafReq q; q.a = p.n_mini, q.b = p.n_anchor, q.q_span = p.q_span, q.kind = 0;
 			R.req[k0 + i] = q;
+			if (DS) R.ds_n[2 * (k0 + i)] = p.has_cigar? (uint64_t)p.ds_len : 0, R.ds_n[2 * (k0 + i) + 1] = p.has_cigar? (uint64_t)p.n_dsoff : 0;
 		}
 		return;
 	}
@@ -72,6 +142,7 @@ MG_HD inline void rec_read(const RecArgs &R, int r, int lane, bool write)
 		const uint64_t *sc = nc? (const uint64_t*)(R.pool + gc[i].cigar_off) : 0;
 		for (uint64_t j = lane; j < nc; j += MGB_W) R.cigar[c0 + j] = sc[j];
 	}
+	if (DS) rec_ds(R, gc, k0, n_gc, lane);
 }
 
 // rows [0, n) of a table of w int64 columns, column j raised by base[j] (the CSR tables of a part joined behind others)
@@ -83,15 +154,17 @@ MG_HD inline void rec_rebase_row(const RecRebase &B, int64_t i)
 }
 
 #ifndef MGB_HOSTSIM
+template<bool DS>
 __global__ void __launch_bounds__(256) k_rec_count(RecArgs R)
 {
 	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < R.n; r += n_warp) rec_read(R, r, lane, false);
+	for (int r = warp; r < R.n; r += n_warp) rec_read<DS>(R, r, lane, false);
 }
+template<bool DS>
 __global__ void __launch_bounds__(256) k_rec_write(RecArgs R)
 {
 	const int lane = threadIdx.x & 31;
-	for (int r = gaf_next_read(R.next, lane); r < R.n; r = gaf_next_read(R.next, lane)) rec_read(R, r, lane, true);
+	for (int r = gaf_next_read(R.next, lane); r < R.n; r = gaf_next_read(R.next, lane)) rec_read<DS>(R, r, lane, true);
 }
 __global__ void __launch_bounds__(256) k_rec_rebase(RecRebase B)
 {

@@ -75,29 +75,39 @@ class MappedTables:
       a         int64 [n_a, 2]        mg128_t x, y (as their bits)
       cigar     int64 [n_cigar]       len<<4 | op
 
-    The ds:Z strings are not here (map_cuda_reads gives them)."""
+    With ds=True (map_cuda_reads_to_tensors), the ds:Z strings too (without them, map_cuda_reads gives them):
 
-    def __init__(self, block, rec):
+      ds_csr    int64 [n_rec + 1, 2]  record k's ds is ds[ds_csr[k,0]:ds_csr[k+1,0]] and its offsets ds_off[ds_csr[k,1]:ds_csr[k+1,1]]
+      ds        uint8 [n_ds]          mg_ds_t.ds of every record, one after another, no terminating 0 (empty without a CIGAR)
+      ds_off    int32 [n_ds_off]      mg_ds_t.off of every record"""
+
+    def __init__(self, block, rec, rec_ds=None):
         import torch
         shapes = {"seq_csr": (torch.int64, (rec.n_seq + 1, 3)), "seq_info": (torch.int32, (rec.n_seq, 2)),
                   "gc": (torch.int32, (rec.n_rec, len(GC_COLUMNS))), "gc_div": (torch.float32, (rec.n_rec,)),
                   "cigar_csr": (torch.int64, (rec.n_rec + 1,)), "lc": (torch.int32, (rec.n_lc, 5)), "a": (torch.int64, (rec.n_a, 2)),
                   "cigar": (torch.int64, (rec.n_cigar,))}
+        tables = [(name, rec.off[t]) for t, name in enumerate(capi.REC_TABLES)]
+        if rec_ds is not None:
+            shapes.update({"ds_csr": (torch.int64, (rec.n_rec + 1, 2)), "ds": (torch.uint8, (rec_ds.n_ds,)),
+                           "ds_off": (torch.int32, (rec_ds.n_ds_off,))})
+            tables += [(name, rec_ds.off[t]) for t, name in enumerate(capi.REC_DS_TABLES)]
         self.block = block
-        for t, name in enumerate(capi.REC_TABLES):
+        for name, o in tables:
             dtype, shape = shapes[name]
             n = 1
             for x in shape:
                 n *= x
-            o = rec.off[t]
             size = n * torch.empty((), dtype=dtype).element_size()
             setattr(self, name, block[o:o + size].view(dtype).view(shape))
 
 
-def map_cuda_reads_to_tensors(lib, gi, seq, off, names=None, opt=None, n_seg=None):
+def map_cuda_reads_to_tensors(lib, gi, seq, off, names=None, opt=None, n_seg=None, ds=False):
     """map_cuda_reads() with the results as tables written on the device into one block that torch allocates on seq's device
-    (mgb_map_batch_dev_rec): returns a MappedTables.  The same arguments, checks and refusals as map_cuda_reads()."""
+    (mgb_map_batch_dev_rec): returns a MappedTables.  The same arguments, checks and refusals as map_cuda_reads().  ds=True: the
+    tables also hold every record's ds:Z string and its offsets (mgb_map_batch_dev_rec_ds), in the same block."""
     import torch
+    who = "mgb_map_batch_dev_rec_ds" if ds else "mgb_map_batch_dev_rec"
     n_seq, args = _batch_args("map_cuda_reads_to_tensors", gi, seq, off, names, opt, n_seg)
     got, failed = [], []
 
@@ -111,7 +121,11 @@ def map_cuda_reads_to_tensors(lib, gi, seq, off, names=None, opt=None, n_seg=Non
 
     cb = capi.mgb_dev_alloc_fn(alloc)  # referenced until the call returns
     rec = capi.mgb_records_t()
-    rc = lib.mgb_map_batch_dev_rec(*args, cb, None, C.byref(rec))
+    rec_ds = capi.mgb_records_ds_t() if ds else None
+    if ds:
+        rc = lib.mgb_map_batch_dev_rec_ds(*args, cb, None, C.byref(rec), C.byref(rec_ds))
+    else:
+        rc = lib.mgb_map_batch_dev_rec(*args, cb, None, C.byref(rec))
     if rc < 0:
-        raise RuntimeError("mgb_map_batch_dev_rec: %s" % lib.mgb_last_error().decode()) from (failed[0] if failed else None)
-    return MappedTables(got[0], rec)
+        raise RuntimeError("%s: %s" % (who, lib.mgb_last_error().decode())) from (failed[0] if failed else None)
+    return MappedTables(got[0], rec, rec_ds)
