@@ -417,8 +417,8 @@ int mgb_test_gchain_gen(const mg_idx_t *gi, const mg_mapopt_t *opt, int n, const
 						const int32_t *seg_len, const uint32_t *hash, const int32_t *rep_len, const int32_t *n_mz, const int32_t *n_u, const uint64_t *u,
 						const int32_t *n_lc, const mg_lchain_t *lc, const int32_t *n_a, const mg128_t *a, int32_t *out, mg_gchains_t **gcs);
 
-/* test hook: the ingest step of reads in device memory as mgb_map_batch_dev() runs it (k_ingest on the device, its host loop in the
- * simulators) on n sequences seq[off[i] .. off[i+1]) (host memory, copied to the device first).  Sequence i's upper-case copy goes
+/* test hook: the ingest step of reads in device memory as mgb_map_batch_dev() runs it (k_ingest on the device, its body on every
+ * lane of a simulated warp in the simulators) on n sequences seq[off[i] .. off[i+1]) (host memory, copied to the device first).  Sequence i's upper-case copy goes
  * to ascii_out[off[i] .. off[i+1]); unless segmented (a batch of fragments with segments, which has no 2-bit words), its
  * (len + 31) / 32 words follow those of sequence i-1 in pk_out; raw_out[i] is 1 when it holds a byte other than A/C/G/T.
  * Returns 0, or a negative code for bad offsets or when the batch's pk_off does not mark exactly the flagged reads. */

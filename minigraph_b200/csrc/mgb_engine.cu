@@ -463,60 +463,29 @@ MG_HD inline uint64_t pack_size(const PackArgs &P, int r)
 	if (P.meta[r].status != 0 || ro.status != 0 || ro.n_gc <= 0) return 0;
 	return (((uint64_t)ro.blob_size + 15) & ~(uint64_t)15) + (((uint64_t)ro.blob2_size + 15) & ~(uint64_t)15);
 }
-MG_HD inline void pack_read(const PackArgs &P, int r, int lane, int nl)
-{
-	ReadOut &ro = P.routs[r];
-	const uint64_t sz = P.off[r + 1] - P.off[r];
-	if (sz == 0) return;
-	const uint64_t n1 = ((uint64_t)ro.blob_size + 15) & ~(uint64_t)15, n2 = sz - n1;
-	const uint64_t *s1 = (const uint64_t*)(P.pool + ro.blob_off), *s2 = (const uint64_t*)(P.pool + ro.blob2_off);
-	uint64_t *d1 = (uint64_t*)(P.packed + P.off[r]), *d2 = d1 + n1 / 8;
-	for (uint64_t i = lane; i < n1 / 8; i += nl) d1[i] = s1[i];
-	for (uint64_t i = lane; i < n2 / 8; i += nl) d2[i] = s2[i];
-#if MGB_ON_DEVICE
-	__syncwarp();
-#endif
-	const int64_t delta = (int64_t)(P.off[r] + n1) - ro.blob2_off;
-	GChain *gc = (GChain*)d1;
-	for (int i = lane; i < ro.n_gc; i += nl)
-		if (gc[i].has_cigar) gc[i].cigar_off += delta, gc[i].ds_off += delta, gc[i].dsoff_off += delta;
-	if (lane == 0) ro.blob_off = (int64_t)P.off[r], ro.blob2_off = (int64_t)(P.off[r] + n1);
-}
-#ifndef MGB_HOSTSIM
-__global__ void __launch_bounds__(1024) k_out_scan(PackArgs P)
-{
-	__shared__ uint64_t part[1024];
-	const int tid = threadIdx.x, per = (P.n + 1023) / 1024;
-	const int r0 = tid * per < P.n? tid * per : P.n, r1 = r0 + per < P.n? r0 + per : P.n;
-	uint64_t sum = 0;
-	for (int r = r0; r < r1; ++r) sum += pack_size(P, r);
-	part[tid] = sum;
-	__syncthreads();
-	if (tid == 0) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[i]; part[i] = acc; acc += c; } P.off[P.n] = acc; }
-	__syncthreads();
-	uint64_t acc = part[tid];
-	for (int r = r0; r < r1; ++r) { P.off[r] = acc; acc += pack_size(P, r); }
-}
-__global__ void __launch_bounds__(256) k_out_pack(PackArgs P)
-{
-	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < P.n; r += n_warp) pack_read(P, r, lane, 32);
-}
-#endif
-static void pack_results(const PackArgs &P)
-{
-#ifndef MGB_HOSTSIM
-	k_out_scan<<<1, 1024, 0, t_stream>>>(P);
-	k_out_pack<<<dev_sm_count() * 8, 256, 0, t_stream>>>(P);
-	CUDA_OK(cudaGetLastError());
-#else
-	uint64_t acc = 0;
-	for (int r = 0; r < P.n; ++r) { P.off[r] = acc; acc += pack_size(P, r); }
-	P.off[P.n] = acc;
-	for (int r = 0; r < P.n; ++r) pack_read(P, r, 0, 1);
-#endif
-	t_launches += 2;
-}
+// Read r's two blobs copied to their place in read order, and its chains' offsets into them moved along (warp-uniform)
+struct PackRead {
+	const PackArgs &a;
+	MG_HD int operator()(int r, int lane) const
+	{
+		ReadOut &ro = a.routs[r];
+		const uint64_t sz = a.off[r + 1] - a.off[r];
+		if (sz == 0) return 0;
+		const uint64_t n1 = ((uint64_t)ro.blob_size + 15) & ~(uint64_t)15, n2 = sz - n1;
+		const uint64_t *s1 = (const uint64_t*)(a.pool + ro.blob_off), *s2 = (const uint64_t*)(a.pool + ro.blob2_off);
+		uint64_t *d1 = (uint64_t*)(a.packed + a.off[r]), *d2 = d1 + n1 / 8;
+		for (uint64_t i = lane; i < n1 / 8; i += MGB_W) d1[i] = s1[i];
+		for (uint64_t i = lane; i < n2 / 8; i += MGB_W) d2[i] = s2[i];
+		// every lane reads blob2_off before the sync, so that lane 0's store of the new offsets below comes after all the loads
+		const int64_t delta = (int64_t)(a.off[r] + n1) - ro.blob2_off;
+		warp_sync();
+		GChain *gc = (GChain*)d1;
+		for (int i = lane; i < ro.n_gc; i += MGB_W)
+			if (gc[i].has_cigar) gc[i].cigar_off += delta, gc[i].ds_off += delta, gc[i].dsoff_off += delta;
+		if (lane == 0) ro.blob_off = (int64_t)a.off[r], ro.blob2_off = (int64_t)(a.off[r] + n1);
+		return 0;
+	}
+};
 
 // ---- reads cross PCIe 2 bits per base ----
 // Host: A/C/G/T -> 0..3 (the order of seq_nt4_table, sketch.c:9-26), 32 bases per 64-bit word, base i in bits 2*(i%32).  Returns false
@@ -569,7 +538,7 @@ static bool pack_read(const char *s, int len, uint64_t *out) { return pack_read_
 
 // Device: the ASCII copy of the packed reads (alignment, ds strings and the sequential sketch read bytes): one 64-bit word = 32 bases =
 // two 16-byte stores per lane, a warp per read.
-struct UnpackArgs { const uint64_t *pk, *pk_off, *seq_off; const int32_t *seq_len; char *seq; int n_reads; };
+struct UnpackArgs { const uint64_t *pk, *pk_off, *seq_off; const int32_t *seq_len; char *seq; int n; };
 MG_HD inline void unpack_word(const UnpackArgs &U, int r, int64_t wd)
 {
 	const int32_t len = U.seq_len[r];
@@ -590,43 +559,17 @@ MG_HD inline void unpack_word(const UnpackArgs &U, int r, int64_t wd)
 #endif
 		}
 }
-#ifndef MGB_HOSTSIM
-__global__ void __launch_bounds__(256) k_unpack(UnpackArgs U)
-{
-	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < U.n_reads; r += n_warp) {
-		if (U.pk_off[r] == ~0ULL) continue; // uploaded as ASCII
-		const int64_t nw = ((int64_t)U.seq_len[r] + 31) >> 5;
-		for (int64_t wd = lane; wd < nw; wd += 32) unpack_word(U, r, wd);
+// read r (warp-uniform); a read uploaded as ASCII has no words
+struct UnpackRead {
+	const UnpackArgs &a;
+	MG_HD int operator()(int r, int lane) const
+	{
+		if (a.pk_off[r] == ~0ULL) return 0;
+		const int64_t nw = ((int64_t)a.seq_len[r] + 31) >> 5;
+		for (int64_t wd = lane; wd < nw; wd += MGB_W) unpack_word(a, r, wd);
+		return 0;
 	}
-}
-#endif
-static void unpack_reads(const UnpackArgs &U)
-{
-#ifndef MGB_HOSTSIM
-	k_unpack<<<dev_sm_count() * 8, 256, 0, t_stream>>>(U);
-	CUDA_OK(cudaGetLastError());
-#else
-	for (int r = 0; r < U.n_reads; ++r) if (U.pk_off[r] != ~0ULL) for (int64_t wd = 0; wd * 32 < U.seq_len[r]; ++wd) unpack_word(U, r, wd);
-#endif
-	++t_launches;
-}
-
-// Reads already in device memory: their ASCII copy, words and flags (mgb_ingest.cuh)
-static void ingest_reads(const IngestArgs &I)
-{
-#ifndef MGB_HOSTSIM
-	k_ingest<<<dev_sm_count() * 8, 256, 0, t_stream>>>(I);
-	CUDA_OK(cudaGetLastError());
-#else
-	for (int r = 0; r < I.n_reads; ++r) {
-		uint32_t bad = 0;
-		for (int64_t wd = 0; wd * 32 < I.seq_len[r]; ++wd) bad |= ingest_word(I, r, wd);
-		ingest_flag(I, r, bad != 0);
-	}
-#endif
-	++t_launches;
-}
+};
 
 // ---- the few words the host needs between two kernels (pool fill levels, queue lengths) ----
 // They do not travel by cudaMemcpy: a copy of 16 bytes queues behind whatever another call in flight has put on the copy engines
@@ -787,105 +730,139 @@ static void launch_stage(LaunchArgs &L, const Workers &W)
 #endif
 }
 
-// ---- GAF text on the device (mgb_gaf.cuh) ----
-// One warp per read in every pass; the count and the write pass pull reads from a counter, the scan between them puts the reads'
-// texts in read order (as k_out_scan does for the blobs).
+// ---- per-read passes ----
+// A pass runs its body b(r, lane) on every read r < b.a.n, one warp per read; b.a are the arguments the kernel is launched with, held
+// by reference (on the device: the kernel's parameter itself, not a copy).  The body is warp-uniform (all lanes enter it for read r,
+// and it strides over its work by MGB_W) and returns a value on which the lanes agree.  Its warps take reads in one of two orders:
+// STRIDE, warp w takes reads w, w + warps, ...; PULL, lane 0 takes the next read from the body's counter b.counter() and the warp
+// gets it by shuffle, so that a long read holds up only its own warp.
+enum class ReadOrder { STRIDE, PULL };
 #ifndef MGB_HOSTSIM
-__global__ void __launch_bounds__(256) k_gaf_req(GafArgs G)
+__device__ inline int pass_next_read(unsigned int *next, int lane)
 {
-	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < G.n; r += n_warp) gaf_requests(G, r, lane);
+	unsigned int r = 0;
+	if (lane == 0) r = atomicAdd(next, 1u);
+	return (int)__shfl_sync(0xffffffffu, r, 0);
 }
-__global__ void __launch_bounds__(256) k_gaf_count(GafArgs G)
+template<ReadOrder O, typename Body>
+__device__ __forceinline__ void pass_loop(const Body &b)
 {
 	const int lane = threadIdx.x & 31;
-	for (int r = gaf_next_read(G.next, lane); r < G.n; r = gaf_next_read(G.next, lane)) {
-		const uint64_t n = gaf_read(G, r, 0, lane);
-		if (lane == 0) G.off[r] = n;
+	if constexpr (O == ReadOrder::PULL) {
+		for (int r = pass_next_read(b.counter(), lane); r < b.a.n; r = pass_next_read(b.counter(), lane)) b(r, lane);
+	} else {
+		const int warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
+		for (int r = warp; r < b.a.n; r += n_warp) b(r, lane);
 	}
 }
-// Rows [0 .. n) of W columns (v[W r + j]) replaced by their exclusive prefix sums, column by column, row n = the totals (the GAF
-// texts' offsets, the records' first CIGAR operations; W = 2: their first ds byte and offset)
-template<int W>
-__global__ void __launch_bounds__(1024) k_scan_u64(uint64_t *v, int n)
+#define MGB_PASS_KERNEL(KERNEL, ARGS, BODY, ORDER) __global__ void __launch_bounds__(256) KERNEL(ARGS a) { pass_loop<ReadOrder::ORDER>(BODY{a}); }
+#define MGB_PASS_PTR(KERNEL) KERNEL
+#else
+#define MGB_PASS_KERNEL(KERNEL, ARGS, BODY, ORDER) void KERNEL(ARGS);
+#define MGB_PASS_PTR(KERNEL) 0
+#endif
+
+// Runs pass b: dev_sm_count() * 8 blocks of 256 threads on the calling thread's stream, a PULL pass's counter zeroed in stream order
+// first.  The simulators run the body on every read in order, on all lanes of a simulated warp.
+template<ReadOrder O, typename K, typename Body>
+static void launch_pass(K kernel, const char *name, const Body &b)
 {
+	if constexpr (O == ReadOrder::PULL) dzero(b.counter(), sizeof(unsigned int));
+	++t_launches;
+#ifdef MGB_HOSTSIM
+	(void)kernel;
+	bool differ = false;
+	for (int r = 0; r < b.a.n; ++r) sim_warp(-1, r, [&](int lane) { return b(r, lane); }, &differ);
+	if (differ) { set_error(std::string("simulated warp: lanes returned different values from ") + name); throw MgbError{MGB_E_INTERNAL}; }
+#else
+	(void)name;
+	kernel<<<dev_sm_count() * 8, 256, 0, t_stream>>>(b.a);
+	CUDA_OK(cudaGetLastError());
+#endif
+}
+
+// One row per pass: its kernel (named, so that profiles read well), the arguments it is launched with, its body and the order in
+// which its warps take reads.  A row defines the kernel and run_pass(body), which launches it.  MGB_PASS_DS: a body instantiated
+// with and without the ds tables, one kernel template.
+#define MGB_PASS_RUN(KERNEL, BODY, ORDER) static void run_pass(const BODY &b) { launch_pass<ReadOrder::ORDER>(MGB_PASS_PTR(KERNEL), #KERNEL, b); }
+#define MGB_PASS(KERNEL, ARGS, BODY, ORDER) MGB_PASS_KERNEL(KERNEL, ARGS, BODY, ORDER) MGB_PASS_RUN(KERNEL, BODY, ORDER)
+#define MGB_PASS_DS(KERNEL, ARGS, BODY, ORDER) \
+	template<bool DS> MGB_PASS_KERNEL(KERNEL, ARGS, BODY<DS>, ORDER) \
+	template<bool DS> MGB_PASS_RUN(KERNEL<DS>, BODY<DS>, ORDER)
+
+// GAF text (mgb_gaf.cuh): what the dv:f values need; the bytes of each read's text (then scanned into offsets); the text
+struct GafRequests { const GafArgs &a; MG_HD int operator()(int r, int lane) const { gaf_requests(a, r, lane); return 0; } };
+struct GafCount {
+	const GafArgs &a;
+	MG_HD unsigned int *counter() const { return a.next; }
+	MG_HD int operator()(int r, int lane) const { const uint64_t b = gaf_read(a, r, 0, lane); if (lane == 0) a.off[r] = b; return (int)b; }
+};
+struct GafWrite {
+	const GafArgs &a;
+	MG_HD unsigned int *counter() const { return a.next + 1; }
+	MG_HD int operator()(int r, int lane) const { return (int)gaf_read(a, r, a.text + a.off[r], lane); }
+};
+
+//          kernel        arguments   body         reads
+MGB_PASS(   k_unpack,     UnpackArgs, UnpackRead,  STRIDE) // the ASCII copy of the reads that crossed PCIe 2 bits per base
+MGB_PASS(   k_out_pack,   PackArgs,   PackRead,    STRIDE) // the result blobs in read order
+MGB_PASS(   k_gaf_req,    GafArgs,    GafRequests, STRIDE) // GAF text: what the dv:f values need,
+MGB_PASS(   k_gaf_count,  GafArgs,    GafCount,    PULL)   // the bytes of each read's text,
+MGB_PASS(   k_gaf_write,  GafArgs,    GafWrite,    PULL)   // the text
+namespace mgb { // (the kernels of the headers' passes keep the names they had there)
+MGB_PASS(   k_ingest,     IngestArgs, IngestRead,  STRIDE) // reads in device memory: their ASCII copy, words and flags (mgb_ingest.cuh)
+MGB_PASS_DS(k_rec_count,  RecArgs,    RecCount,    STRIDE) // result tables (mgb_records.cuh): count pass,
+MGB_PASS_DS(k_rec_write,  RecArgs,    RecWrite,    PULL)   // write pass
+}
+
+// ---- block scan ----
+// The values src(r, j) of rows [0 .. n) of Src::W columns, their exclusive prefix sums written to out[W r + j] column by column, and
+// row n = the totals.  Each thread sums a contiguous run of rows, then one thread per column scans the 1024 partial sums.
+template<int W_> struct ScanCols { // in place: v = out
+	static constexpr int W = W_;
+	const uint64_t *v;
+	MG_HD uint64_t operator()(int r, int j) const { return v[W * r + j]; }
+};
+struct PackSize { // the places of the result blobs in read order (out: PackArgs::off)
+	static constexpr int W = 1;
+	PackArgs P;
+	MG_HD uint64_t operator()(int r, int) const { return pack_size(P, r); }
+};
+#ifndef MGB_HOSTSIM
+template<typename Src>
+__global__ void __launch_bounds__(1024) k_scan(Src src, uint64_t *out, int n)
+{
+	constexpr int W = Src::W;
 	__shared__ uint64_t part[W][1024];
 	const int tid = threadIdx.x, per = (n + 1023) / 1024;
 	const int r0 = tid * per < n? tid * per : n, r1 = r0 + per < n? r0 + per : n;
 	for (int j = 0; j < W; ++j) {
 		uint64_t sum = 0;
-		for (int r = r0; r < r1; ++r) sum += v[W * r + j];
+		for (int r = r0; r < r1; ++r) sum += src(r, j);
 		part[j][tid] = sum;
 	}
 	__syncthreads();
-	if (tid < W) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[tid][i]; part[tid][i] = acc; acc += c; } v[W * n + tid] = acc; }
+	if (tid < W) { uint64_t acc = 0; for (int i = 0; i < 1024; ++i) { uint64_t c = part[tid][i]; part[tid][i] = acc; acc += c; } out[W * n + tid] = acc; }
 	__syncthreads();
 	for (int j = 0; j < W; ++j) {
 		uint64_t acc = part[j][tid];
-		for (int r = r0; r < r1; ++r) { const uint64_t c = v[W * r + j]; v[W * r + j] = acc; acc += c; }
+		for (int r = r0; r < r1; ++r) { const uint64_t c = src(r, j); out[W * r + j] = acc; acc += c; }
 	}
 }
-__global__ void __launch_bounds__(256) k_gaf_write(GafArgs G)
-{
-	const int lane = threadIdx.x & 31;
-	for (int r = gaf_next_read(G.next + 1, lane); r < G.n; r = gaf_next_read(G.next + 1, lane)) gaf_read(G, r, G.text + G.off[r], lane);
-}
-#else
-// fn(r, lane) on every read, a simulated warp each
-template<typename F>
-static void sim_each_read(int n, const F &fn)
-{
-	bool differ = false;
-	for (int r = 0; r < n; ++r) sim_warp(-1, r, [&](int lane) { return fn(r, lane); }, &differ);
-	if (differ) { set_error("simulated warp: lanes returned different codes from the GAF formatter"); throw MgbError{MGB_E_INTERNAL}; }
-}
 #endif
-// what the dv:f values of every read need (G.req)
-static void gaf_list_requests(const GafArgs &G)
+template<typename Src>
+static void scan_u64(const Src &src, uint64_t *out, int n)
 {
 #ifndef MGB_HOSTSIM
-	k_gaf_req<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
+	k_scan<<<1, 1024, 0, t_stream>>>(src, out, n);
 	CUDA_OK(cudaGetLastError());
 #else
-	sim_each_read(G.n, [&](int r, int lane) { gaf_requests(G, r, lane); return 0; });
-#endif
-	++t_launches;
-}
-template<int W = 1>
-static void scan_u64(uint64_t *v, int n)
-{
-#ifndef MGB_HOSTSIM
-	k_scan_u64<W><<<1, 1024, 0, t_stream>>>(v, n);
-	CUDA_OK(cudaGetLastError());
-#else
+	constexpr int W = Src::W;
 	for (int j = 0; j < W; ++j) {
 		uint64_t acc = 0;
-		for (int r = 0; r < n; ++r) { const uint64_t c = v[W * r + j]; v[W * r + j] = acc; acc += c; }
-		v[W * n + j] = acc;
+		for (int r = 0; r < n; ++r) { const uint64_t c = src(r, j); out[W * r + j] = acc; acc += c; }
+		out[W * n + j] = acc;
 	}
-#endif
-	++t_launches;
-}
-// the length of every read's text and where it starts, in read order (G.off; G.off[n]: the whole text); G.next[0] zeroed
-static void gaf_offsets(const GafArgs &G)
-{
-#ifndef MGB_HOSTSIM
-	k_gaf_count<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
-	CUDA_OK(cudaGetLastError());
-#else
-	sim_each_read(G.n, [&](int r, int lane) { const uint64_t b = gaf_read(G, r, 0, lane); if (lane == 0) G.off[r] = b; return (int)b; });
-#endif
-	++t_launches;
-	scan_u64(G.off, G.n);
-}
-// the text (G.text); G.next[1] zeroed
-static void gaf_write(const GafArgs &G)
-{
-#ifndef MGB_HOSTSIM
-	k_gaf_write<<<dev_sm_count() * 8, 256, 0, t_stream>>>(G);
-	CUDA_OK(cudaGetLastError());
-#else
-	sim_each_read(G.n, [&](int r, int lane) { return (int)gaf_read(G, r, G.text + G.off[r], lane); });
 #endif
 	++t_launches;
 }
@@ -1770,7 +1747,7 @@ int GafSink::results(Model *M, Model::Slot &sl, const Batch &B, const Last &L, i
 	{
 		Span span(&sl.timers->d2h);
 		// dv:f values: the device lists what each needs, the host formats them with its libm (SURVEY H3)
-		if (n_req) gaf_list_requests(G);
+		if (n_req) run_pass(GafRequests{G});
 		d2h(h + o_req, d + o_req, sizeof(GafReq) * n_req);
 		const GafReq *hreq = (const GafReq*)(h + o_req);
 		char *hcells = h + o_cells;
@@ -1788,12 +1765,12 @@ int GafSink::results(Model *M, Model::Slot &sl, const Batch &B, const Last &L, i
 		});
 		h2d(d + o_cells, hcells, (size_t)GAF_CELL * n_req);
 		// text: sizes, offsets in read order, bytes
-		dzero(G.next, 2 * sizeof(unsigned int));
-		gaf_offsets(G);
+		run_pass(GafCount{G});
+		scan_u64(ScanCols<1>{G.off}, G.off, G.n);
 		d2h(h + o_off, G.off, 8 * (n + 1));
 		G.text = (char*)sl.d_gaf_text.ensure(hoff[n] + 64);
 		htext = (char*)sl.h_out.ensure(hoff[n] + 64);
-		gaf_write(G);
+		run_pass(GafWrite{G});
 		download_in_pieces(sl, n_reads, hoff, htext, G.text);
 	}
 	const uint64_t total = hoff[n];
@@ -1928,16 +1905,10 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 		Span span(&sl.timers->d2h);
 		h2d(d, h, o_up);
 		S.h2d_bytes += (int64_t)o_up;
-#ifndef MGB_HOSTSIM
-		(with_ds? k_rec_count<true> : k_rec_count<false>)<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
-		CUDA_OK(cudaGetLastError());
-#else
-		sim_each_read(n_reads, [&](int r, int lane) { with_ds? rec_read<true>(A, r, lane, false) : rec_read<false>(A, r, lane, false); return 0; });
-#endif
-		++t_launches;
-		scan_u64(A.cig_off, (int)n_rec);
+		if (with_ds) run_pass(RecCount<true>{A}); else run_pass(RecCount<false>{A});
+		scan_u64(ScanCols<1>{A.cig_off}, A.cig_off, (int)n_rec);
 		int64_t *htot = (int64_t*)(h + o_htot);
-		if (with_ds) scan_u64<2>(A.ds_n, (int)n_rec), d2h_async(htot, A.ds_n + 2 * n_rec, 16);
+		if (with_ds) scan_u64(ScanCols<2>{A.ds_n}, A.ds_n, (int)n_rec), d2h_async(htot, A.ds_n + 2 * n_rec, 16);
 		d2h_async(hreq, A.req, sizeof(GafReq) * n_rec);
 		d2h(&R.n_cigar, A.cig_off + n_rec, 8);
 		S.out_bytes = (int64_t)(sizeof(GafReq) * n_rec + 8);
@@ -1956,14 +1927,7 @@ int RecSink::results(Model *, Model::Slot &sl, const Batch &B, const Last &L, in
 		S.h2d_bytes += (int64_t)(4 * n_rec);
 		A.gc = (int32_t*)(b + R.off[MGB_REC_GC]), A.lc = (uint32_t*)(b + R.off[MGB_REC_LC]);
 		A.a = (uint64_t*)(b + R.off[MGB_REC_A]), A.cigar = (uint64_t*)(b + R.off[MGB_REC_CIGAR]);
-		dzero(A.next, sizeof(unsigned int));
-#ifndef MGB_HOSTSIM
-		(with_ds? k_rec_write<true> : k_rec_write<false>)<<<dev_sm_count() * 8, 256, 0, t_stream>>>(A);
-		CUDA_OK(cudaGetLastError());
-#else
-		sim_each_read(n_reads, [&](int r, int lane) { with_ds? rec_read<true>(A, r, lane, true) : rec_read<false>(A, r, lane, true); return 0; });
-#endif
-		++t_launches;
+		if (with_ds) run_pass(RecWrite<true>{A}); else run_pass(RecWrite<false>{A});
 	}
 	dsync();
 	return 0;
@@ -1981,6 +1945,14 @@ static void rec_totals(const mgb_records_t &R, const mgb_records_ds_t *x)
 	dsync();
 }
 
+#ifndef MGB_HOSTSIM
+namespace mgb { // (named as in mgb_records.cuh, which holds its row function)
+__global__ void __launch_bounds__(256) k_rec_rebase(RecRebase B)
+{
+	for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < B.n; i += (int64_t)gridDim.x * blockDim.x) rec_rebase_row(B, i);
+}
+}
+#endif
 // The tables of the parts (each in its own block on its device) joined in input order into R's block on M's device: every table
 // copied behind those of the parts before, the CSR rows raised by the rows before, the totals written last.  On the caller's stream.
 int RecSink::join(Model *M)
@@ -2134,7 +2106,7 @@ static BatchDev upload_batch(Staging &B, const BatchLayout &lay, const Model *M,
 		}
 		upload_tables(B, b, n_reads, seq_off, d_seq, S);
 		b.pk = packed? d_pk : 0, b.pk_off = packed? d_pk_off : 0;
-		if (packed) unpack_reads(UnpackArgs{d_pk, d_pk_off, b.seq_off, b.seq_len, d_seq, n_reads});
+		if (packed) run_pass(UnpackRead{UnpackArgs{d_pk, d_pk_off, b.seq_off, b.seq_len, d_seq, n_reads}});
 	}
 	upload_read_extras(B, b, M, names, no_diag, seg_off, seg_len);
 	return b;
@@ -2173,7 +2145,7 @@ static BatchDev upload_batch_dev(Staging &B, const BatchLayout &lay, const Model
 		S.h2d_bytes = (int64_t)n * 16;
 		upload_tables(B, b, n_reads, h_tables, d_seq, S);
 		b.pk = packed? d_pk_off + 2 * n8 : 0, b.pk_off = packed? d_pk_off : 0;
-		ingest_reads(IngestArgs{src, (const int64_t*)(d_pk_off + n8), b.seq_off, b.seq_len, d_seq, (uint64_t*)b.pk, d_pk_off, d_raw, n_reads});
+		run_pass(IngestRead{IngestArgs{src, (const int64_t*)(d_pk_off + n8), b.seq_off, b.seq_len, d_seq, (uint64_t*)b.pk, d_pk_off, d_raw, n_reads}});
 	}
 	upload_read_extras(B, b, M, names, no_diag, seg_off, seg_len);
 	return b;
@@ -2317,7 +2289,7 @@ struct Pass {
 	}
 };
 
-// The result blobs of a batch closed up in read order (pack_results), then to the host in pieces, each followed by the event the
+// The result blobs of a batch closed up in read order (k_scan, k_out_pack), then to the host in pieces, each followed by the event the
 // assembly of its reads waits for.  routs gets the blobs' new places.  Returns the host copy.
 static const char *download_blobs(Model::Slot &sl, int n_reads, ReadOut *routs, const char *d_out, uint64_t out_used, EvTimer &tm_d2h, mgb_stats_t &S)
 {
@@ -2326,7 +2298,8 @@ static const char *download_blobs(Model::Slot &sl, int n_reads, ReadOut *routs, 
 	PackArgs P;
 	P.routs = (ReadOut*)sl.d_routs.p, P.meta = (const ReadMeta*)sl.d_meta.p, P.n = n_reads, P.pool = d_out;
 	P.packed = (char*)sl.d_packed.ensure(out_used + 64), P.off = (uint64_t*)sl.d_packoff.ensure(sizeof(uint64_t) * (n + 1));
-	pack_results(P);
+	scan_u64(PackSize{P}, P.off, n_reads);
+	run_pass(PackRead{P});
 	d2h(routs, P.routs, sizeof(ReadOut) * n);
 	std::vector<uint64_t> off(n + 1);
 	d2h(off.data(), P.off, sizeof(uint64_t) * (n + 1));

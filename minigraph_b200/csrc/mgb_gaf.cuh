@@ -282,14 +282,4 @@ MG_HD inline uint64_t gaf_read(const GafArgs &G, int r, char *dst, int lane)
 	return o.n;
 }
 
-#ifndef MGB_HOSTSIM
-// the next read of a pass that pulls its reads from a counter: lane 0 takes it, the warp gets it
-__device__ inline int gaf_next_read(unsigned int *next, int lane)
-{
-	unsigned int r = 0;
-	if (lane == 0) r = atomicAdd(next, 1u);
-	return (int)__shfl_sync(0xffffffffu, r, 0);
-}
-#endif
-
 } // namespace mgb

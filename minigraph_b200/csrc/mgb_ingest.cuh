@@ -14,7 +14,7 @@ namespace mgb {
 struct IngestArgs {
 	const char *src; const int64_t *src_off;
 	const uint64_t *seq_off; const int32_t *seq_len; char *seq;
-	uint64_t *pk, *pk_off; int32_t *raw; int n_reads;
+	uint64_t *pk, *pk_off; int32_t *raw; int n;
 };
 
 // bits [s, s + 32) of hi:lo
@@ -94,19 +94,18 @@ MG_HD inline void ingest_flag(const IngestArgs &I, int r, bool raw)
 	if (raw && I.pk) I.pk_off[r] = ~0ULL;
 }
 
-#ifndef MGB_HOSTSIM
-// one warp per read, each lane whole words, long reads strided over the lanes
-__global__ void __launch_bounds__(256) k_ingest(IngestArgs I)
-{
-	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < I.n_reads; r += n_warp) {
-		const int64_t nw = ((int64_t)I.seq_len[r] + 31) >> 5;
+// read r (warp-uniform): each lane whole words, long reads strided over the lanes; returns the read's flag
+struct IngestRead {
+	const IngestArgs &a;
+	MG_HD int operator()(int r, int lane) const
+	{
+		const int64_t nw = ((int64_t)a.seq_len[r] + 31) >> 5;
 		uint32_t bad = 0;
-		for (int64_t wd = lane; wd < nw; wd += 32) bad |= ingest_word(I, r, wd);
-		const bool raw = __any_sync(0xffffffffu, bad != 0); // (every lane has read pk_off[r] by now)
-		if (lane == 0) ingest_flag(I, r, raw);
+		for (int64_t wd = lane; wd < nw; wd += MGB_W) bad |= ingest_word(a, r, wd);
+		const bool raw = warp_any(bad != 0); // (every lane has read pk_off[r] by now)
+		if (lane == 0) ingest_flag(a, r, raw);
+		return raw;
 	}
-}
-#endif
+};
 
 } // namespace mgb

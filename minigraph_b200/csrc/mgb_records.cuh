@@ -33,7 +33,7 @@ struct RecArgs {
 	uint32_t *lc;
 	uint64_t *a, *cigar;
 	unsigned int *next;      // work counter of the write pass
-	// the ds tables (rec_read<true>)
+	// the ds tables (DS)
 	uint64_t *ds_n;          // [n_rec + 1][2]: ds bytes and offsets of record k (count pass), then its first of each (scan): DS_CSR
 	char *ds;                // the tables (write pass)
 	int32_t *ds_off;
@@ -99,51 +99,68 @@ MG_HD inline void rec_ds(const RecArgs &R, const GChain *gc, int64_t k0, int64_t
 	}
 }
 
-// read r, warp-uniform; write == false: the count pass, otherwise the write pass; DS: with the ds tables
+// Read r (warp-uniform), count pass: each record's CIGAR operations and what its div needs (DS: and its ds bytes and offsets)
 template<bool DS>
-MG_HD inline void rec_read(const RecArgs &R, int r, int lane, bool write)
-{
-	const int32_t s = R.row_of[r];
-	if (s < 0) return;
-	const int64_t *row = R.seq_csr + 3 * (int64_t)s;
-	const int64_t k0 = row[0], n_gc = row[3] - row[0], n_lc = row[4] - row[1], n_a = row[5] - row[2];
-	if (n_gc == 0) return;
-	const ReadBlob B = read_blob(R.pool, R.routs[r]);
-	const GChain *gc = B.gc;
-	if (!write) {
+struct RecCount {
+	const RecArgs &a;
+	MG_HD int operator()(int r, int lane) const
+	{
+		const int32_t s = a.row_of[r];
+		if (s < 0) return 0;
+		const int64_t k0 = a.seq_csr[3 * (int64_t)s], n_gc = a.seq_csr[3 * (int64_t)s + 3] - k0;
+		if (n_gc == 0) return 0;
+		const GChain *gc = read_blob(a.pool, a.routs[r]).gc;
 		for (int64_t i = lane; i < n_gc; i += MGB_W) {
 			const GChain &p = gc[i];
-			R.cig_off[k0 + i] = p.has_cigar? (uint64_t)p.n_cigar : 0;
+			a.cig_off[k0 + i] = p.has_cigar? (uint64_t)p.n_cigar : 0;
 			GafReq q; q.a = p.n_mini, q.b = p.n_anchor, q.q_span = p.q_span, q.kind = 0;
-			R.req[k0 + i] = q;
-			if (DS) R.ds_n[2 * (k0 + i)] = p.has_cigar? (uint64_t)p.ds_len : 0, R.ds_n[2 * (k0 + i) + 1] = p.has_cigar? (uint64_t)p.n_dsoff : 0;
+			a.req[k0 + i] = q;
+			if (DS) a.ds_n[2 * (k0 + i)] = p.has_cigar? (uint64_t)p.ds_len : 0, a.ds_n[2 * (k0 + i) + 1] = p.has_cigar? (uint64_t)p.n_dsoff : 0;
 		}
-		return;
+		return 0;
 	}
-	int32_t *dg = R.gc + k0 * MGB_GC_NCOL;
-	for (int64_t w = lane; w < n_gc * MGB_GC_NCOL; w += MGB_W) {
-		const int64_t i = w / MGB_GC_NCOL;
-		const int c = (int)(w - i * MGB_GC_NCOL);
-		const int32_t *src = (const int32_t*)(gc + i);
-		int32_t v = src[c <= MGB_GC_FLT? c : c + 2];
-		if (c == MGB_GC_MAPQ) v &= 0xff;                        // mg_gchain_t's bit fields
-		else if (c == MGB_GC_FLT) v &= 1;
-		else if (c > MGB_GC_HAS_CIGAR && !gc[i].has_cigar) v = 0; // no mg_cigar_t
-		dg[w] = v;
+};
+
+// Read r (warp-uniform), write pass: its rows of every table
+template<bool DS>
+struct RecWrite {
+	const RecArgs &a;
+	MG_HD unsigned int *counter() const { return a.next; }
+	MG_HD int operator()(int r, int lane) const
+	{
+		const int32_t s = a.row_of[r];
+		if (s < 0) return 0;
+		const int64_t *row = a.seq_csr + 3 * (int64_t)s;
+		const int64_t k0 = row[0], n_gc = row[3] - row[0], n_lc = row[4] - row[1], n_a = row[5] - row[2];
+		if (n_gc == 0) return 0;
+		const ReadBlob B = read_blob(a.pool, a.routs[r]);
+		const GChain *gc = B.gc;
+		int32_t *dg = a.gc + k0 * MGB_GC_NCOL;
+		for (int64_t w = lane; w < n_gc * MGB_GC_NCOL; w += MGB_W) {
+			const int64_t i = w / MGB_GC_NCOL;
+			const int c = (int)(w - i * MGB_GC_NCOL);
+			const int32_t *src = (const int32_t*)(gc + i);
+			int32_t v = src[c <= MGB_GC_FLT? c : c + 2];
+			if (c == MGB_GC_MAPQ) v &= 0xff;                        // mg_gchain_t's bit fields
+			else if (c == MGB_GC_FLT) v &= 1;
+			else if (c > MGB_GC_HAS_CIGAR && !gc[i].has_cigar) v = 0; // no mg_cigar_t
+			dg[w] = v;
+		}
+		const uint32_t *slc = (const uint32_t*)B.lc;
+		uint32_t *dlc = a.lc + row[1] * 5;
+		for (int64_t w = lane; w < n_lc * 5; w += MGB_W) dlc[w] = slc[w];
+		const uint64_t *sa = (const uint64_t*)B.a;
+		uint64_t *da = a.a + row[2] * 2;
+		for (int64_t w = lane; w < n_a * 2; w += MGB_W) da[w] = sa[w];
+		for (int64_t i = 0; i < n_gc; ++i) {
+			const uint64_t c0 = a.cig_off[k0 + i], nc = a.cig_off[k0 + i + 1] - c0;
+			const uint64_t *sc = nc? (const uint64_t*)(a.pool + gc[i].cigar_off) : 0;
+			for (uint64_t j = lane; j < nc; j += MGB_W) a.cigar[c0 + j] = sc[j];
+		}
+		if (DS) rec_ds(a, gc, k0, n_gc, lane);
+		return 0;
 	}
-	const uint32_t *slc = (const uint32_t*)B.lc;
-	uint32_t *dlc = R.lc + row[1] * 5;
-	for (int64_t w = lane; w < n_lc * 5; w += MGB_W) dlc[w] = slc[w];
-	const uint64_t *sa = (const uint64_t*)B.a;
-	uint64_t *da = R.a + row[2] * 2;
-	for (int64_t w = lane; w < n_a * 2; w += MGB_W) da[w] = sa[w];
-	for (int64_t i = 0; i < n_gc; ++i) {
-		const uint64_t c0 = R.cig_off[k0 + i], nc = R.cig_off[k0 + i + 1] - c0;
-		const uint64_t *sc = nc? (const uint64_t*)(R.pool + gc[i].cigar_off) : 0;
-		for (uint64_t j = lane; j < nc; j += MGB_W) R.cigar[c0 + j] = sc[j];
-	}
-	if (DS) rec_ds(R, gc, k0, n_gc, lane);
-}
+};
 
 // rows [0, n) of a table of w int64 columns, column j raised by base[j] (the CSR tables of a part joined behind others)
 struct RecRebase { int64_t *v; int64_t n; int w; int64_t base[3]; };
@@ -152,24 +169,5 @@ MG_HD inline void rec_rebase_row(const RecRebase &B, int64_t i)
 	for (int j = 0; j < 3; ++j) // (constant indices: base stays in registers)
 		if (j < B.w) B.v[i * B.w + j] += B.base[j];
 }
-
-#ifndef MGB_HOSTSIM
-template<bool DS>
-__global__ void __launch_bounds__(256) k_rec_count(RecArgs R)
-{
-	const int lane = threadIdx.x & 31, warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), n_warp = (int)((gridDim.x * blockDim.x) >> 5);
-	for (int r = warp; r < R.n; r += n_warp) rec_read<DS>(R, r, lane, false);
-}
-template<bool DS>
-__global__ void __launch_bounds__(256) k_rec_write(RecArgs R)
-{
-	const int lane = threadIdx.x & 31;
-	for (int r = gaf_next_read(R.next, lane); r < R.n; r = gaf_next_read(R.next, lane)) rec_read<DS>(R, r, lane, true);
-}
-__global__ void __launch_bounds__(256) k_rec_rebase(RecRebase B)
-{
-	for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < B.n; i += (int64_t)gridDim.x * blockDim.x) rec_rebase_row(B, i);
-}
-#endif
 
 } // namespace mgb
