@@ -308,6 +308,32 @@ int mgb_map_batch_dev_rec_ds(const mg_idx_t *gi, int n_frag, const int *n_seg, i
 							 const int64_t *d_off, const char *const *names, const mg_mapopt_t *opt, void *stream,
 							 mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out, mgb_records_ds_t *ds_out);
 
+/* Parse FASTA/FASTQ text that lives in device memory into reads in device memory, on the device: d_text[0 .. text_bytes) gives the
+ * records mgb_reads_load() gives for the same bytes in a file (names up to the first white space, sequences without CR/LF and
+ * upper-cased, qualities skipped; malformed input alike), and SEQ / OFF feed mgb_map_batch_dev*() as they are.  Streaming: *out->used
+ * is the byte where the first record not emitted starts (junk before the first header counts as used).  final == 0: a record is
+ * emitted only when the start of the record after it lies in the text, so a caller that carries d_text[used ..] in front of its next
+ * bytes gets the records of one whole parse, wherever its buffers end; final != 0: the last record runs to the end of the text.
+ * max_bases > 0 stops after the record that reaches it (per call; used is then the start of the record after it).  The stream,
+ * allocator and ownership rules are those of mgb_map_batch_dev_rec(): the first read of d_text is ordered after the work queued on
+ * stream, alloc() is called once, after the parse succeeded, and the call returns once the tables are written:
+ *   MGB_DR_SEQ       uint8 [n_bases]       the bases, records one after another
+ *   MGB_DR_OFF       int64 [n_reads + 1]   record i is SEQ[OFF[i] .. OFF[i+1])
+ *   MGB_DR_NAME      uint8 [name_bytes]    the names, no terminators
+ *   MGB_DR_NAME_OFF  int64 [n_reads + 1]   record i's name is NAME[NAME_OFF[i] .. NAME_OFF[i+1])
+ * Empty text, or text without a header: 0 reads, the two rows of totals written.  Returns 0, or a negative code with the reason
+ * in mgb_last_error() and nothing in *out, also when d_text is not device or managed memory on the index's device, a size is
+ * negative, an emitted record is longer than INT32_MAX or alloc() returns NULL.  Scratch memory (about 8 bytes per line and 25 per
+ * '>' / '@' byte) is kept with the index and grown as needed; one call runs at a time per index. */
+enum { MGB_DR_SEQ, MGB_DR_OFF, MGB_DR_NAME, MGB_DR_NAME_OFF, MGB_DR_NTAB };
+typedef struct {
+	int64_t n_reads, n_bases, name_bytes; /* rows */
+	int64_t used;                         /* bytes of the text consumed: where the next call starts */
+	void *block; int64_t bytes; int64_t off[MGB_DR_NTAB]; /* one block from alloc(), 256-byte aligned tables */
+} mgb_dev_reads_t;
+int mgb_reads_parse_dev(const mg_idx_t *gi, const char *d_text, int64_t text_bytes, int64_t max_bases, int final, void *stream,
+						mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_dev_reads_t *out);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Engine controls and instrumentation (not part of the reference API)
  * ---------------------------------------------------------------------------------------------------------- */

@@ -124,6 +124,15 @@ class mgb_records_ds_t(C.Structure):
 mgb_dev_alloc_fn = C.CFUNCTYPE(C.c_void_p, C.c_void_p, C.c_size_t)
 
 
+# mgb_reads_parse_dev(): the tables of mgb_dev_reads_t (mgb200.h MGB_DR_*)
+DR_TABLES = ("seq", "off", "name", "name_off")
+
+
+class mgb_dev_reads_t(C.Structure):
+    _fields_ = [("n_reads", C.c_int64), ("n_bases", C.c_int64), ("name_bytes", C.c_int64), ("used", C.c_int64),
+                ("block", C.c_void_p), ("bytes", C.c_int64), ("off", C.c_int64 * len(DR_TABLES))]
+
+
 class mgb_reads_t(C.Structure):
     _fields_ = [("n_reads", C.c_int64), ("n_bases", C.c_int64), ("name", C.POINTER(C.c_char_p)), ("seq", C.POINTER(C.c_char_p)),
                 ("len", C.POINTER(C.c_int)), ("block", C.c_void_p)]
@@ -260,6 +269,9 @@ def bind_engine_api(lib):
     lib.mgb_map_batch_dev_rec.argtypes = dev_args + [mgb_dev_alloc_fn, C.c_void_p, C.POINTER(mgb_records_t)]
     lib.mgb_map_batch_dev_rec_ds.restype = C.c_int
     lib.mgb_map_batch_dev_rec_ds.argtypes = dev_args + [mgb_dev_alloc_fn, C.c_void_p, C.POINTER(mgb_records_t), C.POINTER(mgb_records_ds_t)]
+    lib.mgb_reads_parse_dev.restype = C.c_int
+    lib.mgb_reads_parse_dev.argtypes = [C.POINTER(mg_idx_t), C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, mgb_dev_alloc_fn, C.c_void_p,
+                                        C.POINTER(mgb_dev_reads_t)]
     lib.mgb_test_ingest.restype = C.c_int
     lib.mgb_test_ingest.argtypes = [C.c_int, C.c_char_p, i64p, C.c_int, C.c_void_p, C.POINTER(C.c_uint64), i32p]
     return lib

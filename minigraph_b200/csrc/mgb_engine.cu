@@ -27,6 +27,7 @@
 #include "mgb_galign.cuh"
 #include "mgb_gaf.cuh"
 #include "mgb_ingest.cuh"
+#include "mgb_fastx.cuh"
 #include "mgb_records.cuh"
 
 #ifndef MGB_HOSTSIM
@@ -813,6 +814,13 @@ namespace mgb { // (the kernels of the headers' passes keep the names they had t
 MGB_PASS(   k_ingest,     IngestArgs, IngestRead,  STRIDE) // reads in device memory: their ASCII copy, words and flags (mgb_ingest.cuh)
 MGB_PASS_DS(k_rec_count,  RecArgs,    RecCount,    STRIDE) // result tables (mgb_records.cuh): count pass,
 MGB_PASS_DS(k_rec_write,  RecArgs,    RecWrite,    PULL)   // write pass
+MGB_PASS(   k_fx_count,   FxArgs,     FxCount,     STRIDE) // FASTA/FASTQ text in device memory (mgb_fastx.cuh): list entries per chunk,
+MGB_PASS(   k_fx_lists,   FxArgs,     FxLists,     STRIDE) // the lists,
+MGB_PASS(   k_fx_succ,    FxArgs,     FxSucc,      STRIDE) // each candidate's successor,
+MGB_PASS(   k_fx_jump,    FxArgs,     FxJump,      STRIDE) // a round of pointer jumping,
+MGB_PASS(   k_fx_recs,    FxArgs,     FxRecs,      STRIDE) // the records,
+MGB_PASS(   k_fx_tail,    FxArgs,     FxTail,      STRIDE) // those the call emits,
+MGB_PASS(   k_fx_copy,    FxArgs,     FxCopy,      PULL)   // their bases and names
 }
 
 // ---- block scan ----
@@ -1006,6 +1014,8 @@ struct Model {
 	// reachability labels of the graph (mgb_gclabel.cuh): built on demand, kept across batches, grown between them
 	long long *d_lab_off = 0; Pool *d_lab_hdr = 0; char *d_lab_pool = 0;
 	uint64_t lab_cap = 0; int32_t lab_max_dist_g = -1; int64_t lab_sources = 0;
+	// mgb_reads_parse_dev(): one call at a time; the chunk table, the lists and the candidates' jumps and marks, the records
+	struct FxScratch { std::mutex mu; GrowBuf tab, lists, recs; } fx;
 };
 
 static void model_free(Model *M)
@@ -2713,6 +2723,111 @@ extern "C" int mgb_map_batch_dev_rec_ds(const mg_idx_t *gi, int n_frag, const in
 										mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_records_t *out, mgb_records_ds_t *ds_out)
 {
 	return dev_rec("mgb_map_batch_dev_rec_ds", gi, n_frag, n_seg, n_seq, d_seq, seq_bytes, d_off, names, opt, stream, alloc, alloc_ctx, out, ds_out, true);
+}
+
+// ---- FASTA/FASTQ text in device memory (mgb_reads_parse_dev, mgb_fastx.cuh) ----
+// The passes of mgb_fastx.cuh on the caller's stream, with the scratch of M; the host reads back the list totals, one jump per
+// round, the number of records and the call's FxSum.  Returns 0, or a negative code with the reason set and nothing in R.
+static int reads_parse(Model *M, const char *text, int64_t n, int64_t max_bases, int final, void *stream, mgb_dev_alloc_fn alloc,
+					   void *alloc_ctx, mgb_dev_reads_t &R)
+{
+	auto refuse = [&](const std::string &why) { set_error("mgb_reads_parse_dev: " + why); return (int)MGB_E_UNSUPPORTED; };
+	auto al = [](uint64_t x) { return (x + 255) & ~(uint64_t)255; };
+#ifndef MGB_HOSTSIM
+	CUDA_OK(cudaSetDevice(M->device));
+	if (n > 0) {
+		cudaPointerAttributes pa;
+		const bool ok = cudaPointerGetAttributes(&pa, text) == cudaSuccess && (pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged) && pa.device == M->device;
+		cudaGetLastError();
+		if (!ok) return refuse("the text is not device or managed memory on the index's device " + std::to_string(M->device));
+	}
+#endif
+	dev_bind(M->device, (DevStream)(uintptr_t)stream);
+	const int64_t n_chunks = (n + FX_CHUNK - 1) / FX_CHUNK;
+	if (n_chunks >= INT32_MAX) return refuse("a text of " + std::to_string(n) + " bytes");
+	FxArgs A;
+	memset(&A, 0, sizeof(A));
+	A.text = text, A.n_text = n, A.n_chunks = (int)n_chunks, A.max_bases = max_bases, A.final_ = final != 0;
+	Model::FxScratch &X = M->fx;
+	A.tab = (uint64_t*)X.tab.ensure(8 * FX_NLIST * ((size_t)n_chunks + 1));
+	uint64_t tot[FX_NLIST] = {0, 0, 0, 0};
+	if (n_chunks > 0) {
+		A.n = A.n_chunks;
+		run_pass(FxCount{A});
+		scan_u64(ScanCols<FX_NLIST>{A.tab}, A.tab, A.n_chunks);
+		d2h(tot, A.tab + FX_NLIST * n_chunks, sizeof(tot));
+	}
+	if (tot[FX_HD] >= (uint64_t)INT32_MAX) return refuse("more than INT32_MAX - 1 '>' and '@' bytes in one text");
+	const int64_t C = (int64_t)tot[FX_HD], n_groups = (C + 1 + 31) / 32;
+	// the lists | the jumps, twice | the marks | the records before each group
+	uint64_t o = 0, o_list[FX_NLIST];
+	for (int k = 0; k < FX_NLIST; ++k) o_list[k] = o, o += al(8 * tot[k]);
+	const uint64_t o_j0 = o, o_j1 = o_j0 + al(4 * (C + 1)), o_mark = o_j1 + al(4 * (C + 1)), o_grp = o_mark + al(C + 1);
+	char *d = (char*)X.lists.ensure(o_grp + 8 * (n_groups + 1));
+	for (int k = 0; k < FX_NLIST; ++k) A.list[k] = (int64_t*)(d + o_list[k]);
+	int32_t *J[2] = {(int32_t*)(d + o_j0), (int32_t*)(d + o_j1)};
+	A.mark = (uint8_t*)(d + o_mark);
+	uint64_t *grp = (uint64_t*)(d + o_grp);
+	A.n_cand = C;
+	if (n_chunks > 0) run_pass(FxLists{A});
+	A.n = (int)n_groups, A.jout = J[0];
+	run_pass(FxSucc{A});
+	for (int k = 0; C > 0; ++k) { // until the first candidate's jump passes the end: then every record is marked
+		int32_t j0 = 0;
+		d2h(&j0, J[k & 1], 4);
+		if (j0 == (int32_t)C) break;
+		A.jin = J[k & 1], A.jout = J[(k + 1) & 1];
+		run_pass(FxJump{A});
+	}
+	scan_u64(FxMarks{A}, grp, (int)n_groups);
+	uint64_t K = 0;
+	d2h(&K, grp + n_groups, 8);
+	// per record: its row | bases and name bytes | the call's FxSum and FxCopy's counter
+	const uint64_t o_lens = al(sizeof(FxRow) * K), o_sum = o_lens + al(16 * (K + 1));
+	char *e = (char*)X.recs.ensure(o_sum + sizeof(FxSum) + 16);
+	A.grp = grp, A.rows = (FxRow*)e, A.lens = (uint64_t*)(e + o_lens), A.sum = (FxSum*)(e + o_sum), A.next = (unsigned int*)(A.sum + 1);
+	A.n_rec = (int64_t)K;
+	dfill(A.sum, 0x7f, sizeof(FxSum)); // first_long: none
+	run_pass(FxRecs{A});
+	scan_u64(ScanCols<2>{A.lens}, A.lens, (int)K);
+	A.n = 1;
+	run_pass(FxTail{A});
+	FxSum s;
+	d2h(&s, A.sum, sizeof(s));
+	if (s.first_long < s.n_reads) return refuse("record " + std::to_string(s.first_long) + " is longer than INT32_MAX bases");
+	const int64_t bytes[MGB_DR_NTAB] = {s.n_bases, 8 * (s.n_reads + 1), s.name_bytes, 8 * (s.n_reads + 1)};
+	int64_t at = 0;
+	for (int t = 0; t < MGB_DR_NTAB; ++t) R.off[t] = at, at += (int64_t)al((uint64_t)bytes[t]);
+	char *b = (char*)alloc(alloc_ctx, (size_t)at);
+	if (b == 0) { set_error("mgb_reads_parse_dev: the allocator returned no block of " + std::to_string(at) + " bytes"); return MGB_E_INTERNAL; }
+	A.seq = b + R.off[MGB_DR_SEQ], A.name = b + R.off[MGB_DR_NAME];
+	A.off = (int64_t*)(b + R.off[MGB_DR_OFF]), A.name_off = (int64_t*)(b + R.off[MGB_DR_NAME_OFF]);
+	A.n = (int)s.n_reads;
+	run_pass(FxCopy{A});
+	h2d_async(A.off + s.n_reads, &s.n_bases, 8); // the rows of totals
+	h2d_async(A.name_off + s.n_reads, &s.name_bytes, 8);
+	dsync();
+	R.n_reads = s.n_reads, R.n_bases = s.n_bases, R.name_bytes = s.name_bytes, R.used = s.used, R.block = b, R.bytes = at;
+	return 0;
+}
+
+extern "C" int mgb_reads_parse_dev(const mg_idx_t *gi, const char *d_text, int64_t text_bytes, int64_t max_bases, int final, void *stream,
+								   mgb_dev_alloc_fn alloc, void *alloc_ctx, mgb_dev_reads_t *out)
+{
+	if (out) memset(out, 0, sizeof(*out));
+	if (gi == 0 || alloc == 0 || out == 0 || text_bytes < 0 || (text_bytes > 0 && d_text == 0)) {
+		set_error("mgb_reads_parse_dev: an index, an allocator, an mgb_dev_reads_t, and text_bytes at least 0 with the text");
+		return MGB_E_UNSUPPORTED;
+	}
+	Model *M = (Model*)gi->B;
+	std::lock_guard<std::mutex> lk(M->fx.mu);
+	mgb_dev_reads_t R;
+	memset(&R, 0, sizeof(R));
+	int rc;
+	try { rc = reads_parse(M, d_text, text_bytes, max_bases, final, stream, alloc, alloc_ctx, R); } catch (const MgbError &e) { rc = e.code; }
+	dev_bind(M->device, 0);
+	if (rc == 0) *out = R;
+	return rc;
 }
 
 extern "C" void mg_map_frag(const mg_idx_t *gi, int n_segs, const int *qlens, const char **seqs, mg_gchains_t **gcs, mg_tbuf_t *b, const mg_mapopt_t *opt, const char *qname)

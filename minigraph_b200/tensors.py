@@ -1,7 +1,8 @@
 """Reads that live in GPU memory as torch tensors, mapped without a host copy of their bases (mgb_map_batch_dev*, include/mgb200.h).
 
 A batch is two CUDA tensors: `seq`, uint8, every read's bytes one after the other (any case: they are upper-cased on the device), and
-`off`, int64, n + 1 offsets (read i is seq[off[i]:off[i+1]]).  pack_reads() builds them from host bytes for tests and tools."""
+`off`, int64, n + 1 offsets (read i is seq[off[i]:off[i+1]]).  pack_reads() builds them from host bytes for tests and tools;
+parse_cuda_fastx() and iter_cuda_fastx() build them on the GPU from FASTA/FASTQ text (mgb_reads_parse_dev)."""
 import ctypes as C
 
 from . import capi
@@ -129,3 +130,64 @@ def map_cuda_reads_to_tensors(lib, gi, seq, off, names=None, opt=None, n_seg=Non
     if rc < 0:
         raise RuntimeError("%s: %s" % (who, lib.mgb_last_error().decode())) from (failed[0] if failed else None)
     return MappedTables(got[0], rec, rec_ds)
+
+
+def parse_cuda_fastx(lib, gi, text, max_bases=0, final=True):
+    """FASTA/FASTQ text in a uint8 CUDA tensor parsed on its device by mgb_reads_parse_dev(), ordered after the work queued on the
+    current stream: returns (seq, off, names, used).  seq (uint8) and off (int64, n + 1) are views of one block that torch allocates
+    on text's device and go to map_cuda_reads() / map_cuda_reads_to_tensors() as they are; names is a list of bytes, one per read,
+    copied back to the host; used is the number of bytes of text consumed.  The records are those mgb_reads_load() gives for the
+    same bytes.  final=False: the last record is held back (it may continue past the end of text), so that text[used:] followed by
+    the next bytes of the input parses on; max_bases > 0: stop after the record that reaches it.  Raises RuntimeError with the
+    library's reason when it refuses the text."""
+    import torch
+    if text.dtype != torch.uint8 or not text.is_cuda or text.dim() != 1 or not text.is_contiguous():
+        raise ValueError("parse_cuda_fastx: text must be a contiguous 1-D torch.uint8 CUDA tensor (%s, %s)" % (text.dtype, text.device))
+    got, failed = [], []
+
+    def alloc(ctx, nbytes):
+        try:
+            got.append(torch.empty(nbytes, dtype=torch.uint8, device=text.device))
+            return got[-1].data_ptr()
+        except BaseException as e:  # a NULL block fails the call with a reason; the exception is raised from it below
+            failed.append(e)
+            return None
+
+    cb = capi.mgb_dev_alloc_fn(alloc)  # referenced until the call returns
+    dr = capi.mgb_dev_reads_t()
+    stream = torch.cuda.current_stream(text.device).cuda_stream
+    rc = lib.mgb_reads_parse_dev(gi, text.data_ptr(), text.numel(), max_bases, int(bool(final)), stream, cb, None, C.byref(dr))
+    if rc < 0:
+        raise RuntimeError("mgb_reads_parse_dev: %s" % lib.mgb_last_error().decode()) from (failed[0] if failed else None)
+    block, n = got[0], dr.n_reads
+    seq = block[dr.off[0]:dr.off[0] + dr.n_bases]
+    off = block[dr.off[1]:dr.off[1] + 8 * (n + 1)].view(torch.int64)
+    name = bytes(block[dr.off[2]:dr.off[2] + dr.name_bytes].cpu().numpy())
+    noff = block[dr.off[3]:dr.off[3] + 8 * (n + 1)].view(torch.int64).tolist()
+    return seq, off, [name[noff[i]:noff[i + 1]] for i in range(n)], dr.used
+
+
+def iter_cuda_fastx(lib, gi, path, chunk_bytes=64 << 20, max_bases=0, device=None):
+    """The reads of a FASTA/FASTQ file (plain or gzip, inflated on the host), parsed on the GPU chunk by chunk: each chunk_bytes
+    of the file is copied to the device behind the bytes the parse before left unused, and parse_cuda_fastx() runs on the
+    concatenation.  Yields (seq, off, names) batches; with max_bases > 0, batches of at most the reads that reach max_bases bases.
+    The batches hold the records of mgb_reads_load() on the whole file, in order, wherever the chunks end."""
+    import gzip
+    import torch
+    device = torch.device(device if device is not None else "cuda")
+    with open(path, "rb") as f:
+        gz = f.read(2) == b"\x1f\x8b"
+    tail = torch.empty(0, dtype=torch.uint8, device=device)
+    with (gzip.open(path, "rb") if gz else open(path, "rb")) as f:
+        final = False
+        while not final:
+            data = f.read(chunk_bytes)
+            final = len(data) == 0
+            if data:
+                tail = torch.cat([tail, torch.frombuffer(bytearray(data), dtype=torch.uint8).to(device)])
+            while True:
+                seq, off, names, used = parse_cuda_fastx(lib, gi, tail, max_bases, final)
+                tail = tail[used:]
+                if not names:
+                    break
+                yield seq, off, names
