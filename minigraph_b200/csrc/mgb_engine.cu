@@ -13,6 +13,7 @@
 #include <array>
 #include <memory>
 #include <algorithm>
+#include <numeric>
 #include <string>
 #include <chrono>
 #include <thread>
@@ -29,10 +30,11 @@
 #include "mgb_ingest.cuh"
 #include "mgb_fastx.cuh"
 #include "mgb_records.cuh"
+#include "mgb_index.cuh"
 
 #ifndef MGB_HOSTSIM
 #include <cuda_runtime.h>
-#include "mgb_index.cuh"
+#include <cub/cub.cuh>
 #endif
 
 using namespace mgb;
@@ -814,6 +816,7 @@ namespace mgb { // (the kernels of the headers' passes keep the names they had t
 MGB_PASS(   k_ingest,     IngestArgs, IngestRead,  STRIDE) // reads in device memory: their ASCII copy, words and flags (mgb_ingest.cuh)
 MGB_PASS_DS(k_rec_count,  RecArgs,    RecCount,    STRIDE) // result tables (mgb_records.cuh): count pass,
 MGB_PASS_DS(k_rec_write,  RecArgs,    RecWrite,    PULL)   // write pass
+MGB_PASS(   k_rec_rebase, RecRebase,  RecRebaseRows, STRIDE) // the CSR rows of a part joined behind others
 MGB_PASS(   k_fx_count,   FxArgs,     FxCount,     STRIDE) // FASTA/FASTQ text in device memory (mgb_fastx.cuh): list entries per chunk,
 MGB_PASS(   k_fx_lists,   FxArgs,     FxLists,     STRIDE) // the lists,
 MGB_PASS(   k_fx_succ,    FxArgs,     FxSucc,      STRIDE) // each candidate's successor,
@@ -821,6 +824,12 @@ MGB_PASS(   k_fx_jump,    FxArgs,     FxJump,      STRIDE) // a round of pointer
 MGB_PASS(   k_fx_recs,    FxArgs,     FxRecs,      STRIDE) // the records,
 MGB_PASS(   k_fx_tail,    FxArgs,     FxTail,      STRIDE) // those the call emits,
 MGB_PASS(   k_fx_copy,    FxArgs,     FxCopy,      PULL)   // their bases and names
+MGB_PASS(   k_idx_split,  IdxArgs,    IdxChunk<IdxSplit>,  STRIDE) // the minimizer table (mgb_index.cuh): records split into keys and positions,
+MGB_PASS(   k_idx_flag,   IdxArgs,    IdxChunk<IdxFlag>,   STRIDE) // after the sorts, the first record of each minimizer flagged,
+MGB_PASS(   k_idx_starts, IdxArgs,    IdxChunk<IdxStarts>, STRIDE) // after the scan, where each run starts,
+MGB_PASS(   k_idx_counts, IdxArgs,    IdxChunk<IdxCounts>, STRIDE) // its length,
+MGB_PASS(   k_idx_lists,  IdxArgs,    IdxChunk<IdxLists>,  STRIDE) // after the scan, the occurrence lists,
+MGB_PASS(   k_idx_insert, IdxArgs,    IdxChunk<IdxInsert>, STRIDE) // the slots
 }
 
 // ---- block scan ----
@@ -965,12 +974,11 @@ struct Model {
 	std::vector<char> seq;
 	std::vector<uint64_t> arc_idx;
 	std::vector<DevArc> arc;
-	std::vector<u128> slot;
+	std::vector<u128> slot;         // the table and the occurrence lists, copied from the device when mg_idx_get() is first called
 	std::vector<uint64_t> pos;
-	std::vector<uint32_t> occ;      // occurrences per distinct minimizer (for the quantiles)
 	uint64_t n_slots_mask;
 	int k, w;
-	uint32_t *d_occ_sorted = 0; uint64_t n_keys = 0, n_pos = 0; // device-built index: ascending occurrence counts; host copies of slot/pos are made on demand
+	uint32_t *d_occ_sorted = 0; uint64_t n_keys = 0, n_pos = 0; // ascending occurrence counts per distinct minimizer (for the quantiles)
 	std::mutex host_ix_mutex;
 	// device image
 	GraphDev g;
@@ -1101,9 +1109,104 @@ static void slot_prepare(Model *M, Model::Slot &sl, int n_workers)
 	dev_bind(M->device, sl.stream);
 }
 
-static Model *model_build(gfa_t *g, int k, int w)
+// ---- the sorts and sums of the index build: CUB's on the device, the standard library's in the simulators ----
+// sort_pairs_u64: the n pairs (k[i], v[i]) sorted stably by bits [0, bits) of the key (the other bits travel along); kb and vb are
+// scratch of n elements.  The sorted pairs end up in one buffer of each pair, and k and v are left pointing at them.
+// prefix_sum_u32: out[i] = in[0] + ... + in[i] (inclusive) or + in[i - 1] (exclusive), modulo 2^32.
+// sort_u32: out = in[0 .. n) in ascending order.
+#ifndef MGB_HOSTSIM
+static void sort_pairs_u64(uint64_t *&k, uint64_t *&kb, uint64_t *&v, uint64_t *&vb, int n, int bits)
 {
-	Model *M = new Model();
+	cub::DoubleBuffer<uint64_t> K(k, kb), V(v, vb);
+	size_t bytes = 0;
+	CUDA_OK(cub::DeviceRadixSort::SortPairs(0, bytes, K, V, n, 0, bits, t_stream));
+	DevBuf<char> tmp(bytes);
+	CUDA_OK(cub::DeviceRadixSort::SortPairs(tmp, bytes, K, V, n, 0, bits, t_stream));
+	k = K.Current(), kb = K.Alternate(), v = V.Current(), vb = V.Alternate();
+}
+static void prefix_sum_u32(uint32_t *in, uint32_t *out, int n, bool inclusive)
+{
+	size_t bytes = 0;
+	if (inclusive) CUDA_OK(cub::DeviceScan::InclusiveSum(0, bytes, in, out, n, t_stream));
+	else CUDA_OK(cub::DeviceScan::ExclusiveSum(0, bytes, in, out, n, t_stream));
+	DevBuf<char> tmp(bytes);
+	if (inclusive) CUDA_OK(cub::DeviceScan::InclusiveSum(tmp, bytes, in, out, n, t_stream));
+	else CUDA_OK(cub::DeviceScan::ExclusiveSum(tmp, bytes, in, out, n, t_stream));
+}
+static void sort_u32(const uint32_t *in, uint32_t *out, int n)
+{
+	size_t bytes = 0;
+	CUDA_OK(cub::DeviceRadixSort::SortKeys(0, bytes, in, out, n, 0, 32, t_stream));
+	DevBuf<char> tmp(bytes);
+	CUDA_OK(cub::DeviceRadixSort::SortKeys(tmp, bytes, in, out, n, 0, 32, t_stream));
+}
+#else
+static void sort_pairs_u64(uint64_t *&k, uint64_t *&, uint64_t *&v, uint64_t *&, int n, int bits)
+{
+	const uint64_t m = bits < 64? (1ULL << bits) - 1 : ~0ULL;
+	std::vector<std::pair<uint64_t, uint64_t>> p((size_t)n);
+	for (int i = 0; i < n; ++i) p[i] = {k[i], v[i]};
+	std::stable_sort(p.begin(), p.end(), [m](const std::pair<uint64_t, uint64_t> &a, const std::pair<uint64_t, uint64_t> &b) { return (a.first & m) < (b.first & m); });
+	for (int i = 0; i < n; ++i) k[i] = p[i].first, v[i] = p[i].second;
+}
+static void prefix_sum_u32(uint32_t *in, uint32_t *out, int n, bool inclusive)
+{
+	if (inclusive) std::partial_sum(in, in + n, out);
+	else if (n > 0) out[0] = 0, std::partial_sum(in, in + n - 1, out + 1);
+}
+static void sort_u32(const uint32_t *in, uint32_t *out, int n) { std::copy(in, in + n, out), std::sort(out, out + n); }
+#endif
+
+// The minimizer table of M (mgb_index.cuh) from the n records of the segment sketch in mz: order them by (minimizer, position),
+// group them into runs, lay out the lists and insert the slots, then sort the run lengths for the quantiles.  The table, the lists
+// and the sorted counts go to M as soon as they exist, which frees them.
+static void build_index(Model *M, const u128 *mz, uint64_t n)
+{
+	IdxArgs A;
+	memset(&A, 0, sizeof(A));
+	DevBuf<uint64_t> key0(n), key1(n), val0(n), val1(n);
+	DevBuf<uint32_t> flag(n), rank(n);
+	uint64_t *key = key0, *key_b = key1, *val = val0, *val_b = val1;
+	const int n_chunks = (int)((n + 31) / 32);
+	A.mz = mz, A.n_mz = n, A.key = key, A.val = val, A.n = n_chunks;
+	run_pass(IdxChunk<IdxSplit>{A});
+	sort_pairs_u64(val, val_b, key, key_b, (int)n, 64); // by position, then stably by minimizer (2k bits)
+	sort_pairs_u64(key, key_b, val, val_b, (int)n, std::min(2 * M->k, 64));
+	A.key = key, A.val = val, A.flag = flag, A.rank = rank;
+	run_pass(IdxChunk<IdxFlag>{A});
+	prefix_sum_u32(flag, rank, (int)n, true);
+	uint32_t n_keys = 0;
+	if (n) d2h(&n_keys, rank + (n - 1), 4);
+	DevBuf<uint32_t> start(n_keys), cnt(n_keys), multi(n_keys), pos_off(n_keys);
+	A.n_keys = n_keys, A.start = start, A.cnt = cnt, A.multi = multi, A.pos_off = pos_off;
+	run_pass(IdxChunk<IdxStarts>{A});
+	const int n_key_chunks = (int)((n_keys + 31) / 32);
+	A.n = n_key_chunks;
+	run_pass(IdxChunk<IdxCounts>{A});
+	prefix_sum_u32(multi, pos_off, (int)n_keys, false);
+	uint32_t last_off = 0, last_multi = 0;
+	if (n_keys) d2h_async(&last_off, pos_off + (n_keys - 1), 4), d2h(&last_multi, multi + (n_keys - 1), 4);
+	uint64_t n_slots = 16;
+	while (n_slots < (uint64_t)n_keys * 2) n_slots <<= 1;
+	M->n_keys = n_keys, M->n_pos = (uint64_t)last_off + last_multi, M->n_slots_mask = M->ix.n_slots_mask = n_slots - 1;
+	A.slot = (u128*)dmalloc(n_slots * sizeof(u128)), M->dev_ptrs.push_back(A.slot), M->ix.slot = A.slot;
+	A.pos = (uint64_t*)dmalloc(M->n_pos * 8), M->dev_ptrs.push_back(A.pos), M->ix.pos = A.pos;
+	M->d_occ_sorted = (uint32_t*)dmalloc((size_t)n_keys * 4);
+	A.mask = n_slots - 1;
+	dfill(A.slot, 0xff, n_slots * sizeof(u128));
+	A.n = n_chunks;
+	run_pass(IdxChunk<IdxLists>{A});
+	A.n = n_key_chunks;
+	run_pass(IdxChunk<IdxInsert>{A});
+	sort_u32(cnt, M->d_occ_sorted, (int)n_keys);
+	dsync();
+}
+
+// M's graph, uploaded, and its minimizer table, built on `device`.  A failure throws MgbError with nothing left allocated.
+static Model *model_build(gfa_t *g, int k, int w, int device)
+{
+	std::unique_ptr<Model, void (*)(Model*)> M(new Model(), model_free);
+	M->device = device;
 	M->k = k, M->w = w, M->d_logf = 0, M->n_logf = 0, M->es = 0;
 	memset(&M->W, 0, sizeof(Workers)), memset(&M->Wbig, 0, sizeof(Workers));
 	memset(&M->stats, 0, sizeof(M->stats));
@@ -1168,99 +1271,44 @@ static Model *model_build(gfa_t *g, int k, int w)
 		M->gafg.seg_len = M->g.seg_len;
 	}
 
-	// sketch every segment on the device (K1 reused), then build the table: on the device (the simulators: on the host)
-#ifdef MGB_HOSTSIM
-	std::vector<u128> mz;
-#endif
-	{
-		uint64_t tot_len = 0;
-		int32_t max_len = 1;
-		for (uint32_t i = 0; i < n_seg; ++i) { tot_len += (uint64_t)g->seg[i].len; if (g->seg[i].len > max_len) max_len = g->seg[i].len; }
-		uint64_t cap = (tot_len / 2 + 64 * (uint64_t)n_seg + 1024) * sizeof(u128);
-		// a worker sketches one whole segment inside its arena: ~ (len/w + growth slack) records
-		uint64_t need = (uint64_t)max_len * 16 + ((uint64_t)1 << 20);
-		uint64_t arena_b = std::max<uint64_t>((uint64_t)p_arena_mb << 20, need);
-		int nw = default_workers();
-		while (nw > 1 && (uint64_t)nw * arena_b > dev_free_mem() / 2) nw /= 2;
-		for (;;) {
-			ensure_workers(M->W, nw, arena_b);
-			Pool hp; hp.used = 0, hp.cap = cap;
-			Pool *d_pool = (Pool*)dmalloc(sizeof(Pool));
-			u128 *d_mz = (u128*)dmalloc(cap);
-			int *d_status = (int*)dmalloc(sizeof(int));
-			unsigned int *d_next = (unsigned int*)dmalloc(sizeof(unsigned int));
-			int st0 = 0;
-			h2d(d_pool, &hp, sizeof(Pool));
-			h2d(d_status, &st0, sizeof(int));
-			LaunchArgs L;
-			memset(&L, 0, sizeof(L));
-			L.c.g = M->g, L.c.ix = M->ix, L.c.next_read = d_next;
-			L.routs = (ReadOut*)d_status, L.rid_list = 0, L.n_work = (int32_t)n_seg, L.pool_mz = d_pool, L.mz = d_mz;
-			launch_stage<S_INDEX_SKETCH>(L, M->W);
-			dsync();
-			d2h(&st0, d_status, sizeof(int));
-			d2h(&hp, d_pool, sizeof(Pool));
-			bool retry = false;
-			if (st0 == MGB_E_POOL) cap *= 2, retry = true;
-			else if (st0 == MGB_E_ARENA) arena_b *= 2, nw = std::max(1, nw / 2), retry = true;
-			else if (st0 < 0) { set_error("segment sketch failed with code " + std::to_string(st0)); throw MgbError{st0}; }
-#ifndef MGB_HOSTSIM
-			if (!retry) { // group, lay out and insert on the device (mgb_index.cuh)
-				DevIndexOut out;
-				dfree(M->W.arena), dfree(M->W.peak); // the sketch arenas are not needed again; the sort wants the memory
-				memset(&M->W, 0, sizeof(Workers));
-				cudaError_t e = build_index_device(d_mz, hp.used / sizeof(u128), 2 * k, t_stream, &out);
-				dfree(d_pool), dfree(d_mz), dfree(d_status), dfree(d_next);
-				if (e != cudaSuccess) { set_error(std::string("index build on the device: ") + cudaGetErrorString(e)); throw MgbError{MGB_E_INTERNAL}; }
-				M->n_slots_mask = out.n_slots - 1, M->n_keys = out.n_keys, M->n_pos = out.n_pos, M->d_occ_sorted = out.occ_sorted;
-				M->ix.n_slots_mask = M->n_slots_mask, M->ix.slot = out.slot, M->ix.pos = out.pos;
-				M->dev_ptrs.push_back((void*)out.slot), M->dev_ptrs.push_back((void*)out.pos);
-				return M;
-			}
-#else
-			if (!retry) {
-				mz.resize(hp.used / sizeof(u128));
-				d2h(mz.data(), d_mz, hp.used);
-			}
-#endif
-			dfree(d_pool), dfree(d_mz), dfree(d_status), dfree(d_next);
-			if (!retry) break;
+	// sketch every segment on the device (K1 reused), then build the table
+	uint64_t tot_len = 0;
+	int32_t max_len = 1;
+	for (uint32_t i = 0; i < n_seg; ++i) { tot_len += (uint64_t)g->seg[i].len; if (g->seg[i].len > max_len) max_len = g->seg[i].len; }
+	uint64_t cap = tot_len / 2 + 64 * (uint64_t)n_seg + 1024; // records
+	// a worker sketches one whole segment inside its arena: ~ (len/w + growth slack) records
+	uint64_t need = (uint64_t)max_len * 16 + ((uint64_t)1 << 20);
+	uint64_t arena_b = std::max<uint64_t>((uint64_t)p_arena_mb << 20, need);
+	int nw = default_workers();
+	while (nw > 1 && (uint64_t)nw * arena_b > dev_free_mem() / 2) nw /= 2;
+	for (;;) {
+		ensure_workers(M->W, nw, arena_b);
+		Pool hp; hp.used = 0, hp.cap = cap * sizeof(u128);
+		DevBuf<Pool> d_pool(1);
+		DevBuf<u128> d_mz(cap);
+		DevBuf<int> d_status(1);
+		DevBuf<unsigned int> d_next(1);
+		int st0 = 0;
+		h2d(d_pool, &hp, sizeof(Pool));
+		h2d(d_status, &st0, sizeof(int));
+		LaunchArgs L;
+		memset(&L, 0, sizeof(L));
+		L.c.g = M->g, L.c.ix = M->ix, L.c.next_read = d_next;
+		L.routs = (ReadOut*)d_status.p, L.rid_list = 0, L.n_work = (int32_t)n_seg, L.pool_mz = d_pool, L.mz = d_mz;
+		launch_stage<S_INDEX_SKETCH>(L, M->W);
+		dsync();
+		d2h(&st0, d_status, sizeof(int));
+		d2h(&hp, d_pool, sizeof(Pool));
+		if (st0 == MGB_E_POOL) cap *= 2;
+		else if (st0 == MGB_E_ARENA) arena_b *= 2, nw = std::max(1, nw / 2);
+		else if (st0 < 0) { set_error("segment sketch failed with code " + std::to_string(st0)); throw MgbError{st0}; }
+		else {
+			dfree(M->W.arena), dfree(M->W.peak); // the sketch arenas are not needed again (every mapping slot owns its arenas); the sort wants the memory
+			memset(&M->W, 0, sizeof(Workers));
+			build_index(M.get(), d_mz, hp.used / sizeof(u128));
+			return M.release();
 		}
 	}
-#ifdef MGB_HOSTSIM
-	// the sketch arenas are not needed again (every mapping slot owns its arenas)
-	dfree(M->W.arena), dfree(M->W.peak);
-	memset(&M->W, 0, sizeof(Workers));
-	// group by minimizer; occurrence lists ascending (reference: index.c:115-165 mg_idx_a2h)
-	std::sort(mz.begin(), mz.end(), [](const u128 &a, const u128 &b) { return (a.x >> 8) != (b.x >> 8)? (a.x >> 8) < (b.x >> 8) : a.y < b.y; });
-	size_t n_keys = 0;
-	for (size_t i = 0; i < mz.size(); ++i) if (i == 0 || (mz[i].x >> 8) != (mz[i-1].x >> 8)) ++n_keys;
-	uint64_t n_slots = 16;
-	while (n_slots < n_keys * 2) n_slots <<= 1;
-	M->n_slots_mask = n_slots - 1;
-	M->slot.assign(n_slots, u128{~0ULL, ~0ULL});
-	M->occ.reserve(n_keys);
-	for (size_t i = 0; i < mz.size();) {
-		size_t j = i;
-		uint64_t key = mz[i].x >> 8;
-		while (j < mz.size() && (mz[j].x >> 8) == key) ++j;
-		uint64_t h = idx_slot_hash(key) & M->n_slots_mask;
-		while (M->slot[h].x != ~0ULL) h = (h + 1) & M->n_slots_mask;
-		if (j - i == 1) {
-			M->slot[h].x = key << 1 | 1, M->slot[h].y = mz[i].y;
-			M->occ.push_back(1);
-		} else {
-			M->slot[h].x = key << 1, M->slot[h].y = (uint64_t)M->pos.size() << 32 | (uint64_t)(j - i);
-			for (size_t t = i; t < j; ++t) M->pos.push_back(mz[t].y);
-			M->occ.push_back((uint32_t)(j - i));
-		}
-		i = j;
-	}
-	M->ix.n_slots_mask = M->n_slots_mask;
-	M->ix.slot = upload(M->slot.data(), M->slot.size()).release(), M->dev_ptrs.push_back((void*)M->ix.slot);
-	M->ix.pos = upload(M->pos.data(), M->pos.size()).release(), M->dev_ptrs.push_back((void*)M->ix.pos);
-#endif
-	return M;
 }
 
 static const Model *model_of(const mg_idx_t *gi) { return (const Model*)gi->B; }
@@ -1269,51 +1317,40 @@ static const Model *model_of(const mg_idx_t *gi) { return (const Model*)gi->B; }
 // C ABI: index
 // ---------------------------------------------------------------------------------------------------------------
 
+// the occurrence counts at the quantiles f[] (0 where the copy from the device fails: the reason is in mgb_last_error())
 extern "C" void mg_idx_cal_quantile(const mg_idx_t *gi, int32_t m, float f[], int32_t q[])
 {
 	const Model *M = model_of(gi);
-#ifndef MGB_HOSTSIM
-	if (M->d_occ_sorted) { // the table was built on the device: the counts are there, sorted
-		const uint64_t n = M->n_keys;
-		for (int32_t i = 0; i < m; ++i) {
+	const uint64_t n = M->n_keys;
+	for (int32_t i = 0; i < m; ++i) q[i] = 0;
+	try {
+		dev_bind(M->device, 0);
+		for (int32_t i = 0; i < m && n > 0; ++i) {
 			size_t kk = (size_t)((1.0 - (double)f[i]) * (double)n);
-			if (n == 0) { q[i] = 0; continue; }
 			if (kk >= n) kk = n - 1;
 			uint32_t v = 0;
-			cudaSetDevice(M->device);
-			cudaMemcpy(&v, M->d_occ_sorted + kk, 4, cudaMemcpyDeviceToHost);
+			d2h(&v, M->d_occ_sorted + kk, 4);
 			q[i] = (int32_t)v;
 		}
-		return;
-	}
-#endif
-	std::vector<uint32_t> a(M->occ);
-	uint64_t n = a.size();
-	for (int32_t i = 0; i < m; ++i) {
-		size_t kk = (size_t)((1.0 - (double)f[i]) * (double)n);
-		if (n == 0) { q[i] = 0; continue; }
-		if (kk >= n) kk = n - 1;
-		std::nth_element(a.begin(), a.begin() + kk, a.end());
-		q[i] = (int32_t)a[kk];
-	}
+	} catch (const MgbError &) {}
 }
 
 extern "C" const uint64_t *mg_idx_get(const mg_idx_t *gi, uint64_t minier, int *n)
 {
 	Model *M = (Model*)model_of(gi);
-#ifndef MGB_HOSTSIM
-	if (M->slot.empty() && M->ix.slot) { // device-built table: the host view is fetched the first time somebody asks for it
+	if (M->slot.empty()) { // the host view of the table is fetched the first time somebody asks for it
 		std::lock_guard<std::mutex> lk(M->host_ix_mutex);
 		if (M->slot.empty()) {
-			cudaSetDevice(M->device);
-			M->pos.resize(M->n_pos? M->n_pos : 1);
-			cudaMemcpy(M->pos.data(), M->ix.pos, M->n_pos * 8, cudaMemcpyDeviceToHost);
-			std::vector<u128> sl(M->n_slots_mask + 1);
-			cudaMemcpy(sl.data(), M->ix.slot, sl.size() * sizeof(u128), cudaMemcpyDeviceToHost);
-			M->slot.swap(sl);
+			try {
+				dev_bind(M->device, 0);
+				std::vector<uint64_t> pos(M->n_pos? M->n_pos : 1);
+				std::vector<u128> sl(M->n_slots_mask + 1);
+				d2h(pos.data(), M->ix.pos, M->n_pos * 8);
+				d2h(sl.data(), M->ix.slot, sl.size() * sizeof(u128));
+				M->pos.swap(pos), M->slot.swap(sl);
+			} catch (const MgbError &) { *n = 0; return 0; } // (the reason is in mgb_last_error())
 		}
 	}
-#endif
 	IndexDev ix;
 	ix.k = M->k, ix.w = M->w, ix.n_slots_mask = M->n_slots_mask, ix.slot = M->slot.data(), ix.pos = M->pos.data();
 	return idx_get(ix, minier, n);
@@ -1353,13 +1390,12 @@ extern "C" mg_idx_t *mg_index(gfa_t *g, const mg_idxopt_t *io, int n_threads, mg
 	if (k * 2 < b) b = k * 2;
 	if (w < 1) w = 1;
 	Model *M = 0;
-	try { M = model_build(g, k, w); } catch (const MgbError &) { return 0; }
-	M->device = devs[0];
+	try { M = model_build(g, k, w, devs[0]); } catch (const MgbError &) { return 0; }
 	if (devs.size() > 1) { // every further device builds its own copy, all at once
 		M->peers.resize(devs.size() - 1, (Model*)0);
 		std::vector<std::thread> th;
 		for (size_t i = 1; i < devs.size(); ++i)
-			th.emplace_back([&, i]() { try { if (dev_ok(devs[i])) { M->peers[i - 1] = model_build(g, k, w); M->peers[i - 1]->device = devs[i]; } } catch (const MgbError &) {} });
+			th.emplace_back([&, i]() { try { if (dev_ok(devs[i])) M->peers[i - 1] = model_build(g, k, w, devs[i]); } catch (const MgbError &) {} });
 		for (auto &t : th) t.join();
 		dev_ok(devs[0]);
 		for (Model *P : M->peers) if (P == 0) { model_free(M); return 0; } // mgb_last_error() has the reason
@@ -1955,14 +1991,6 @@ static void rec_totals(const mgb_records_t &R, const mgb_records_ds_t *x)
 	dsync();
 }
 
-#ifndef MGB_HOSTSIM
-namespace mgb { // (named as in mgb_records.cuh, which holds its row function)
-__global__ void __launch_bounds__(256) k_rec_rebase(RecRebase B)
-{
-	for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < B.n; i += (int64_t)gridDim.x * blockDim.x) rec_rebase_row(B, i);
-}
-}
-#endif
 // The tables of the parts (each in its own block on its device) joined in input order into R's block on M's device: every table
 // copied behind those of the parts before, the CSR rows raised by the rows before, the totals written last.  On the caller's stream.
 int RecSink::join(Model *M)
@@ -1972,9 +2000,7 @@ int RecSink::join(Model *M)
 		R.n_seq += p->R.n_seq, R.n_rec += p->R.n_rec, R.n_lc += p->R.n_lc, R.n_a += p->R.n_a, R.n_cigar += p->R.n_cigar;
 		X.n_ds += p->X.n_ds, X.n_ds_off += p->X.n_ds_off;
 	}
-#ifndef MGB_HOSTSIM
-	dev_bind(M->device, (cudaStream_t)stream);
-#endif
+	dev_bind(M->device, (DevStream)(uintptr_t)stream);
 	if (!block()) return MGB_E_INTERNAL;
 	// the tables of R, then those of X
 	enum { SEQ, REC, LC, A, CIG, DS, DSO, N_KIND };
@@ -1991,17 +2017,13 @@ int RecSink::join(Model *M)
 		if (p.block)
 			for (int t = 0; t < n_tab; ++t)
 				d2d_peer(b + off(R, X, t) + at[kind[t]] * row_bytes[t], M->device, (const char*)p.block + off(p, px, t), parts[d]->device, (size_t)(rows[kind[t]] * row_bytes[t]));
-		const RecRebase rb[3] = {{(int64_t*)(b + R.off[MGB_REC_SEQ_CSR]) + 3 * at[SEQ], p.n_seq, 3, {at[REC], at[LC], at[A]}},
-								 {(int64_t*)(b + R.off[MGB_REC_CIGAR_CSR]) + at[REC], p.n_rec, 1, {at[CIG], 0, 0}},
-								 {(int64_t*)(b + X.off[MGB_REC_DS_CSR]) + 2 * at[REC], with_ds? p.n_rec : 0, 2, {at[DS], at[DSO], 0}}};
-		for (const RecRebase &B : rb) {
-			if (B.n == 0 || (B.base[0] == 0 && B.base[1] == 0 && B.base[2] == 0)) continue;
-#ifndef MGB_HOSTSIM
-			k_rec_rebase<<<(int)std::min<int64_t>((B.n + 255) / 256, dev_sm_count() * 8), 256, 0, t_stream>>>(B);
-			CUDA_OK(cudaGetLastError());
-#else
-			for (int64_t i = 0; i < B.n; ++i) rec_rebase_row(B, i);
-#endif
+		RecRebase rb[3] = {{(int64_t*)(b + R.off[MGB_REC_SEQ_CSR]) + 3 * at[SEQ], p.n_seq, 3, {at[REC], at[LC], at[A]}},
+						   {(int64_t*)(b + R.off[MGB_REC_CIGAR_CSR]) + at[REC], p.n_rec, 1, {at[CIG], 0, 0}},
+						   {(int64_t*)(b + X.off[MGB_REC_DS_CSR]) + 2 * at[REC], with_ds? p.n_rec : 0, 2, {at[DS], at[DSO], 0}}};
+		for (RecRebase &B : rb) {
+			if (B.rows == 0 || (B.base[0] == 0 && B.base[1] == 0 && B.base[2] == 0)) continue;
+			B.n = (int)((B.rows + 31) / 32);
+			run_pass(RecRebaseRows{B});
 		}
 		for (int k = 0; k < N_KIND; ++k) at[k] += rows[k];
 	}

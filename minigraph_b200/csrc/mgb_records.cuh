@@ -162,12 +162,22 @@ struct RecWrite {
 	}
 };
 
-// rows [0, n) of a table of w int64 columns, column j raised by base[j] (the CSR tables of a part joined behind others)
-struct RecRebase { int64_t *v; int64_t n; int w; int64_t base[3]; };
+// rows [0, rows) of a table of w int64 columns, column j raised by base[j] (the CSR tables of a part joined behind others), in n
+// items of 32 rows
+struct RecRebase { int64_t *v; int64_t rows; int w; int64_t base[3]; int n; };
 MG_HD inline void rec_rebase_row(const RecRebase &B, int64_t i)
 {
 	for (int j = 0; j < 3; ++j) // (constant indices: base stays in registers)
 		if (j < B.w) B.v[i * B.w + j] += B.base[j];
 }
+// item c: rows 32 c .. 32 c + 31, the lanes striding through them by MGB_W (one row per thread on the device)
+struct RecRebaseRows {
+	const RecRebase &a;
+	MG_HD int operator()(int c, int lane) const
+	{
+		for (int j = lane; j < 32; j += MGB_W) { const int64_t i = 32 * (int64_t)c + j; if (i < a.rows) rec_rebase_row(a, i); }
+		return 0;
+	}
+};
 
 } // namespace mgb

@@ -551,9 +551,9 @@ def case_concurrent_calls(lib, workdir, n_threads=3, n_reads=90):
 
 
 def case_index_big(lib, workdir, graph_len=50000000, n_probe=40000):
-    """the minimizer table of a graph whose index does not fit L2 (built on the device, mgb_index.cuh; in the simulators on the
-    host) against the reference's (index.c:115-165): the same occurrence list -- content and order -- for tens of thousands of
-    probed minimizers and for keys that are not there, and the same quantile-derived mapping options (options.c:120-134)"""
+    """the minimizer table of a graph whose index does not fit L2 (built by the passes of mgb_index.cuh, on the device or in the
+    simulators) against the reference's (index.c:115-165): the same occurrence list -- content and order -- for tens of thousands
+    of probed minimizers and for keys that are not there, and the same quantile-derived mapping options (options.c:120-134)"""
     import ctypes as C
     import random
     from minigraph_b200 import options

@@ -95,3 +95,7 @@ def test_bridging_alignment(lib, workdir):
 
 def test_rmq_chaining_with_interleaved_diagonals(lib, workdir):
     cases.case_tandem_diagonals(lib, workdir)
+
+
+def test_index_vs_reference_lists(lib, workdir):
+    cases.case_index_big(lib, workdir, graph_len=2000000, n_probe=5000)

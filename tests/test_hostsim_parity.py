@@ -65,7 +65,7 @@ def test_upload_modes_chosen_per_batch(lib, workdir):
 
 
 @pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not built")
-def test_host_index_vs_reference_lists(lib, workdir):
+def test_index_vs_reference_lists(lib, workdir):
     cases.case_index_big(lib, workdir, graph_len=2000000, n_probe=5000)
 
 
